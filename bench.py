@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — SDXL UNet conditioned-forward passes/sec (rank-4 LoRA, 1024 px) on 1..8 B200s.
+"""bench.py — SDXL UNet conditioned-forward passes/sec (rank-4 LoRA, 1024 px) on 1..8 H100s.
 
 Workload (BASELINE.json metric; SURVEY.md §8d): SDXL-base UNet, synthetic seeded weights (no checkpoint is reachable
 offline), rank-4 alpha-1 LoRA on the `noxattn` + `c3lier` leaf set (346 adaptors, lora_up != 0, multiplier 1), latents
@@ -16,15 +16,17 @@ One *step* = one UNet forward over B conditioned passes per GPU (B = 8: the refe
             re-captured per kernel class (gemm_kernel = every Linear / conv; attention; norms; the rest) as graphs of
             their own on the same buffers; each class graph is replayed and timed with CUDA events like the forward.
             achieved = algorithmic FLOPs of the gemm_kernel launches / their time; peak = MEASURED_PEAKS.json
-            bf16_tflops_sustained.  (Round 1 bracketed eager launches with events, which counted host launch jitter.)
+            bf16_tflops_sustained where present, else the H100 SXM data-sheet dense bf16 rate (989 TFLOP/s at 700 W).
   configs   the other BASELINE.json configurations (extra keys, the headline is unchanged): SD-1.5 bf16 at
             B in {1, 2, 8} (config 2), the sharded text-slider iteration (config 3, `train`), the rank-8 image-slider
             step (config 4), a bounded sample of the 50-step x 11-scale x batch-16 inference sweep (config 5) and, on the
             host cores, one SD-1.5 text-slider iteration in fp32 (config 1).
   cpu_baseline  the reference's CPU path for the headline workload on the host cores (rank 0, N = 1), bounded sample.
-`--impl reference`: times that CPU path alone — the reference's unmodified `train_util.predict_noise_xl` + `lora.py`
-hook on the fp32 oracle UNet where /root/reference exists (kind "reference"), else the port of the same code in
-oracle/port.py (kind "port"; the GPU box has no /root/reference and diffusers is not installable anywhere here).
+`--impl reference`: times that CPU path alone — oracle/port.py (the port of the reference's `train_util.predict_noise_xl`
++ `lora.py` hook, pinned against the reference in tests/test_oracle.py) on the fp32 oracle UNet (kind "port").
+`--dump-outputs DIR`: after the timed steps, writes what the timed paths computed in their last step as float32 .npy
+files: unet_sample.npy (the whole-forward graph's eps, [B, 4, 128, 128]) and e2e_eps.npy (the guided eps the public
+call returned, [B / 2, 4, 128, 128]).  Inputs and weights are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -85,7 +87,8 @@ def load_peaks():
             p = json.load(f)
         return {"sustained": float(p["bf16_tflops_sustained"]), "burst": float(p["bf16_tflops"]),
                 "hbm": float(p["hbm_gbs"]), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"sustained": 1400.0, "burst": 1590.0, "hbm": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"sustained": 989.0, "burst": 989.0, "hbm": 3350.0,
+            "source": "H100 SXM data sheet, dense bf16 at 700 W (not a measured rate)"}
 
 
 class ClockSampler:
@@ -140,9 +143,23 @@ class ClockSampler:
                 "samples": len(sm)}
 
 
+def gpu_identity(index: int):
+    """The card a number was measured on: its name and the power limit it runs under (a card set below 700 W clocks
+    lower under sustained load)."""
+    ident = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        ident["power_limit_w"] = float(out.splitlines()[0])
+    except (OSError, ValueError, IndexError, subprocess.TimeoutExpired):
+        pass
+    return ident
+
+
 # ----------------------------------------------------------------------------------------------------
 def build_product(dev, arch="sdxl", rank=4, seed=0, share=None):
-    """UNet (seeded synthetic weights, or the parameters of `share`) + LoRANetwork(noxattn, c3lier) with lora_up != 0."""
+    """UNet (seeded synthetic weights, or the parameters of `share`) + LoRANetwork(noxattn, c3lier) with seeded adaptor
+    weights, lora_up != 0."""
     from sliders_b200 import lora as plora
     from sliders_b200 import synthetic
     from sliders_b200.unet import UNet2DConditionModel, UNetConfig
@@ -164,7 +181,9 @@ def build_product(dev, arch="sdxl", rank=4, seed=0, share=None):
         net = plora.LoRANetwork(unet, rank=rank, multiplier=1.0, alpha=1.0, train_method="noxattn").to(dev, torch.bfloat16)
     finally:
         del plora.DEFAULT_TARGET_REPLACE[len(saved):]
-    synthetic.init_lora_nonzero_(net, seed=seed + 2, up_std=0.02)
+    # lora_down is redrawn per key from the seed as well (same variance, 1 / fan_in, as LoRAModule's kaiming init, which
+    # draws from the global RNG): the adaptors, and so every output, are identical from run to run
+    synthetic.init_lora_nonzero_(net, seed=seed + 2, up_std=0.02, reseed_down=True)
     return unet, net
 
 
@@ -234,8 +253,9 @@ def class_timings(unet, call, steps, warmup):
 # ---------------------------------------------------------------------------------------------------- CPU legs
 def cpu_pair_call(arch="sdxl", rank=4, seed=0, lora_state=None, unet_state=None):
     """The reference's CPU path for one CFG-pair call of the headline workload: `predict_noise_xl` with the LoRA hook
-    live on the fp32 oracle UNet.  Returns (callable -> eps, kind, description)."""
-    from oracle import reference_bridge as rb
+    live on the fp32 oracle UNet, through oracle/port.py.  Returns (callable -> eps, kind, description)."""
+    from oracle import ddim as oddim
+    from oracle import port
     from oracle import unet as ounet
     from sliders_b200 import synthetic
 
@@ -252,29 +272,13 @@ def cpu_pair_call(arch="sdxl", rank=4, seed=0, lora_state=None, unet_state=None)
                             for k, p in om.named_parameters()}, assign=True)
     om.requires_grad_(False)
     om.eval()
-    if rb.available():
-        lora, tu, mu = rb.load("lora"), rb.load("train_util"), rb.load("model_util")
-        saved = list(lora.DEFAULT_TARGET_REPLACE)
-        lora.DEFAULT_TARGET_REPLACE += lora.UNET_TARGET_REPLACE_MODULE_CONV
-        try:
-            net = lora.LoRANetwork(om, rank=rank, multiplier=1.0, alpha=1.0, train_method="noxattn")
-        finally:
-            del lora.DEFAULT_TARGET_REPLACE[len(saved):]
-        sched = mu.create_noise_scheduler("ddim")
-        predict_xl, predict, kind = tu.predict_noise_xl, tu.predict_noise, "reference"
-        what = ("the reference's unmodified trainscripts/textsliders/train_util.py + lora.py (LoRA hook live) on the fp32 "
-                "oracle UNet (oracle/unet.py = diffusers 0.20.2 restated; diffusers itself is not installable)")
-    else:
-        from oracle import ddim as oddim
-        from oracle import port
-
-        net = port.LoRAHooks(om, rank=rank, alpha=1.0, c3lier=True)
-        sched = oddim.DDIMScheduler(beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
-                                    num_train_timesteps=1000, clip_sample=False)
-        predict_xl, predict, kind = port.predict_noise_xl, port.predict_noise, "port"
-        what = ("oracle/port.py (port of the reference's train_util.py + lora.py hook, pinned against them in "
-                "tests/test_oracle.py) on the fp32 oracle UNet; /root/reference is absent on this box")
-    synthetic.init_lora_nonzero_(net, seed=seed + 2, up_std=0.02)
+    net = port.LoRAHooks(om, rank=rank, alpha=1.0, c3lier=True)
+    sched = oddim.DDIMScheduler(beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
+                                num_train_timesteps=1000, clip_sample=False)
+    predict_xl, predict, kind = port.predict_noise_xl, port.predict_noise, "port"
+    what = ("oracle/port.py (port of the reference's train_util.py + lora.py hook, pinned against them in "
+            "tests/test_oracle.py) on the fp32 oracle UNet")
+    synthetic.init_lora_nonzero_(net, seed=seed + 2, up_std=0.02, reseed_down=True)
     if lora_state is not None:   # the kernel path's adaptor weights, so that the two runs compute the same function
         own = net.state_dict()
         net.load_state_dict({k: lora_state[k].detach().float().cpu().reshape(own[k].shape) for k in own if k in lora_state},
@@ -349,6 +353,8 @@ def main():
     ap.add_argument("--cpu-seconds", type=float, default=30.0)
     ap.add_argument("--no-train", action="store_true", help="skip the training-iteration timings (configs 3 and 4)")
     ap.add_argument("--no-extra", action="store_true", help="skip BASELINE configs 1, 2 and 5")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else max(min(args.warmup, 1), 1)
 
@@ -359,7 +365,7 @@ def main():
     config = {"workload": f"sdxl_unet_fwd_{args.batch}passes_per_gpu_1024px_lora_r4_noxattn_c3lier",
               "latent": [args.batch, 4, 128, 128], "timestep": 500, "lora": "rank4 alpha1 noxattn+c3lier (346)",
               "parallelism": f"dp{world} (independent passes, weights replicated, no data-path collective)",
-              "l2": "working set (5.1 GB bf16 weights + activations) >> 126 MB L2; no flush needed"}
+              "l2": "working set (5.1 GB bf16 weights + activations) >> 50 MB L2; no flush needed"}
 
     # ------------------------------------------------------------------ reference arm (CPU, rank 0 only)
     if args.impl == "reference":
@@ -407,24 +413,20 @@ def main():
 
         # ---- value: graph replay of the whole forward, inputs resident
         sampler = ClockSampler(local_rank)
-        ms_step = timed(fwd, args.steps, args.warmup, dm, sampler)
+        last = {}
+
+        def fwd_keep():
+            last["unet_sample"] = fwd()
+
+        ms_step = timed(fwd_keep, args.steps, args.warmup, dm, sampler)
         clocks = sampler.stop()
     value = world * B / (ms_step * 1e-3)
     gm = classes.get("gemm", {"ms": 0.0, "launches": 0, "flops": 0.0})
     achieved = gm["flops"] / (gm["ms"] * 1e-3) / 1e12 if gm["ms"] > 0 else 0.0
-    traffic, traffic_note = None, None
-    try:  # per-launch DRAM bytes of the dominant kernel from the committed ncu capture of this workload
-        with open(os.path.join(ROOT, "profiles", "r02_dram_b8.json")) as f:
-            dj = json.load(f)["per_kernel"]["gemm_kernel"]
-        if B == 8:
-            traffic = dj["dram_read_bytes_per_launch"] + dj["dram_write_bytes_per_launch"]
-            traffic_note = dj.get("note")
-    except (OSError, KeyError, ValueError):
-        pass
     sum_ms = sum(c["ms"] for c in classes.values())
-    roofline = {"bound": "tensor", "kernel": "gemm_kernel (tcgen05 GEMM / implicit-GEMM conv)",
+    roofline = {"bound": "tensor", "kernel": "gemm_kernel (wgmma GEMM / implicit-GEMM conv)",
                 "achieved": achieved, "peak": peaks["sustained"], "unit": "TFLOP/s",
-                "frac": achieved / peaks["sustained"], "traffic": traffic, "traffic_note": traffic_note,
+                "frac": achieved / peaks["sustained"],
                 "peak_source": peaks["source"], "launches": gm["launches"],
                 "avg_launch_us": 1e3 * gm["ms"] / max(gm["launches"], 1),
                 "share_of_step": gm["ms"] / ms_step,
@@ -451,6 +453,12 @@ def main():
 
     with torch.no_grad():
         e2e_ms = timed(e2e_step, args.steps, args.warmup, dm)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "unet_sample.npy"), last["unet_sample"].float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "e2e_eps.npy"), eps_host[:half].numpy())
     h2d = (lat_h[:half].numel() * 4 + ehs_h[:2 * half].numel() * 2 + pooled_h[:2 * half].numel() * 2
            + tids_h[:2 * half].numel() * 4)
     e2e = {"value": world * 2 * half / (e2e_ms * 1e-3), "unit": UNIT, "h2d_bytes_per_step": h2d,
@@ -570,7 +578,7 @@ def main():
                 rows[f"B{b}"] = {"ms_per_forward": ms15, "passes_per_s": pps,
                                  "frac_of_sustained": pps * (FLOPS_PER_PASS["sd15"] + FLOPS_LORA[("sd15", 4)]) / 1e12 / peaks["sustained"]}
         extra["config2_sd15_bf16"] = {"what": "SD-1.5 UNet forward, rank-4 LoRA (150 adaptors), latents [B,4,64,64], CUDA-graph "
-                                              "replay; 100 % of sustained = 1775 passes/s", **rows}
+                                              "replay", **rows}
         del u15, n15
 
     # ---- CPU legs (rank 0, N == 1 only): the headline workload's CPU baseline + BASELINE config 1
@@ -609,7 +617,7 @@ def main():
         line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
                 "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "dtype": "bf16", "data": "synthetic", "config": config,
-                "clocks": clocks, "e2e": e2e, "gpu_launches": launches_per_fwd * args.steps,
+                "gpu": gpu_identity(local_rank), "clocks": clocks, "e2e": e2e, "gpu_launches": launches_per_fwd * args.steps,
                 "launches_per_step": launches_per_fwd, "roofline": roofline, "cpu_baseline": cpu_baseline,
                 "train": train, "configs": extra}
         print(json.dumps(line))

@@ -3,7 +3,7 @@
     python eval-scripts/generate_images_xl.py --model_name 'models/ageslider_alpha1.0_rank4_noxattn/..._last.pt' \
         --prompts_path prompts/prompts-person.csv --save_path out/ --embeds person_embeds.pt
 
-The denoise loop runs in sliders_b200 (sm_100a kernels; needs a B200).  See sliders_b200/eval_sweep.py."""
+The denoise loop runs in sliders_b200 (sm_90a kernels; needs an H100).  See sliders_b200/eval_sweep.py."""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 """Text-slider training loop on sliders_b200 — the body of trainscripts/textsliders/train_lora_xl.py:153-380 with the UNet
-forward / backward, the scheduler step and AdamW running in the sm_100a kernels.  Prompt embeddings are inputs: the two
+forward / backward, the scheduler step and AdamW running in the sm_90a kernels.  Prompt embeddings are inputs: the two
 SDXL text encoders run once before the loop in the reference (:100-151) and are off the denoise path, so this example
 takes them from a file written by that code (`torch.save({"target": (text_embeds, pooled_embeds), ...})`) or, with
 --synthetic, draws random ones (shape check / throughput only).
@@ -9,7 +9,7 @@ takes them from a file written by that code (`torch.save({"target": (text_embeds
     python examples/train_text_slider_xl.py --unet /path/unet/diffusion_pytorch_model.safetensors --embeds pair.pt \
         --rank 4 --alpha 1 --train_method noxattn --save_path models/ageslider
 
-Needs a B200 (there is no CPU path).
+Needs an H100 (there is no CPU path).
 """
 import argparse
 import os

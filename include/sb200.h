@@ -1,5 +1,5 @@
 /*
- * sb200.h — C ABI of the sliders_b200 CUDA extension (libsb200.so, sm_100a only).
+ * sb200.h — C ABI of the sliders_b200 CUDA extension (libsb200.so, sm_90a only).
  *
  * This is the drop-in boundary for the per-timestep UNet denoise of rohitgandikota/sliders. The reference
  * has no FFI of its own (it is pure Python on top of diffusers/torch); the entry points below are what a
@@ -29,7 +29,7 @@ typedef enum sb200_status {
   SB200_OK = 0,
   SB200_ERR_INVALID = -1,   /* bad shape / alignment / flag combination */
   SB200_ERR_CUDA = -2,      /* a CUDA runtime / driver call failed */
-  SB200_ERR_UNSUPPORTED = -3 /* device is not sm_100 */
+  SB200_ERR_UNSUPPORTED = -3 /* device is not sm_90 */
 } sb200_status;
 
 /* epilogue flags of sb200_gemm / sb200_conv3x3 */
@@ -41,7 +41,7 @@ enum {
   SB200_EPI_LORA = 16     /* + scale * (X . down^T) . up^T, rank r, computed in the same tile loop */
 };
 
-/* ABI / build identification: "sb200 <version> sm_100a". */
+/* ABI / build identification: "sb200 <version> sm_90a". */
 const char* sb200_version(void);
 const char* sb200_last_error(void);
 
@@ -185,7 +185,7 @@ int sb200_colsum(void* handle, void* stream, const void* dy, int ld, float* out,
  * and the 3x3-conv forms (down is a 3x3 conv with the leaf's stride, D = lora_down packed [r,3,3,C]).
  * ws: SB200_WGRAD_WS_FLOATS(C, r) floats (C = 9 * channels for the conv form). */
 #define SB200_WGRAD_CBLOCKS(C) (((C) / 8 + 31) / 32)
-#define SB200_WGRAD_CHUNKS(cblocks) ((296 + (cblocks) - 1) / (cblocks) > 256 ? 256 : (296 + (cblocks) - 1) / (cblocks))
+#define SB200_WGRAD_CHUNKS(cblocks) ((264 + (cblocks) - 1) / (cblocks) > 256 ? 256 : (264 + (cblocks) - 1) / (cblocks))
 #define SB200_WGRAD_WS_FLOATS(C, r) ((size_t)SB200_WGRAD_CHUNKS(SB200_WGRAD_CBLOCKS(C)) * (C) * (r))
 int sb200_lora_proj(void* handle, void* stream, const void* A, int lda, const void* Bt, int ldb, float* T, int M,
                     int C, int r, int accumulate);
@@ -255,10 +255,6 @@ int sb200_cfg_ddim(void* handle, void* stream, const void* eps2, int eps_is_f32,
  * carries): cx = 1, ce = sigma_next - sigma. */
 int sb200_cfg_step(void* handle, void* stream, const void* eps2, int eps_is_f32, float g, const void* x, float cx,
                    float ce, void* x_prev, void* eps_out, int out_is_f32, int64_t n);
-
-/* Debug: clock64 phase stamps of CTA (0,0,0) of the last ping-pong attention launch made with SB200_ATTN_POLY=1
- * (layout: sliders_b200/csrc/attention.cu, g_pp_trace).  n <= 8192 values.  Synchronises the device. */
-int sb200_debug_attention_trace(long long* dst, int n);
 
 #ifdef __cplusplus
 }

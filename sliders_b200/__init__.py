@@ -1,4 +1,4 @@
-"""sliders_b200 — B200-native (sm_100a) concept-slider UNet denoise path.
+"""sliders_b200 — H100-native (sm_90a) concept-slider UNet denoise path.
 
 Public surface mirrors rohitgandikota/sliders (trainscripts/textsliders): `LoRANetwork`, `LoRAModule`,
 `train_util.predict_noise(_xl)`, `diffusion(_xl)`; the arithmetic runs in hand-written CUDA kernels behind

@@ -1,7 +1,7 @@
 """ctypes binding of libsb200.so (C ABI in include/sb200.h).
 
 The product path has no CPU or PyTorch fallback: if the CUDA extension is missing or the device is not
-sm_100 every entry point raises.  torch is used only for device memory, streams and torch.distributed.
+sm_90 every entry point raises.  torch is used only for device memory, streams and torch.distributed.
 """
 from __future__ import annotations
 
@@ -62,7 +62,6 @@ SIGNATURES = {
     "sb200_conv3x3": [_p, _p, _p, _i, _p, _i, _i, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p, _i,
                       _LP, _i],
     "sb200_attention": [_p, _p, _p, _i, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _i, _f, _p],
-    "sb200_debug_attention_trace": [_p, _i],
     "sb200_attention_bwd": [_p, _p, _p, _i, _p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _p, _i, _p, _i, _p, _i,
                             _i, _i, _i, _i, _i, _f],
     "sb200_groupnorm_bwd": [_p, _p, _p, _i, _i, _p, _i, _i, _p, _p, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _p, _p],

@@ -3,7 +3,7 @@
 autograd through the frozen diffusers UNet down to every `lora_down.weight` / `lora_up.weight` (lora.py:97-112).
 
 The frozen weights need no gradient, so the pass is
-  * the input-gradient chain of every op (dense products on the same tcgen05 GEMM / implicit-GEMM conv kernels with
+  * the input-gradient chain of every op (dense products on the same wgmma GEMM / implicit-GEMM conv kernels with
     transposed weights, flash-attention backward, GroupNorm / LayerNorm / GEGLU / SiLU backward), and
   * per adapted leaf  y = W x + s up (down x):  d_up = s dY^T (x down^T),  d_down = s (dY up)^T x,  dX += s (dY up) down
     as rank-r reductions (csrc/backward.cu).

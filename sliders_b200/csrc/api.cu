@@ -77,7 +77,7 @@ using namespace sb200;
 
 extern "C" {
 
-const char* sb200_version(void) { return "sb200 0.1 sm_100a"; }
+const char* sb200_version(void) { return "sb200 0.1 sm_90a"; }
 
 const char* sb200_last_error(void) { return g_err; }
 
@@ -86,8 +86,8 @@ int sb200_create(int device, void** handle) {
   SB200_CUDA_CHECK(cudaSetDevice(device));
   cudaDeviceProp prop;
   SB200_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return set_error(SB200_ERR_UNSUPPORTED, "device %d is sm_%d%d; libsb200 is built for sm_100a only",
+  if (prop.major != 9 || prop.minor != 0)
+    return set_error(SB200_ERR_UNSUPPORTED, "device %d is sm_%d%d; libsb200 is built for sm_90a only",
                      device, prop.major, prop.minor);
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult qres;

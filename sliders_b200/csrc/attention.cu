@@ -1,19 +1,18 @@
-// Flash-attention forward for sm_100a:  O = softmax(Q K^T * scale) V  per (batch, head), head dim d <= 192
+// Flash-attention forward for sm_90a:  O = softmax(Q K^T * scale) V  per (batch, head), head dim d <= 192
 // (SDXL: 64; SD1.x: 40 / 80 / 160).  The head dim is padded to ND x 64 columns by TMA's out-of-bounds zero
 // fill: Q/K/V are addressed through 4-D descriptors (d, heads, tokens, batch), so a 64-wide box that sticks out
 // of a 40- or 80-wide head reads zeros, never the neighbouring head.
 //
-// One CTA per (128-query tile, head, batch).  ND = 1: two CTAs resident per SM (256 TMEM columns, ~81 KB smem
-// each) so one CTA's tensor-core work overlaps the other's softmax; ND = 2, 3: one CTA per SM.
-//   warp 0      TMA producer: Q tile once, then K / V tiles (128 keys x ND x 64) through a ring of stages
-//   warp 1      MMA issuer  : S = Q K^T   (tcgen05.mma SS, 128x128x16 per k-step, fp32 in TMEM columns [0,128))
-//                             O += P V    (tcgen05.mma TS: P read from TMEM, V MN-major from smem, N = 64 per
-//                                          sub-tile of the head dim)
-//   warps 2..9  softmax     : one query row per PAIR of threads (warp w and w + 4 split the 128 key columns). Two passes over S in TMEM (row max, then exp2 + bf16
-//                             pack), P written back to TMEM columns [128,192) as the A operand of the PV MMA; the
-//                             O accumulator (columns [192, 192 + 64 ND)) stays in TMEM and is rescaled lazily
-//                             (only when the running max grows by > 2^8).
-// Keys beyond Skv (cross-attention: 77) are masked to -inf; TMA zero-fills the out-of-range rows.
+// One CTA per (128-query tile, head, batch), 288 threads:
+//   warp 8      TMA producer: Q tile once, then K / V tiles (KV keys x ND x 64) through a ring of stages
+//   warps 0..7  two consumer warpgroups, 64 query rows each:
+//                 S = Q K^T   wgmma m64 x KV x 16 from shared memory, fp32 in registers
+//                 online softmax on the accumulator fragment (each thread holds two rows; a row's max / sum is
+//                 reduced over the four threads of a quad), P packed to bf16 in place as the A operand of
+//                 O += P V   wgmma m64 x 64 x 16 per 64 columns of the head, A from registers, V MN-major from smem
+// The two warpgroups run independently, so one's softmax overlaps the other's tensor work.  KV = 128 keys for
+// d <= 64 and 64 keys for wider heads (the O accumulator takes the registers).  Keys beyond Skv are masked to -inf;
+// TMA zero-fills the out-of-range rows.
 //
 // Replaces the attention processor that diffusers' Attention calls (xformers memory_efficient_attention /
 // torch SDPA; reference: trainscripts/textsliders/train_lora_xl.py:79-80, train_lora.py:68).
@@ -22,9 +21,8 @@
 
 namespace sb200 {
 
-constexpr int kAttnThreads = 320;  // TMA warp, MMA warp, 8 softmax warps
-constexpr int kTileBytes = 128 * 128;  // 128 rows x 64 bf16
-constexpr uint32_t kColS = 0, kColP = 128, kColO = 192;
+constexpr int kAttnThreads = 288;       // two consumer warpgroups + the TMA warp
+constexpr int kQTileBytes = 128 * 128;  // 128 rows x 64 bf16
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
@@ -32,110 +30,12 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
-// ---- packed fp32 pairs (FFMA2 / FADD2, new on sm_100): one issue slot for two elements.  The softmax warps are bound by
-// their own instruction streams (profiles/r02_attention_ncu_summary.txt: no pipe above 62 %), so instructions per
-// element, not pipe throughput, is what the exp loop is written for.
-__device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-
-// 2^x on the FMA / ALU pipes (Cody-Waite split + degree-3 minimax polynomial, max relative error 7.5e-5 — far below
-// the bf16 rounding of P) for a PAIR of arguments.  MUFU.EX2 runs at 16 lanes / clk / SM; one pair in every kPolyDen
-// goes here instead (FlashAttention-4 does the same), kPolyDen = 0: none.
-__device__ __forceinline__ void poly_exp2_x2(uint64_t x2, float& p0, float& p1) {
-  float x0, x1;
-  f2_unpack(x2, x0, x1);
-  x2 = f2_pack(fmaxf(x0, -126.f), fmaxf(x1, -126.f));
-  const uint64_t t2 = f2_add(x2, f2_pack(12582912.f, 12582912.f));  // 1.5 * 2^23: round(x) in the low mantissa bits
-  const uint64_t n2 = f2_add(t2, f2_pack(-12582912.f, -12582912.f));
-  const uint64_t f2 = f2_fma(n2, f2_pack(-1.f, -1.f), x2);          // x - round(x), in [-0.5, 0.5]
-  uint64_t r2 = f2_fma(f2_pack(0.0551716685295105f, 0.0551716685295105f), f2,
-                       f2_pack(0.2426111251115799f, 0.2426111251115799f));
-  r2 = f2_fma(r2, f2, f2_pack(0.6932609677314758f, 0.6932609677314758f));
-  r2 = f2_fma(r2, f2, f2_pack(0.9999280571937561f, 0.9999280571937561f));
-  float t0, t1, r0, r1;
-  f2_unpack(t2, t0, t1);
-  f2_unpack(r2, r0, r1);
-  p0 = __int_as_float(__float_as_int(r0) + (__float_as_int(t0) << 23));  // * 2^round(x)
-  p1 = __int_as_float(__float_as_int(r1) + (__float_as_int(t1) << 23));
-}
-
-// 32 scores (registers v[0..32), as loaded from TMEM) -> p = 2^(v * scale - m): 16 packed bf16 pairs in pk, row sums
-// accumulated into the two packed accumulators acc[0..2) (four independent chains)
-template <int kPolyDen>
-__device__ __forceinline__ void exp_chunk32(const uint32_t* v, float scale, float m, uint32_t* pk, uint64_t* acc) {
-  const uint64_t scale2 = f2_pack(scale, scale), negm2 = f2_pack(-m, -m);
-#pragma unroll
-  for (int e = 0; e < 16; ++e) {
-    const uint64_t x2 = f2_fma(f2_pack(__uint_as_float(v[2 * e]), __uint_as_float(v[2 * e + 1])), scale2, negm2);
-    float p0, p1;
-    if (kPolyDen != 0 && (e % (kPolyDen ? kPolyDen : 1)) == (kPolyDen ? kPolyDen : 1) - 1) {
-      poly_exp2_x2(x2, p0, p1);
-    } else {
-      float x0, x1;
-      f2_unpack(x2, x0, x1);
-      p0 = fast_exp2(x0);
-      p1 = fast_exp2(x1);
-    }
-    acc[e & 1] = f2_add(acc[e & 1], f2_pack(p0, p1));
-    pk[e] = pack_bf16x2(p0, p1);
-  }
-}
-
-// The same work split in two, for a caller that puts a scheduling fence (__syncwarp) between "issue" of one chunk and
-// "consume" of the previous one.  ptxas paces a warp's MUFUs at the pipe rate (8 clk) and places each consumer one
-// pair (16 clk) behind its producer; the real latency is longer, more so when two warps share the unit, so a warp in
-// exp_chunk32 stalls on every pair — 16 clk per MUFU measured, alone or not (tools/gpu_attn_trace.py).  With 32
-// exponentials in flight before the first one is read, the stall disappears.
-template <int kPolyDen>
-__device__ __forceinline__ void exp_issue32(uint32_t* v, float scale, float m) {
-  const uint64_t scale2 = f2_pack(scale, scale), negm2 = f2_pack(-m, -m);
-#pragma unroll
-  for (int e = 0; e < 16; ++e) {
-    const uint64_t x2 = f2_fma(f2_pack(__uint_as_float(v[2 * e]), __uint_as_float(v[2 * e + 1])), scale2, negm2);
-    float p0, p1;
-    if (kPolyDen != 0 && (e % (kPolyDen ? kPolyDen : 1)) == (kPolyDen ? kPolyDen : 1) - 1) {
-      poly_exp2_x2(x2, p0, p1);
-    } else {
-      float x0, x1;
-      f2_unpack(x2, x0, x1);
-      p0 = fast_exp2(x0);
-      p1 = fast_exp2(x1);
-    }
-    v[2 * e] = __float_as_uint(p0);
-    v[2 * e + 1] = __float_as_uint(p1);
-  }
-}
-__device__ __forceinline__ void exp_consume32(const uint32_t* v, uint32_t* pk, uint64_t* acc) {
-#pragma unroll
-  for (int e = 0; e < 16; ++e) {
-    const float p0 = __uint_as_float(v[2 * e]), p1 = __uint_as_float(v[2 * e + 1]);
-    acc[e & 1] = f2_add(acc[e & 1], f2_pack(p0, p1));
-    pk[e] = pack_bf16x2(p0, p1);
-  }
-}
-
 template <int ND>
 struct AttnCfg {
-  static constexpr int kStages = ND == 3 ? 1 : 2;
-  static constexpr int kSmem = kTileBytes * ND * (1 + 2 * kStages) + 1024 /*barriers*/ + 2048 /*pair exchange*/ + 1024 /*align*/;
-  static constexpr int kTmemCols = ND == 1 ? 256 : 512;
-  static constexpr int kMinBlocks = ND == 1 ? 2 : 1;
+  static constexpr int kKV = ND == 1 ? 128 : 64;  // keys per K / V tile
+  static constexpr int kStages = 2;
+  static constexpr uint32_t kKVBytes = kKV * 128 * ND;  // one K or V tile
+  static constexpr int kSmem = kQTileBytes * ND + 2 * kStages * kKVBytes + 1024 /*barriers*/ + 1024 /*align*/;
 };
 
 struct AttnParams {
@@ -146,48 +46,33 @@ struct AttnParams {
   int Sq, Skv;
   int d;           // head dim (multiple of 8)
   int n_kv_tiles;
-  int split_issue;   // 1: Q K^T issued by the TMA warp, P V by the MMA warp (default); 0: both by the MMA warp
-  int q_per_cta;     // two-CTA kernel: consecutive 128-query tiles one CTA walks (> 1 for short key sequences: the
-                     // per-CTA fixed cost of a cross-attention tile is several times its work)
-  int split_exp;     // two-CTA kernel: 1 = issue a chunk's 32 exponentials, fence, then sum / pack them
-  int pp_token;      // ping-pong kernel: 1 = the two warpgroups hand the MUFU unit to each other explicitly
   float scale_log2;  // scale * log2(e)
 };
 
-template <int ND, int kPoly>
-__global__ void __launch_bounds__(kAttnThreads, AttnCfg<ND>::kMinBlocks)
-    attention_kernel(const __grid_constant__ AttnParams p) {
+template <int ND>
+__global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid_constant__ AttnParams p) {
+  constexpr int kKV = AttnCfg<ND>::kKV;
   constexpr int kStages = AttnCfg<ND>::kStages;
-  constexpr uint32_t kStageBytes = kTileBytes * ND;
+  constexpr uint32_t kKVBytes = AttnCfg<ND>::kKVBytes;
+  constexpr uint32_t kKVChunk = kKV * 128;  // 64 head columns of a K / V tile
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t base = (raw_addr + 1023u) & ~1023u;
-  uint8_t* smem = smem_raw + (base - raw_addr);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int qpc = p.q_per_cta;             // query tiles of this CTA: blockIdx.x * qpc + qi
-  const int qt0 = blockIdx.x * qpc, head = blockIdx.y, b = blockIdx.z;
-  const int nq = min(qpc, (p.Sq + 127) / 128 - qt0);
+  const int qt = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
 
   const uint32_t sQ = base;
-  const uint32_t sK = base + kStageBytes;
-  const uint32_t sV = sK + kStages * kStageBytes;
-  const uint32_t bars = sV + kStages * kStageBytes;
+  const uint32_t sK = base + kQTileBytes * ND;
+  const uint32_t sV = sK + kStages * kKVBytes;
+  const uint32_t bars = sV + kStages * kKVBytes;
   const uint32_t bar_q = bars;
   const uint32_t bar_kfull = bars + 8;                   // kStages
   const uint32_t bar_kempty = bar_kfull + 8 * kStages;   // kStages
   const uint32_t bar_vfull = bar_kempty + 8 * kStages;
   const uint32_t bar_vempty = bar_vfull + 8 * kStages;
-  const uint32_t bar_sfull = bar_vempty + 8 * kStages;
-  const uint32_t bar_sfree = bar_sfull + 8;
-  const uint32_t bar_pfull = bar_sfree + 8;
-  const uint32_t bar_pvdone = bar_pfull + 8;
-  const uint32_t bar_qfree = bar_pvdone + 8;   // Q tile read by its last Q K^T (query-tile loop)
-  const uint32_t bar_ofree = bar_qfree + 8;    // O read by the epilogue of the previous query tile
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + (bars - base) + 512);
-  float* xch = reinterpret_cast<float*>(smem + (bars - base) + 1024);  // [2 parities][2 halves][128 rows]
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tmQ);
@@ -198,694 +83,163 @@ __global__ void __launch_bounds__(kAttnThreads, AttnCfg<ND>::kMinBlocks)
     mbar_init(bar_q, 1);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(bar_kfull + 8 * i, 1);
-      mbar_init(bar_kempty + 8 * i, 1);
+      mbar_init(bar_kempty + 8 * i, 2);  // one arrival per consumer warpgroup
       mbar_init(bar_vfull + 8 * i, 1);
-      mbar_init(bar_vempty + 8 * i, 1);
+      mbar_init(bar_vempty + 8 * i, 2);
     }
-    mbar_init(bar_sfull, 1);
-    mbar_init(bar_sfree, 8);
-    mbar_init(bar_pfull, 8);
-    mbar_init(bar_pvdone, 1);
-    mbar_init(bar_qfree, 1);
-    mbar_init(bar_ofree, 8);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), AttnCfg<ND>::kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
   const int n = p.n_kv_tiles;
-  const int dsteps = (p.d + 15) >> 4;  // 16-wide k-steps of the QK^T contraction that hold data
-
-  // S_t = Q K_t^T.  Tile j + 1 is issued BEFORE P_j V_j, as soon as the softmax warps have read S_j, so the next S is
-  // ready when they finish tile j.  One thread can issue a tcgen05.mma only every ~176 cycles whatever its size
-  // (tools/micro/umma_bench.cu), and a tile needs 4 + 8 of them, so the two products are issued by DIFFERENT warps
-  // (split_issue): warp 0 issues Q K^T right behind its TMA loads, warp 1 issues P V.  (Measured neutral at d = 64:
-  // 646 vs 643 TFLOP/s — with two CTAs per SM the SM already has two issuing threads; kept because it shortens the
-  // MMA warp's critical path for ND > 1.)
-  const uint32_t idesc_qk = umma_idesc_bf16(128, 128, 0);
-  auto issue_qk = [&](int t, bool last_of_q) {
-    const int s = t % kStages;
-    const uint32_t ph = (t / kStages) & 1;
-    mbar_wait(bar_kfull + 8 * s, ph);
-    mbar_wait(bar_sfree, (t & 1) ^ 1u);  // softmax finished reading S_{t-1}
-    tc_fence_after();
-    if (elect_one()) {
-      for (int k = 0; k < dsteps; ++k) {
-        const uint32_t off = static_cast<uint32_t>(k >> 2) * kTileBytes + static_cast<uint32_t>(k & 3) * 32;
-        umma_ss(tmem_base + kColS, umma_desc_sw128(sQ + off), umma_desc_sw128(sK + s * kStageBytes + off), idesc_qk,
-                k != 0);
-      }
-      umma_commit(bar_kempty + 8 * s);
-      umma_commit(bar_sfull);
-      if (last_of_q) umma_commit(bar_qfree);
-    }
-    __syncwarp();
-  };
-
-  if (warp == 0) {
-    // converged warp, one ELECTed lane issues (a `lane == 0` branch makes ptxas wrap every uniform-datapath
-    // instruction in an ELECT / BRA.U.ANY retry loop)
-    for (int qi = 0; qi < nq; ++qi) {
-      if (qi > 0) mbar_wait(bar_qfree, (qi - 1) & 1);  // the previous tile's products have read sQ
-      if (elect_one()) {
-        mbar_expect_tx(bar_q, kStageBytes);
-#pragma unroll
-        for (int i = 0; i < ND; ++i) tma_load_4d(sQ + i * kTileBytes, &p.tmQ, bar_q, i * 64, head, (qt0 + qi) * 128, b);
-      }
-      __syncwarp();
-      for (int j = 0; j < n; ++j) {
-        const int g = qi * n + j;  // tiles of this CTA so far: stages and barrier phases run on
-        const int s = g % kStages;
-        const uint32_t ph = (g / kStages) & 1;
-        mbar_wait(bar_kempty + 8 * s, ph ^ 1u);
-        if (elect_one()) {
-          mbar_expect_tx(bar_kfull + 8 * s, kStageBytes);
-#pragma unroll
-          for (int i = 0; i < ND; ++i)
-            tma_load_4d(sK + s * kStageBytes + i * kTileBytes, &p.tmK, bar_kfull + 8 * s, i * 64, head, j * 128, b);
-        }
-        __syncwarp();
-        mbar_wait(bar_vempty + 8 * s, ph ^ 1u);
-        if (elect_one()) {
-          mbar_expect_tx(bar_vfull + 8 * s, kStageBytes);
-#pragma unroll
-          for (int i = 0; i < ND; ++i)
-            tma_load_4d(sV + s * kStageBytes + i * kTileBytes, &p.tmV, bar_vfull + 8 * s, i * 64, head, j * 128, b);
-        }
-        __syncwarp();
-        if (p.split_issue) {
-          if (j == 0) mbar_wait(bar_q, qi & 1);
-          issue_qk(g, j == n - 1);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    const uint32_t idesc_pv = umma_idesc_bf16(128, 64, 1);  // B (= V) is MN-major
-    if (!p.split_issue) {  // single issuing warp (same-box A/B; one query tile per CTA in this mode)
-      mbar_wait(bar_q, 0);
-      issue_qk(0, n == 1);
-    }
-    for (int qi = 0; qi < nq; ++qi) {
-      for (int j = 0; j < n; ++j) {
-        const int g = qi * n + j;
-        const int s = g % kStages;
-        const uint32_t ph = (g / kStages) & 1;
-        if (!p.split_issue && j + 1 < n) issue_qk(j + 1, j + 2 == n);
-        // ---- O += P_j V_j
-        mbar_wait(bar_vfull + 8 * s, ph);
-        mbar_wait(bar_pfull, g & 1);
-        if (j == 0 && qi > 0) mbar_wait(bar_ofree, (qi - 1) & 1);  // the previous tile's O has been read out
-        tc_fence_after();
-        if (elect_one()) {
-          const int kv_left = p.Skv - j * 128;
-          const int ksteps = kv_left >= 128 ? 8 : (kv_left + 15) >> 4;  // keys beyond Skv contribute nothing
-          for (int k = 0; k < ksteps; ++k) {
-#pragma unroll
-            for (int i = 0; i < ND; ++i)
-              umma_ts(tmem_base + kColO + i * 64, tmem_base + kColP + k * 8,
-                      umma_desc_sw128(sV + s * kStageBytes + i * kTileBytes + k * 2048), idesc_pv, (j | k) != 0);
-          }
-          umma_commit(bar_vempty + 8 * s);
-          umma_commit(bar_pvdone);
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    // ---------------------------------------------------------------- softmax / correction / store
-    // Two warps per 32-row TMEM lane quarter (warps w and w + 4): each owns 64 of the tile's 128 key columns.  The
-    // pair exchanges its row maxima through shared memory once per tile.  (Measured: 551 -> 565 TFLOP/s at S = 4096;
-    // a variant that kept the 64 S values in registers to read TMEM once was 40 % slower at 96 registers / thread.)
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int row = q * 32 + lane;
-    const uint32_t tl = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    const uint32_t colS = kColS + half * 64, colP = kColP + half * 32;
-    const uint32_t pair_bar = 1 + q;
-    int xc = 0;  // pair exchanges so far (alternating buffers)
-    for (int qi = 0; qi < nq; ++qi) {  // query tiles of this CTA (body not re-indented)
-    const int g0 = qi * n;
-    float m_run = -INFINITY;  // running max, already multiplied by scale*log2e
-    float l_run = 0.f;        // this warp's share of the row sum
-    for (int j = 0; j < n; ++j) {
-      const int g = g0 + j;   // tiles of this CTA so far: barrier phases run on across query tiles
-      mbar_wait(bar_sfull, g & 1);
-      tc_fence_after();
-      const int kv_left = p.Skv - j * 128 - half * 64;  // valid keys among this warp's 64 columns (may be <= 0)
-      // pass 1: row max over my columns
-      float mx = -INFINITY;
-      if (kv_left > 0) {
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          uint32_t v[32];
-          tmem_ld_x32(tl + colS + c * 32, v);
-          tmem_ld_wait();
-          if (kv_left >= (c + 1) * 32) {
-            // four independent chains: a single running max is a 32-deep dependent chain (4 clk each)
-            float m0 = __uint_as_float(v[0]), m1 = __uint_as_float(v[1]), m2 = __uint_as_float(v[2]),
-                  m3 = __uint_as_float(v[3]);
-#pragma unroll
-            for (int i = 4; i < 32; i += 4) {
-              m0 = fmaxf(m0, __uint_as_float(v[i]));
-              m1 = fmaxf(m1, __uint_as_float(v[i + 1]));
-              m2 = fmaxf(m2, __uint_as_float(v[i + 2]));
-              m3 = fmaxf(m3, __uint_as_float(v[i + 3]));
-            }
-            mx = fmaxf(mx, fmaxf(fmaxf(m0, m1), fmaxf(m2, m3)));
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (c * 32 + i < kv_left) mx = fmaxf(mx, __uint_as_float(v[i]));
-          }
-        }
-      }
-      float* xs = xch + ((xc++ & 1) * 2) * 128;
-      xs[half * 128 + row] = mx;
-      asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-      mx = fmaxf(mx, xs[(half ^ 1) * 128 + row]);
-      mx *= p.scale_log2;
-      float alpha = 1.f;
-      bool need = false;
-      if (j == 0) {
-        m_run = mx;
-      } else if (mx - m_run > 8.f) {
-        need = true;
-        alpha = fast_exp2(m_run - mx);
-        m_run = mx;
-      }
-      if (g > 0) {
-        // the previous P has been consumed (and, for j > 0, O holds the sum over tiles < j)
-        mbar_wait(bar_pvdone, (g - 1) & 1);
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, need)) {  // identical in both warps of the pair (same rows, same maxima)
-          l_run *= alpha;
-#pragma unroll
-          for (int c = 0; c < ND; ++c) {
-            uint32_t o[32];
-            tmem_ld_x32(tl + kColO + c * 64 + half * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st_x16(tl + kColO + c * 64 + half * 32, o);
-            tmem_st_x16(tl + kColO + c * 64 + half * 32 + 16, o + 16);
-          }
-          tmem_st_wait();
-        }
-      }
-      // pass 2: p = exp2(s*scale*log2e - m), pack to bf16, store as the A operand of the PV MMA
-      float lsum = 0.f;
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        if (kv_left > c * 32) {
-          tmem_ld_x32(tl + colS + c * 32, v);
-          tmem_ld_wait();
-        }
-        if (c == 1) {
-          // every S column of this warp is now in registers: release S for the next QK MMA
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_sfree);
-        }
-        if (kv_left <= c * 32) continue;  // columns beyond Skv: the PV MMA never reads them (ksteps limit)
-        uint32_t pk[16];
-        if (kv_left >= (c + 1) * 32) {  // warp-uniform: no masking code on full chunks
-          uint64_t acc[2] = {0ull, 0ull};
-          if (p.split_exp) {
-            // all 32 exponentials in flight before the first one is read (see exp_issue32)
-            exp_issue32<kPoly>(v, p.scale_log2, m_run);
-            __syncwarp();
-            exp_consume32(v, pk, acc);
-          } else {
-            exp_chunk32<kPoly>(v, p.scale_log2, m_run, pk, acc);
-          }
-          float a0, a1, a2, a3;
-          f2_unpack(acc[0], a0, a1);
-          f2_unpack(acc[1], a2, a3);
-          lsum += (a0 + a1) + (a2 + a3);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float p0 = fast_exp2(fmaf(__uint_as_float(v[2 * i]), p.scale_log2, -m_run));
-            float p1 = fast_exp2(fmaf(__uint_as_float(v[2 * i + 1]), p.scale_log2, -m_run));
-            if (c * 32 + 2 * i >= kv_left) p0 = 0.f;
-            if (c * 32 + 2 * i + 1 >= kv_left) p1 = 0.f;
-            lsum += p0 + p1;
-            pk[i] = pack_bf16x2(p0, p1);
-          }
-        }
-        tmem_st_x16(tl + colP + c * 16, pk);
-      }
-      l_run += lsum;
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_pfull);
-    }
-    // ---- finalize: O / l -> bf16 -> global (only the first d columns of the padded head); each warp of the pair
-    // writes its 32 of every 64 O columns
-    {
-      float* xs = xch + ((xc++ & 1) * 2) * 128;
-      xs[half * 128 + row] = l_run;
-      asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-      l_run += xs[(half ^ 1) * 128 + row];
-    }
-    mbar_wait(bar_pvdone, (g0 + n - 1) & 1);
-    tc_fence_after();
-    const float inv = 1.f / l_run;
-    const int srow = (qt0 + qi) * 128 + row;
-    if (half == 0 && p.lse != nullptr && srow < p.Sq)
-      p.lse[(static_cast<size_t>(b) * gridDim.y + head) * p.Sq + srow] = m_run + log2f(l_run);
-    __nv_bfloat16* op = p.o + (static_cast<size_t>(b) * p.Sq + srow) * p.ldo + head * p.d;
-#pragma unroll
-    for (int c = 0; c < ND; ++c) {
-      const int col0 = c * 64 + half * 32;
-      if (col0 < p.d) {  // warp-uniform
-        uint32_t o[32];
-        tmem_ld_x32(tl + kColO + col0, o);
-        tmem_ld_wait();
-        if (srow < p.Sq) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            if (col0 + i * 8 < p.d) {
-              uint4 w;
-              w.x = pack_bf16x2(__uint_as_float(o[8 * i + 0]) * inv, __uint_as_float(o[8 * i + 1]) * inv);
-              w.y = pack_bf16x2(__uint_as_float(o[8 * i + 2]) * inv, __uint_as_float(o[8 * i + 3]) * inv);
-              w.z = pack_bf16x2(__uint_as_float(o[8 * i + 4]) * inv, __uint_as_float(o[8 * i + 5]) * inv);
-              w.w = pack_bf16x2(__uint_as_float(o[8 * i + 6]) * inv, __uint_as_float(o[8 * i + 7]) * inv);
-              *reinterpret_cast<uint4*>(op + col0 + i * 8) = w;
-            }
-          }
-        }
-      }
-    }
-    // O is in registers / on its way out: the next query tile's first P V may overwrite it
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar_ofree);
-    }  // query tiles
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, AttnCfg<ND>::kTmemCols);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Ping-pong variant for head dim <= 64 and long key sequences (self-attention: S = 4096 / 1024).
-//
-// The kernel above keeps two CTAs per SM, and in each a PAIR of threads per query row that exchanges maxima through
-// shared memory; its stall samples (profiles/r02_attention_ncu_summary.txt) show the softmax warps in the exp block
-// only 42 % of their time and the two warps of a pair in lock-step, so an SM sub-partition has effectively two
-// independent exp streams and its MUFU unit idles ~40 % of the time.  Here ONE CTA per SM owns TWO 128-query tiles that
-// share every K / V tile: tile i has its own S_i / P_i / O_i in TMEM (512 columns in all) and its own softmax
-// warpgroup (one thread per query row, the row's 128 scores in registers: one TMEM read, no exchange).  Q_i K(j+1)^T is
-// issued the moment warpgroup i has S_i(j) in registers, so the next scores are ready before it has finished
-// exponentiating the current ones; P_i(j) V(j) follows the warpgroup's last store, and the only thing a warpgroup ever
-// waits for in steady state is the MUFU unit.  (First version, one MMA warp alternating P_0 V, Q_0 K, P_1 V, Q_1 K
-// behind the softmax: 590 TFLOP/s at S = 4096 against 643 for the kernel above — each warpgroup idled ~1 500 cycles
-// per tile waiting for its own two products.)
-//   warps 0..3  softmax of query tile 0 (TMEM lane quarter = warp)      warp 8  TMA producer
-//   warps 4..7  softmax of query tile 1                                  warp 9  Q K^T issuer, warp 10  P V issuer
-// SB200_ATTN_POLY=1 selects a build of the kernel that timestamps (clock64) the phases of CTA (0,0,0) into
-// g_pp_trace: [role][event] with roles 0 / 1 = first softmax warp of tile 0 / 1 (six stamps per key tile: scores full,
-// scores in registers, max done, first 32 exponentials done, previous P V done, P stored), 2 = Q K^T issuer (two per
-// product: waits over, issued), 3 = P V issuer (same).  tools/gpu_attn_trace.py prints the timeline.
-constexpr int kPpTraceLen = 2048;
-__device__ long long g_pp_trace[4 * kPpTraceLen];
-constexpr int kPpThreads = 352;
-constexpr int kPpStages = 3;
-constexpr int kPpSmem = kTileBytes * (2 + 2 * kPpStages) + 1024 /*barriers*/ + 1024 /*align*/;
-constexpr uint32_t kPpColS = 0, kPpColP = 256, kPpColO = 384;
-
-template <int kPolyArg>
-__global__ void __launch_bounds__(kPpThreads, 1) attention_pp_kernel(const __grid_constant__ AttnParams p) {
-  constexpr bool kTrace = kPolyArg == 1;
-  constexpr int kPoly = kTrace ? 0 : kPolyArg;
-  int trace_n = 0;
-  const bool trace_on = kTrace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (threadIdx.x & 31) == 0;
-  auto stamp = [&](int role) {
-    if (kTrace && trace_on && trace_n < kPpTraceLen) g_pp_trace[role * kPpTraceLen + trace_n++] = clock64();
-  };
-  pdl_trigger();
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  const uint32_t base = (raw_addr + 1023u) & ~1023u;
-  uint8_t* smem = smem_raw + (base - raw_addr);
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int qt = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
-
-  const uint32_t sQ = base;                        // two 128-row tiles
-  const uint32_t sK = base + 2 * kTileBytes;
-  const uint32_t sV = sK + kPpStages * kTileBytes;
-  const uint32_t bars = sV + kPpStages * kTileBytes;
-  const uint32_t bar_q = bars;
-  const uint32_t bar_kfull = bars + 8;
-  const uint32_t bar_kempty = bar_kfull + 8 * kPpStages;
-  const uint32_t bar_vfull = bar_kempty + 8 * kPpStages;
-  const uint32_t bar_vempty = bar_vfull + 8 * kPpStages;
-  const uint32_t bar_sfull = bar_vempty + 8 * kPpStages;  // [2]
-  const uint32_t bar_pfull = bar_sfull + 16;               // [2]
-  const uint32_t bar_sfree = bar_pfull + 16;               // [2]
-  const uint32_t bar_pvdone = bar_sfree + 16;              // [2]
-  const uint32_t bar_turn = bar_pvdone + 16;               // [2 tiles][4 lane quarters]: the MUFU token
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + (bars - base) + 512);
-
-  if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&p.tmQ);
-    tma_prefetch_desc(&p.tmK);
-    tma_prefetch_desc(&p.tmV);
-  }
-  if (warp == 9 && lane == 0) {
-    mbar_init(bar_q, 1);
-    for (int i = 0; i < kPpStages; ++i) {
-      mbar_init(bar_kfull + 8 * i, 1);
-      mbar_init(bar_kempty + 8 * i, 1);
-      mbar_init(bar_vfull + 8 * i, 1);
-      mbar_init(bar_vempty + 8 * i, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(bar_sfull + 8 * i, 1);
-      mbar_init(bar_pfull + 8 * i, 4);
-      mbar_init(bar_sfree + 8 * i, 4);
-      mbar_init(bar_pvdone + 8 * i, 1);
-    }
-    for (int i = 0; i < 8; ++i) mbar_init(bar_turn + 8 * i, 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();
-  const int n = p.n_kv_tiles;
-  const int dsteps = (p.d + 15) >> 4;
 
   if (warp == 8) {
+    // ------------------------------------------------------------------ TMA producer, converged warp
     if (elect_one()) {
-      mbar_expect_tx(bar_q, 2 * kTileBytes);
-      tma_load_4d(sQ, &p.tmQ, bar_q, 0, head, qt * 256, b);
-      tma_load_4d(sQ + kTileBytes, &p.tmQ, bar_q, 0, head, qt * 256 + 128, b);
+      mbar_expect_tx(bar_q, kQTileBytes * ND);
+#pragma unroll
+      for (int i = 0; i < ND; ++i) tma_load_4d(sQ + i * kQTileBytes, &p.tmQ, bar_q, i * 64, head, qt * 128, b);
     }
     __syncwarp();
     for (int j = 0; j < n; ++j) {
-      const int s = j % kPpStages;
-      const uint32_t ph = (j / kPpStages) & 1;
+      const int s = j % kStages;
+      const uint32_t ph = (j / kStages) & 1;
       mbar_wait(bar_kempty + 8 * s, ph ^ 1u);
       if (elect_one()) {
-        mbar_expect_tx(bar_kfull + 8 * s, kTileBytes);
-        tma_load_4d(sK + s * kTileBytes, &p.tmK, bar_kfull + 8 * s, 0, head, j * 128, b);
+        mbar_expect_tx(bar_kfull + 8 * s, kKVBytes);
+#pragma unroll
+        for (int i = 0; i < ND; ++i)
+          tma_load_4d(sK + s * kKVBytes + i * kKVChunk, &p.tmK, bar_kfull + 8 * s, i * 64, head, j * kKV, b);
       }
       __syncwarp();
       mbar_wait(bar_vempty + 8 * s, ph ^ 1u);
       if (elect_one()) {
-        mbar_expect_tx(bar_vfull + 8 * s, kTileBytes);
-        tma_load_4d(sV + s * kTileBytes, &p.tmV, bar_vfull + 8 * s, 0, head, j * 128, b);
+        mbar_expect_tx(bar_vfull + 8 * s, kKVBytes);
+#pragma unroll
+        for (int i = 0; i < ND; ++i)
+          tma_load_4d(sV + s * kKVBytes + i * kKVChunk, &p.tmV, bar_vfull + 8 * s, i * 64, head, j * kKV, b);
       }
       __syncwarp();
     }
-  } else if (warp == 9) {
-    // ---- S_i(j) = Q_i K(j)^T, issued as soon as the softmax warpgroup has S_i(j-1) in registers: the next scores
-    // are computed while the warpgroup is still exponentiating the current ones
-    const uint32_t idesc_qk = umma_idesc_bf16(128, 128, 0);
-    auto qk = [&](int i, int j) {  // whole warp: S_i(j) = Q_i K(j)^T, then "S_i full"
-      const int s = j % kPpStages;
-      tc_fence_after();
-      stamp(2);
-      if (elect_one()) {
-        for (int k = 0; k < dsteps; ++k)
-          umma_ss(tmem_base + kPpColS + i * 128, umma_desc_sw128(sQ + i * kTileBytes + k * 32),
-                  umma_desc_sw128(sK + s * kTileBytes + k * 32), idesc_qk, k != 0);
-        umma_commit(bar_sfull + 8 * i);
-        if (i == 1) umma_commit(bar_kempty + 8 * s);  // tile 1 is the last reader of K(j)
-      }
-      __syncwarp();
-      stamp(2);
-    };
-    auto kwait = [&](int j) { mbar_wait(bar_kfull + 8 * (j % kPpStages), (j / kPpStages) & 1); };
-    mbar_wait(bar_q, 0);
-    kwait(0);
-    qk(0, 0);
-    qk(1, 0);
-    for (int j = 0; j + 1 < n; ++j) {
-      kwait(j + 1);
-      mbar_wait(bar_sfree, j & 1);
-      qk(0, j + 1);
-      mbar_wait(bar_sfree + 8, j & 1);
-      qk(1, j + 1);
-    }
-  } else if (warp == 10) {
-    // ---- O_i += P_i(j) V(j)
-    const uint32_t idesc_pv = umma_idesc_bf16(128, 64, 1);  // B (= V) is MN-major
-    for (int j = 0; j < n; ++j) {
-      const int s = j % kPpStages;
-      const uint32_t ph = (j / kPpStages) & 1;
-      const int kv_left = p.Skv - j * 128;
-      const int ksteps = kv_left >= 128 ? 8 : (kv_left + 15) >> 4;  // keys beyond Skv contribute nothing
-      mbar_wait(bar_vfull + 8 * s, ph);
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        mbar_wait(bar_pfull + 8 * i, j & 1);
-        tc_fence_after();
-        stamp(3);
-        if (elect_one()) {
-          for (int k = 0; k < ksteps; ++k)
-            umma_ts(tmem_base + kPpColO + i * 64, tmem_base + kPpColP + i * 64 + k * 8,
-                    umma_desc_sw128(sV + s * kTileBytes + k * 2048), idesc_pv, (j | k) != 0);
-          umma_commit(bar_pvdone + 8 * i);
-          if (i == 1) umma_commit(bar_vempty + 8 * s);
-        }
-        __syncwarp();
-        stamp(3);
-      }
-    }
-  } else {
-    const int i = warp >> 2;  // query tile of this warpgroup
-    const int q = warp & 3;   // TMEM lane quarter
-    const int row = q * 32 + lane;
-    const uint32_t tl = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    const uint32_t colS = kPpColS + i * 128, colP = kPpColP + i * 64, colO = kPpColO + i * 64;
-    const uint32_t sfull = bar_sfull + 8 * i, pfull = bar_pfull + 8 * i;
-    const uint32_t sfree = bar_sfree + 8 * i, pvdone = bar_pvdone + 8 * i;
-    const uint32_t my_turn = bar_turn + 8 * (i * 4 + q), partner_turn = bar_turn + 8 * ((i ^ 1) * 4 + q);
-    float m_run = -INFINITY;  // running max, already multiplied by scale*log2e
-    float l_run = 0.f;
-    const bool tr = q == 0;  // traced warps: 0 (tile 0) and 4 (tile 1)
-    for (int j = 0; j < n; ++j) {
-      mbar_wait(sfull, j & 1);
-      tc_fence_after();
-      if (tr) stamp(i);
-      const int kv_left = p.Skv - j * 128;
-      uint32_t v[128];
-#pragma unroll
-      for (int c = 0; c < 4; ++c) tmem_ld_x32(tl + colS + c * 32, v + c * 32);
-      tmem_ld_wait();
-      if (tr) stamp(i);
-      // the scores are in registers: S_i may be overwritten by the next Q_i K^T
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(sfree);
-      bool pv_waited = j == 0;  // P_i(j-1) consumed and O_i complete up to tile j-1?
-      float mx;
-      if (kv_left >= 128) {
-        float m0 = __uint_as_float(v[0]), m1 = __uint_as_float(v[1]), m2 = __uint_as_float(v[2]),
-              m3 = __uint_as_float(v[3]);
-#pragma unroll
-        for (int c = 4; c < 128; c += 4) {
-          m0 = fmaxf(m0, __uint_as_float(v[c]));
-          m1 = fmaxf(m1, __uint_as_float(v[c + 1]));
-          m2 = fmaxf(m2, __uint_as_float(v[c + 2]));
-          m3 = fmaxf(m3, __uint_as_float(v[c + 3]));
-        }
-        mx = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-      } else {
-        mx = -INFINITY;
-#pragma unroll
-        for (int c = 0; c < 128; ++c)
-          if (c < kv_left) mx = fmaxf(mx, __uint_as_float(v[c]));
-      }
-      mx *= p.scale_log2;
-      if (j == 0) {
-        m_run = mx;
-      } else {
-        // lazy rescale: only when the running max grows by more than 2^8
-        const bool need = mx - m_run > 8.f;
-        if (__any_sync(0xffffffffu, need)) {
-          mbar_wait(pvdone, (j - 1) & 1);
-          tc_fence_after();
-          pv_waited = true;
-          float alpha = 1.f;
-          if (need) {
-            alpha = fast_exp2(m_run - mx);
-            m_run = mx;
-          }
-          l_run *= alpha;
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t o[32];
-            tmem_ld_x32(tl + colO + c * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 32; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * alpha);
-            tmem_st_x16(tl + colO + c * 32, o);
-            tmem_st_x16(tl + colO + c * 32 + 16, o + 16);
-          }
-          tmem_st_wait();
-        }
-      }
-      if (tr) stamp(i);
-      // The warps q of the two warpgroups share a sub-partition's MUFU unit (8 clk per warp instruction).  Left alone
-      // they fall into step — both exponentiate at half rate, then both run their ~1 000 non-MUFU cycles with the unit
-      // idle (trace: 3 530 clk per key tile, MUFU 54 % busy) — so the unit is handed over explicitly: a warp starts
-      // its exponentials when its partner has issued its last one, and loads / max / stores run under the partner's.
-      if (p.pp_token && (i == 1 || j > 0)) mbar_wait(my_turn, (i == 1 ? j : j - 1) & 1);
-      float s0 = 0.f, s1 = 0.f;
-      uint64_t acc[2] = {0ull, 0ull};
-      auto store_p = [&](int c, const uint32_t* pk) {
-        if (kTrace && c == 0 && tr) stamp(i);
-        if (!pv_waited) {  // first store of the tile: the previous P_i must have been read by its MMAs
-          mbar_wait(pvdone, (j - 1) & 1);
-          tc_fence_after();
-          pv_waited = true;
-        }
-        if (kTrace && c == 0 && tr) stamp(i);
-        tmem_st_x16(tl + colP + c * 16, pk);
-      };
-      if (kv_left >= 128) {
-        // software pipeline over the four 32-column chunks: the exponentials of chunk c + 1 are in flight while chunk c
-        // is summed, packed and stored (the __syncwarp()s keep ptxas from pulling consumers up behind their producers)
-        exp_issue32<kPoly>(v, p.scale_log2, m_run);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          if (c + 1 < 4) exp_issue32<kPoly>(v + (c + 1) * 32, p.scale_log2, m_run);
-          __syncwarp();
-          uint32_t pk[16];
-          exp_consume32(v + c * 32, pk, acc);
-          store_p(c, pk);
-          __syncwarp();
-        }
-      } else {
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          if (kv_left <= c * 32) continue;  // beyond Skv: the PV MMA never reads these columns (ksteps limit)
-          uint32_t pk[16];
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            float p0 = fast_exp2(fmaf(__uint_as_float(v[c * 32 + 2 * e]), p.scale_log2, -m_run));
-            float p1 = fast_exp2(fmaf(__uint_as_float(v[c * 32 + 2 * e + 1]), p.scale_log2, -m_run));
-            if (c * 32 + 2 * e >= kv_left) p0 = 0.f;
-            if (c * 32 + 2 * e + 1 >= kv_left) p1 = 0.f;
-            s0 += p0;
-            s1 += p1;
-            pk[e] = pack_bf16x2(p0, p1);
-          }
-          store_p(c, pk);
-        }
-      }
-      {
-        float a0, a1, a2, a3;
-        f2_unpack(acc[0], a0, a1);
-        f2_unpack(acc[1], a2, a3);
-        l_run += ((s0 + s1) + (a0 + a1)) + (a2 + a3);  // consumes every exponential of the tile
-      }
-      __syncwarp();
-      if (p.pp_token && lane == 0) mbar_arrive(partner_turn);
-      tmem_st_wait();
-      if (tr) stamp(i);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(pfull);
-    }
-    // ---- finalize: O / l -> bf16 -> global (only the first d columns of the padded head)
-    mbar_wait(pvdone, (n - 1) & 1);
-    tc_fence_after();
-    const float inv = 1.f / l_run;
-    const int srow = qt * 256 + i * 128 + row;
-    if (p.lse != nullptr && srow < p.Sq)
-      p.lse[(static_cast<size_t>(b) * gridDim.y + head) * p.Sq + srow] = m_run + log2f(l_run);
-    __nv_bfloat16* op = p.o + (static_cast<size_t>(b) * p.Sq + srow) * p.ldo + head * p.d;
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      const int col0 = c * 32;
-      if (col0 < p.d) {
-        uint32_t o[32];
-        tmem_ld_x32(tl + colO + col0, o);
-        tmem_ld_wait();
-        if (srow < p.Sq) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            if (col0 + e * 8 < p.d) {
-              uint4 w;
-              w.x = pack_bf16x2(__uint_as_float(o[8 * e + 0]) * inv, __uint_as_float(o[8 * e + 1]) * inv);
-              w.y = pack_bf16x2(__uint_as_float(o[8 * e + 2]) * inv, __uint_as_float(o[8 * e + 3]) * inv);
-              w.z = pack_bf16x2(__uint_as_float(o[8 * e + 4]) * inv, __uint_as_float(o[8 * e + 5]) * inv);
-              w.w = pack_bf16x2(__uint_as_float(o[8 * e + 6]) * inv, __uint_as_float(o[8 * e + 7]) * inv);
-              *reinterpret_cast<uint4*>(op + col0 + e * 8) = w;
-            }
-          }
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  // ------------------------------------------------------------------ consumer warpgroups
+  const int wg = warp >> 2;
+  const bool signal = (threadIdx.x & 127) == 0;
+  const int dsteps = (p.d + 15) >> 4;  // 16-wide k-steps of the Q K^T contraction that hold data
+  const uint32_t sQw = sQ + static_cast<uint32_t>(wg) * 64u * 128u;  // this warpgroup's 64 query rows
+  float o[ND * 32];
+#pragma unroll
+  for (int i = 0; i < ND * 32; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};  // rows lane / 4 and lane / 4 + 8 of the warp's 16
+  mbar_wait(bar_q, 0);
+  for (int j = 0; j < n; ++j) {
+    const int s = j % kStages;
+    const uint32_t ph = (j / kStages) & 1;
+    float sc[kKV / 2];
+    mbar_wait(bar_kfull + 8 * s, ph);
+    wgmma_fence();
+    for (int k = 0; k < dsteps; ++k) {
+      const uint32_t qoff = static_cast<uint32_t>(k >> 2) * kQTileBytes + static_cast<uint32_t>(k & 3) * 32;
+      const uint32_t koff = static_cast<uint32_t>(k >> 2) * kKVChunk + static_cast<uint32_t>(k & 3) * 32;
+      if constexpr (kKV == 128)
+        wgmma_ss_n128(sc, gmma_desc_sw128(sQw + qoff), gmma_desc_sw128(sK + s * kKVBytes + koff), k != 0);
+      else
+        wgmma_ss_n64(sc, gmma_desc_sw128(sQw + qoff), gmma_desc_sw128(sK + s * kKVBytes + koff), k != 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < kKV / 2; ++i) reg_fence(sc[i]);
+    if (signal) mbar_arrive(bar_kempty + 8 * s);
+
+    // ---- online softmax in the log2 domain: x = s * scale * log2(e)
+    const int left = p.Skv - j * kKV;  // valid keys in this tile
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < kKV / 2; ++i) {
+      const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+      sc[i] = col < left ? sc[i] * p.scale_log2 : -INFINITY;
+      mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], sc[i]);
+    }
+    float alpha[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float mn = fmaxf(m[r], mx[r]);  // finite: every tile holds at least one valid key
+      alpha[r] = fast_exp2(m[r] - mn);
+      m[r] = mn;
+      l[r] *= alpha[r];
+    }
+    uint32_t pa[kKV / 16][4];  // P as bf16 A fragments, one group of four registers per 16 keys
+#pragma unroll
+    for (int i = 0; i < kKV / 2; i += 2) {
+      const int r = (i >> 1) & 1;
+      const float p0 = fast_exp2(sc[i] - m[r]), p1 = fast_exp2(sc[i + 1] - m[r]);
+      l[r] += p0 + p1;
+      pa[i >> 3][(i >> 1) & 3] = pack_bf16x2(p0, p1);
+    }
+#pragma unroll
+    for (int i = 0; i < ND * 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+
+    mbar_wait(bar_vfull + 8 * s, ph);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kKV / 16; ++kk) {
+#pragma unroll
+      for (int c = 0; c < ND; ++c)
+        wgmma_rs_n64_tb(o + 32 * c, pa[kk], gmma_desc_sw128(sV + s * kKVBytes + c * kKVChunk + kk * 2048), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < ND * 32; ++i) reg_fence(o[i]);
+    if (signal) mbar_arrive(bar_vempty + 8 * s);
+  }
+
+  // ---- normalise and write O (first d columns of each padded head), log-sum-exp for the backward pass
+  const int wl = warp & 3;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+  }
+  const int heads = gridDim.y;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int q = qt * 128 + wg * 64 + wl * 16 + (lane >> 2) + 8 * r;
+    if (q >= p.Sq) continue;
+    const float inv = 1.f / l[r];
+    __nv_bfloat16* orow = p.o + (static_cast<size_t>(b) * p.Sq + q) * p.ldo + static_cast<size_t>(head) * p.d;
+#pragma unroll
+    for (int c = 0; c < ND; ++c) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int col = c * 64 + 8 * e + 2 * (lane & 3);
+        if (col < p.d) {
+          const int i = 32 * c + 4 * e + 2 * r;
+          *reinterpret_cast<uint32_t*>(orow + col) = pack_bf16x2(o[i] * inv, o[i + 1] * inv);
+        }
+      }
+    }
+    if (p.lse != nullptr && (lane & 3) == 0)
+      p.lse[(static_cast<size_t>(b) * heads + head) * p.Sq + q] = m[r] + __log2f(l[r]);
   }
 }
 
-template <int kPoly>
-static int launch_attention_pp(Ctx* ctx, cudaStream_t stream, const AttnParams& p, dim3 grid) {
+template <int ND>
+static int launch_attention(cudaStream_t stream, const AttnParams& p, dim3 grid) {
   static bool attr_set = false;
   if (!attr_set) {
     SB200_CUDA_CHECK(
-        cudaFuncSetAttribute(attention_pp_kernel<kPoly>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPpSmem));
+        cudaFuncSetAttribute(attention_kernel<ND>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnCfg<ND>::kSmem));
     attr_set = true;
   }
-  SB200_CUDA_CHECK(
-      launch_pdl(attention_pp_kernel<kPoly>, grid, dim3(kPpThreads), static_cast<size_t>(kPpSmem), stream, p));
+  SB200_CUDA_CHECK(launch_pdl(attention_kernel<ND>, grid, dim3(kAttnThreads), AttnCfg<ND>::kSmem, stream, p));
   SB200_CUDA_CHECK(cudaGetLastError());
-  (void)ctx;
   return 0;
-}
-
-template <int ND, int kPoly>
-static int launch_attention(Ctx* ctx, cudaStream_t stream, const AttnParams& p, dim3 grid) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    SB200_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<ND, kPoly>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          AttnCfg<ND>::kSmem));
-    attr_set = true;
-  }
-  SB200_CUDA_CHECK(launch_pdl(attention_kernel<ND, kPoly>, grid, dim3(kAttnThreads), AttnCfg<ND>::kSmem, stream, p));
-  SB200_CUDA_CHECK(cudaGetLastError());
-  (void)ctx;
-  return 0;
-}
-
-// one pair of exponentials in every SB200_ATTN_POLY (0 = none, 8, 4, 2) goes through poly_exp2_x2 (same-box A/B)
-static int attn_poly() {
-  static const int v = [] {
-    const char* e = getenv("SB200_ATTN_POLY");
-    return e ? atoi(e) : 4;  // 25 %: +4.5 % at S = 4096, +1 % at S = 1024; 50 % is slower than none
-  }();
-  return v;
 }
 
 }  // namespace sb200
@@ -905,18 +259,20 @@ extern "C" int sb200_attention(void* handle, void* stream, const void* q, int ld
   SB200_REQUIRE(ldq >= heads * head_dim && ldk >= heads * head_dim && ldv >= heads * head_dim &&
                     ldo >= heads * head_dim,
                 "attention: heads=%d x head_dim=%d exceeds a row", heads, head_dim);
+  const int kv = head_dim <= 64 ? AttnCfg<1>::kKV : AttnCfg<2>::kKV;
   AttnParams p;
   memset(&p, 0, sizeof(p));
   int st;
-  const uint32_t box[4] = {64, 1, 128, 1};
   const uint64_t hs = static_cast<uint64_t>(head_dim) * 2;  // byte stride between heads
   {
+    const uint32_t box[4] = {64, 1, 128, 1};
     const uint64_t dims[4] = {static_cast<uint64_t>(head_dim), static_cast<uint64_t>(heads),
                               static_cast<uint64_t>(Sq), static_cast<uint64_t>(B)};
     const uint64_t strides[3] = {hs, static_cast<uint64_t>(ldq) * 2, static_cast<uint64_t>(ldq) * 2 * Sq};
     if ((st = make_tmap_bf16(ctx, &p.tmQ, q, 4, dims, strides, box))) return st;
   }
   {
+    const uint32_t box[4] = {64, 1, static_cast<uint32_t>(kv), 1};
     const uint64_t dims[4] = {static_cast<uint64_t>(head_dim), static_cast<uint64_t>(heads),
                               static_cast<uint64_t>(Skv), static_cast<uint64_t>(B)};
     const uint64_t sk[3] = {hs, static_cast<uint64_t>(ldk) * 2, static_cast<uint64_t>(ldk) * 2 * Skv};
@@ -930,89 +286,12 @@ extern "C" int sb200_attention(void* handle, void* stream, const void* q, int ld
   p.Sq = Sq;
   p.Skv = Skv;
   p.d = head_dim;
-  p.n_kv_tiles = (Skv + 127) / 128;
-  {
-    static const bool split = [] {
-      const char* e = getenv("SB200_ATTN_SPLIT");  // "0" = single issuing warp (same-box A/B)
-      return !(e && e[0] == '0');
-    }();
-    p.split_issue = split ? 1 : 0;
-    static const bool token = [] {
-      const char* e = getenv("SB200_ATTN_TOKEN");
-      return e && e[0] == '1';
-    }();
-    p.pp_token = token ? 1 : 0;
-    static const bool split_exp = [] {
-      const char* e = getenv("SB200_ATTN_SPLIT_EXP");
-      return e && e[0] == '1';
-    }();
-    p.split_exp = split_exp ? 1 : 0;
-  }
+  p.n_kv_tiles = (Skv + kv - 1) / kv;
   p.scale_log2 = scale * 1.4426950408889634f;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  {
-    // ping-pong kernel (two query tiles per CTA), opt-in with SB200_ATTN_PP=1: equal to the two-CTA kernel at
-    // S = 4096 x 8 passes (676 vs 672 TFLOP/s with the same polynomial share) and behind it on shorter sequences and
-    // smaller batches (457 vs 499 at S = 1024, 492 vs 547 at 2 passes): profiles/r02_attention_experiments.md
-    static const bool pp = [] {
-      const char* e = getenv("SB200_ATTN_PP");
-      return e && e[0] == '1';
-    }();
-    if (pp && head_dim <= 64 && p.n_kv_tiles >= 4 && Sq > 128) {
-      dim3 grid2((Sq + 255) / 256, heads, B);
-      pdl_hint() = static_cast<long long>(grid2.x) * grid2.y * grid2.z <= 2LL * ctx->num_sms;
-      switch (attn_poly()) {
-        case 1: return launch_attention_pp<1>(ctx, s, p, grid2);  // phase-trace build
-        case 8: return launch_attention_pp<8>(ctx, s, p, grid2);
-        case 4: return launch_attention_pp<4>(ctx, s, p, grid2);
-        case 2: return launch_attention_pp<2>(ctx, s, p, grid2);
-        default: return launch_attention_pp<0>(ctx, s, p, grid2);
-      }
-    }
-  }
-  // Short key sequences (cross-attention: one key tile): a CTA's fixed cost (launch, TMEM allocation, Q / K / V load
-  // latency, output drain) is several times the work of one 128-query tile, so one CTA walks several consecutive query
-  // tiles of its (batch, head) — the next Q and K / V arrive while the current tile is in the softmax.  The smallest
-  // divisor of the tile count that brings the grid under two CTAs per SM.  Opt-in (SB200_ATTN_QLOOP=1): measured
-  // 31.5 -> 35.3 us (S = 1024, 8 passes), 57.4 -> 68.2 (S = 4096), 43.4 -> 36.6 (d = 40): with single S / P / O
-  // buffers the tiles of one CTA run strictly one after the other (~4.4 us each), and one CTA per SM has nothing to
-  // overlap with, whereas 4.3 waves of independent CTAs, two per SM, hide each other's latencies.
-  const int nq_tiles = (Sq + 127) / 128;
-  p.q_per_cta = 1;
-  {
-    static const bool qloop = [] {
-      const char* e = getenv("SB200_ATTN_QLOOP");
-      return e && e[0] == '1';
-    }();
-    if (qloop && p.split_issue && p.n_kv_tiles == 1 && nq_tiles > 1) {
-      const long long slots = 2LL * ctx->num_sms;
-      int d = nq_tiles;
-      for (int c = 1; c <= nq_tiles; ++c)
-        if (nq_tiles % c == 0 && static_cast<long long>(nq_tiles / c) * heads * B <= slots) {
-          d = c;
-          break;
-        }
-      p.q_per_cta = d;
-    }
-  }
-  dim3 grid((nq_tiles + p.q_per_cta - 1) / p.q_per_cta, heads, B);
-  pdl_hint() = static_cast<long long>(grid.x) * grid.y * grid.z <= 4LL * ctx->num_sms;
-  if (head_dim <= 64) {
-    switch (attn_poly()) {
-      case 8: return launch_attention<1, 8>(ctx, s, p, grid);
-      case 4: return launch_attention<1, 4>(ctx, s, p, grid);
-      case 2: return launch_attention<1, 2>(ctx, s, p, grid);
-      default: return launch_attention<1, 0>(ctx, s, p, grid);
-    }
-  }
-  // wider heads: twice / three times the tensor work per exponential, MUFU is not the bound
-  if (head_dim <= 128) return launch_attention<2, 0>(ctx, s, p, grid);
-  return launch_attention<3, 0>(ctx, s, p, grid);
-}
-
-extern "C" int sb200_debug_attention_trace(long long* dst, int n) {
-  SB200_REQUIRE(dst && n > 0 && n <= 4 * kPpTraceLen, "attention trace: bad arguments");
-  SB200_CUDA_CHECK(cudaDeviceSynchronize());
-  SB200_CUDA_CHECK(cudaMemcpyFromSymbol(dst, g_pp_trace, sizeof(long long) * n));
-  return 0;
+  dim3 grid((Sq + 127) / 128, heads, B);
+  pdl_hint() = static_cast<long long>(grid.x) * grid.y * grid.z <= 2LL * ctx->num_sms;
+  if (head_dim <= 64) return launch_attention<1>(s, p, grid);
+  if (head_dim <= 128) return launch_attention<2>(s, p, grid);
+  return launch_attention<3>(s, p, grid);
 }

@@ -1,53 +1,49 @@
-// Flash-attention backward for sm_100a (tcgen05 + TMEM + TMA), the gradient path of
+// Flash-attention backward for sm_90a (wgmma + TMA), the gradient path of
 //   loss.backward()  (trainscripts/textsliders/train_lora_xl.py:345; train_lora-scale-xl.py:340,372)
 // through diffusers' Attention (xformers memory_efficient_attention backward in the reference).
 //
 // With S = scale * Q K^T, P = softmax(S), O = P V and D[q] = sum_d dO[q,d] O[q,d]:
 //   dV = P^T dO          dP = dO V^T          dS = P o (dP - D)          dQ = scale dS K      dK = scale dS^T Q
-// One kernel template, two roles (each CTA keeps a 128-row "resident" pair of tiles and streams 64-row tiles):
-//   mode 0 (dQ)      resident R1 = Q tile, R2 = dO tile   streamed T1 = K_j, T2 = V_j      out1 = dQ
-//   mode 1 (dK, dV)  resident R1 = K tile, R2 = V tile    streamed T1 = Q_i, T2 = dO_i     out1 = dV, out2 = dK
-// so that in both modes
-//   S'  = R1 T1^T   (SS UMMA 128x64xd, fp32 in TMEM columns [0,64))
-//   dP' = R2 T2^T   (SS UMMA,          TMEM columns [64,128))
-//   every thread of the 4 compute warps owns one resident row: p = exp2(s*scale*log2e - lse), ds = p (dp - D) scale,
-//   written back IN PLACE as bf16 (P over S', dS over dP'), then consumed as the A operand of TS UMMAs:
-//   mode 0: dQ += dS K_j;  mode 1: dV += P^T dO_i, dK += dS^T Q_i   (B operand = the streamed tile, MN-major).
-// The log-sum-exp comes from the forward kernel (attention.cu, `lse`), D from attn_bwd_prep_kernel.  Mode 1 reads
-// lse / D per streamed column (staged in shared memory), mode 0 per resident row.
-// Head dim padded to ND x 64 columns by TMA zero fill as in the forward.  TMEM: 128 + 64 ND (mode 0) or
-// 128 + 128 ND (mode 1) columns -> for ND = 1 two CTAs share an SM so one CTA's MMAs overlap the other's softmax math.
-// Deterministic: no atomics (dQ and dK/dV come from separate launches, each output tile has one owner CTA).
+// One kernel template, three launches.  Each CTA keeps a 128-row "resident" pair of tiles (64 rows per consumer
+// warpgroup) and streams kT-row tiles:
+//   mode 0 (dQ)  resident R1 = Q, R2 = dO   streamed T1 = K_j, T2 = V_j    out = dQ += dS T1
+//   mode 1 (dV)  resident R1 = K            streamed T1 = Q_i, T2 = dO_i   out = dV += P^T T2
+//   mode 2 (dK)  resident R1 = K, R2 = V    streamed T1 = Q_i, T2 = dO_i   out = dK += dS^T T1
+// so that in every mode
+//   S'  = R1 T1^T   and   dP' = R2 T2^T   (wgmma m64 x kT x 16 from shared memory, fp32 in registers)
+//   p = exp2(s * scale * log2e - lse), ds = p (dp - D) scale, packed to bf16 in place as the A operand of
+//   out += {P | dS} . T   (wgmma m64 x 64 x 16 per 64 head columns, A from registers, the streamed tile MN-major).
+// dV and dK come from separate launches so that one accumulator holds the registers of a thread.
+// The log-sum-exp comes from the forward kernel (attention.cu, `lse`), D from attn_bwd_prep_kernel.  Modes 1 / 2 read
+// lse / D per streamed column, mode 0 per resident row.  Head dim padded to ND x 64 columns by TMA zero fill as in
+// the forward.  Deterministic: no atomics (each output tile has one owner CTA).
 #include "common.h"
 #include "ptx.cuh"
 
 namespace sb200 {
 
-constexpr int kBwdThreads = 192;
+constexpr int kBwdThreads = 288;        // two consumer warpgroups + the TMA warp
 constexpr uint32_t kRTile = 128 * 128;  // 128 rows x 64 bf16, SWIZZLE_128B
-constexpr uint32_t kTTile = 64 * 128;   // 64 rows x 64 bf16
-constexpr uint32_t kBColS = 0, kBColDP = 64, kBColOut = 128;
 
 template <int ND>
 struct AttnBwdCfg {
+  static constexpr int kT = ND == 3 ? 32 : 64;  // streamed rows per tile (the output accumulator takes the registers)
   static constexpr int kStages = 2;
+  static constexpr uint32_t kTChunk = kT * 128;  // 64 head columns of a streamed tile
   static constexpr uint32_t kRBytes = kRTile * ND;
-  static constexpr uint32_t kTBytes = kTTile * ND;
-  static constexpr int kSmem = 2 * kRBytes + kStages * 2 * kTBytes + 2048 /*barriers + stats*/ + 1024 /*align*/;
-  static constexpr int kTmemCols = ND == 1 ? 256 : 512;
-  static constexpr int kMinBlocks = ND == 1 ? 2 : 1;
+  static constexpr uint32_t kTBytes = kTChunk * ND;
+  static constexpr int kSmem = 2 * kRBytes + kStages * 2 * kTBytes + 1024 /*barriers*/ + 1024 /*align*/;
 };
 
 struct AttnBwdParams {
   CUtensorMap tmR1, tmR2, tmT1, tmT2;
-  __nv_bfloat16* out1;
-  __nv_bfloat16* out2;
-  int ld1, ld2;
+  __nv_bfloat16* out;
+  int ld;
   const float* lse;   // [B, heads, Sq]
   const float* dsum;  // [B, heads, Sq]
   int Sq;
-  int n_res;     // valid resident rows in total (mode 0: Sq, mode 1: Skv)
-  int n_stream;  // valid streamed rows in total (mode 0: Skv, mode 1: Sq)
+  int n_res;     // valid resident rows in total (mode 0: Sq, modes 1 / 2: Skv)
+  int n_stream;  // valid streamed rows in total (mode 0: Skv, modes 1 / 2: Sq)
   int d;
   int mode;
   float scale_log2, scale;
@@ -59,35 +55,40 @@ __device__ __forceinline__ float bwd_exp2(float x) {
   return y;
 }
 
+template <int kN>
+__device__ __forceinline__ void wgmma_ss_t(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  if constexpr (kN == 64)
+    wgmma_ss_n64(d, a, b, acc);
+  else
+    wgmma_ss_n32(d, a, b, acc);
+}
+
 template <int ND>
-__global__ void __launch_bounds__(kBwdThreads, AttnBwdCfg<ND>::kMinBlocks)
-    attention_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
+__global__ void __launch_bounds__(kBwdThreads, 1) attention_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
+  constexpr int kT = AttnBwdCfg<ND>::kT;
   constexpr int kStages = AttnBwdCfg<ND>::kStages;
   constexpr uint32_t kRBytes = AttnBwdCfg<ND>::kRBytes;
   constexpr uint32_t kTBytes = AttnBwdCfg<ND>::kTBytes;
+  constexpr uint32_t kTChunk = AttnBwdCfg<ND>::kTChunk;
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t base = (raw_addr + 1023u) & ~1023u;
-  uint8_t* smem = smem_raw + (base - raw_addr);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int rt = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
+  const int mode = p.mode;
+  const bool need_dp = mode != 1;
 
   const uint32_t sR1 = base;
   const uint32_t sR2 = sR1 + kRBytes;
-  const uint32_t sT1 = sR2 + kRBytes;               // kStages x kTBytes
-  const uint32_t sT2 = sT1 + kStages * kTBytes;     // kStages x kTBytes
+  const uint32_t sT1 = sR2 + kRBytes;            // kStages x kTBytes
+  const uint32_t sT2 = sT1 + kStages * kTBytes;  // kStages x kTBytes
   const uint32_t bars = sT2 + kStages * kTBytes;
   const uint32_t bar_r = bars;
-  const uint32_t bar_full = bars + 8;                // kStages
+  const uint32_t bar_full = bars + 8;  // kStages
   const uint32_t bar_empty = bar_full + 8 * kStages;
-  const uint32_t bar_s = bar_empty + 8 * kStages;    // S', dP' complete
-  const uint32_t bar_p = bar_s + 8;                  // P / dS written (4 warps)
-  const uint32_t bar_done = bar_p + 8;               // TS MMAs of this tile complete
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + (bars - base) + 64);
-  float* stat_sh = reinterpret_cast<float*>(smem + (bars - base) + 128);  // [2 buffers][2 (lse, D)][64]
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tmR1);
@@ -99,33 +100,23 @@ __global__ void __launch_bounds__(kBwdThreads, AttnBwdCfg<ND>::kMinBlocks)
     mbar_init(bar_r, 1);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(bar_full + 8 * i, 1);
-      mbar_init(bar_empty + 8 * i, 1);
+      mbar_init(bar_empty + 8 * i, 2);  // one arrival per consumer warpgroup
     }
-    mbar_init(bar_s, 1);
-    mbar_init(bar_p, 4);
-    mbar_init(bar_done, 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), AttnBwdCfg<ND>::kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
-  const int n = (p.n_stream + 63) >> 6;
-  const int dsteps = (p.d + 15) >> 4;
+  const int n = (p.n_stream + kT - 1) / kT;
   const size_t stat_base = (static_cast<size_t>(b) * gridDim.y + head) * p.Sq;
 
-  if (warp == 0) {
+  if (warp == 8) {
+    // ------------------------------------------------------------------ TMA producer, converged warp
     if (elect_one()) {
-      mbar_expect_tx(bar_r, 2 * kRBytes);
+      mbar_expect_tx(bar_r, need_dp ? 2 * kRBytes : kRBytes);
 #pragma unroll
       for (int i = 0; i < ND; ++i) {
         tma_load_4d(sR1 + i * kRTile, &p.tmR1, bar_r, i * 64, head, rt * 128, b);
-        tma_load_4d(sR2 + i * kRTile, &p.tmR2, bar_r, i * 64, head, rt * 128, b);
+        if (need_dp) tma_load_4d(sR2 + i * kRTile, &p.tmR2, bar_r, i * 64, head, rt * 128, b);
       }
     }
     __syncwarp();
@@ -137,170 +128,125 @@ __global__ void __launch_bounds__(kBwdThreads, AttnBwdCfg<ND>::kMinBlocks)
         mbar_expect_tx(bar_full + 8 * s, 2 * kTBytes);
 #pragma unroll
         for (int i = 0; i < ND; ++i) {
-          tma_load_4d(sT1 + s * kTBytes + i * kTTile, &p.tmT1, bar_full + 8 * s, i * 64, head, t * 64, b);
-          tma_load_4d(sT2 + s * kTBytes + i * kTTile, &p.tmT2, bar_full + 8 * s, i * 64, head, t * 64, b);
+          tma_load_4d(sT1 + s * kTBytes + i * kTChunk, &p.tmT1, bar_full + 8 * s, i * 64, head, t * kT, b);
+          tma_load_4d(sT2 + s * kTBytes + i * kTChunk, &p.tmT2, bar_full + 8 * s, i * 64, head, t * kT, b);
         }
       }
       __syncwarp();
     }
-  } else if (warp == 1) {
-    const uint32_t idesc_ss = umma_idesc_bf16(128, 64, 0);
-    const uint32_t idesc_ts = umma_idesc_bf16(128, 64, 1);  // B (streamed tile) MN-major
-    mbar_wait(bar_r, 0);
-    for (int t = 0; t < n; ++t) {
-      const int s = t % kStages;
-      const uint32_t ph = (t / kStages) & 1;
-      mbar_wait(bar_full + 8 * s, ph);
-      tc_fence_after();
-      if (elect_one()) {
-        for (int k = 0; k < dsteps; ++k) {
-          const uint32_t ro = static_cast<uint32_t>(k >> 2) * kRTile + static_cast<uint32_t>(k & 3) * 32;
-          const uint32_t to = static_cast<uint32_t>(k >> 2) * kTTile + static_cast<uint32_t>(k & 3) * 32;
-          umma_ss(tmem_base + kBColS, umma_desc_sw128(sR1 + ro), umma_desc_sw128(sT1 + s * kTBytes + to), idesc_ss,
-                  k != 0);
-        }
-        for (int k = 0; k < dsteps; ++k) {
-          const uint32_t ro = static_cast<uint32_t>(k >> 2) * kRTile + static_cast<uint32_t>(k & 3) * 32;
-          const uint32_t to = static_cast<uint32_t>(k >> 2) * kTTile + static_cast<uint32_t>(k & 3) * 32;
-          umma_ss(tmem_base + kBColDP, umma_desc_sw128(sR2 + ro), umma_desc_sw128(sT2 + s * kTBytes + to), idesc_ss,
-                  k != 0);
-        }
-        umma_commit(bar_s);
-      }
-      __syncwarp();
-      mbar_wait(bar_p, t & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const int left = p.n_stream - t * 64;
-        const int ksteps = left >= 64 ? 4 : (left + 15) >> 4;  // streamed rows beyond the end contribute nothing
-        for (int k = 0; k < ksteps; ++k) {
+    return;
+  }
+
+  // ------------------------------------------------------------------ consumer warpgroups
+  const int wg = warp >> 2, wl = warp & 3;
+  const bool signal = (threadIdx.x & 127) == 0;
+  const int dsteps = (p.d + 15) >> 4;
+  const uint32_t roff = static_cast<uint32_t>(wg) * 64u * 128u;  // this warpgroup's 64 resident rows
+  const int row0 = rt * 128 + wg * 64 + wl * 16 + (lane >> 2);   // resident rows row0 and row0 + 8 of this thread
+  float lse_r[2] = {INFINITY, INFINITY}, d_r[2] = {0.f, 0.f};
+  if (mode == 0) {
 #pragma unroll
-          for (int i = 0; i < ND; ++i) {
-            if (p.mode == 1) {
-              umma_ts(tmem_base + kBColOut + i * 64, tmem_base + kBColS + k * 8,
-                      umma_desc_sw128(sT2 + s * kTBytes + i * kTTile + k * 2048), idesc_ts, (t | k) != 0);
-              umma_ts(tmem_base + kBColOut + (ND + i) * 64, tmem_base + kBColDP + k * 8,
-                      umma_desc_sw128(sT1 + s * kTBytes + i * kTTile + k * 2048), idesc_ts, (t | k) != 0);
-            } else {
-              umma_ts(tmem_base + kBColOut + i * 64, tmem_base + kBColDP + k * 8,
-                      umma_desc_sw128(sT1 + s * kTBytes + i * kTTile + k * 2048), idesc_ts, (t | k) != 0);
-            }
-          }
-        }
-        umma_commit(bar_empty + 8 * s);
-        umma_commit(bar_done);
-      }
-      __syncwarp();
-      // P / dS live in the S' / dP' columns: the next tile's SS MMAs may only start once these TS MMAs have read them
-      mbar_wait(bar_done, t & 1);
-    }
-  } else {
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const int ct = threadIdx.x - 64;  // 0..127 among the compute threads
-    const uint32_t tl = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    const int grow = rt * 128 + row;
-    float lse_r = INFINITY, d_r = 0.f;
-    if (p.mode == 0 && grow < p.n_res) {
-      lse_r = __ldg(p.lse + stat_base + grow);
-      d_r = __ldg(p.dsum + stat_base + grow);
-    }
-    for (int t = 0; t < n; ++t) {
-      const int left = p.n_stream - t * 64;
-      float* st = stat_sh + (t & 1) * 128;
-      if (p.mode == 1) {
-        // stage lse / D of the 64 streamed query columns (threads 0..63: lse, 64..127: D)
-        const int c = ct & 63;
-        const int gq = t * 64 + c;
-        float v;
-        if (ct < 64)
-          v = gq < p.n_stream ? __ldg(p.lse + stat_base + gq) : INFINITY;
-        else
-          v = gq < p.n_stream ? __ldg(p.dsum + stat_base + gq) : 0.f;
-        st[ct] = v;
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-      }
-      mbar_wait(bar_s, t & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t sv[32], dv[32];
-        tmem_ld_x32(tl + kBColS + c * 32, sv);
-        tmem_ld_x32(tl + kBColDP + c * 32, dv);
-        tmem_ld_wait();
-        uint32_t pk[16], dk[16];
-        if (p.mode == 1) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 l4 = *reinterpret_cast<const float4*>(st + c * 32 + 4 * i);
-            const float4 d4 = *reinterpret_cast<const float4*>(st + 64 + c * 32 + 4 * i);
-            const float p0 = bwd_exp2(fmaf(__uint_as_float(sv[4 * i + 0]), p.scale_log2, -l4.x));
-            const float p1 = bwd_exp2(fmaf(__uint_as_float(sv[4 * i + 1]), p.scale_log2, -l4.y));
-            const float p2 = bwd_exp2(fmaf(__uint_as_float(sv[4 * i + 2]), p.scale_log2, -l4.z));
-            const float p3 = bwd_exp2(fmaf(__uint_as_float(sv[4 * i + 3]), p.scale_log2, -l4.w));
-            pk[2 * i] = pack_bf16x2(p0, p1);
-            pk[2 * i + 1] = pack_bf16x2(p2, p3);
-            dk[2 * i] = pack_bf16x2(p0 * (__uint_as_float(dv[4 * i + 0]) - d4.x) * p.scale,
-                                    p1 * (__uint_as_float(dv[4 * i + 1]) - d4.y) * p.scale);
-            dk[2 * i + 1] = pack_bf16x2(p2 * (__uint_as_float(dv[4 * i + 2]) - d4.z) * p.scale,
-                                        p3 * (__uint_as_float(dv[4 * i + 3]) - d4.w) * p.scale);
-          }
-          tmem_st_x16(tl + kBColS + c * 16, pk);
-          tmem_st_x16(tl + kBColDP + c * 16, dk);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float p0 = bwd_exp2(fmaf(__uint_as_float(sv[2 * i]), p.scale_log2, -lse_r));
-            float p1 = bwd_exp2(fmaf(__uint_as_float(sv[2 * i + 1]), p.scale_log2, -lse_r));
-            if (c * 32 + 2 * i >= left) p0 = 0.f;      // keys beyond Skv
-            if (c * 32 + 2 * i + 1 >= left) p1 = 0.f;
-            dk[i] = pack_bf16x2(p0 * (__uint_as_float(dv[2 * i]) - d_r) * p.scale,
-                                p1 * (__uint_as_float(dv[2 * i + 1]) - d_r) * p.scale);
-          }
-          tmem_st_x16(tl + kBColDP + c * 16, dk);
-        }
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p);
-    }
-    // ---- write the accumulators (first d columns of each padded head)
-    mbar_wait(bar_done, (n - 1) & 1);
-    tc_fence_after();
-    const int nout = p.mode == 1 ? 2 : 1;
-    for (int o = 0; o < nout; ++o) {
-      __nv_bfloat16* op = (o == 0 ? p.out1 : p.out2) +
-                          (static_cast<size_t>(b) * p.n_res + grow) * (o == 0 ? p.ld1 : p.ld2) + head * p.d;
-#pragma unroll
-      for (int c = 0; c < 2 * ND; ++c) {
-        if (c * 32 < p.d) {  // warp-uniform
-          uint32_t a[32];
-          tmem_ld_x32(tl + kBColOut + o * ND * 64 + c * 32, a);
-          tmem_ld_wait();
-          if (grow < p.n_res) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              if (c * 32 + i * 8 < p.d) {
-                uint4 w;
-                w.x = pack_bf16x2(__uint_as_float(a[8 * i + 0]), __uint_as_float(a[8 * i + 1]));
-                w.y = pack_bf16x2(__uint_as_float(a[8 * i + 2]), __uint_as_float(a[8 * i + 3]));
-                w.z = pack_bf16x2(__uint_as_float(a[8 * i + 4]), __uint_as_float(a[8 * i + 5]));
-                w.w = pack_bf16x2(__uint_as_float(a[8 * i + 6]), __uint_as_float(a[8 * i + 7]));
-                *reinterpret_cast<uint4*>(op + c * 32 + i * 8) = w;
-              }
-            }
-          }
-        }
+    for (int r = 0; r < 2; ++r) {
+      if (row0 + 8 * r < p.n_res) {
+        lse_r[r] = __ldg(p.lse + stat_base + row0 + 8 * r);
+        d_r[r] = __ldg(p.dsum + stat_base + row0 + 8 * r);
       }
     }
   }
+  float acc[ND * 32];
+#pragma unroll
+  for (int i = 0; i < ND * 32; ++i) acc[i] = 0.f;
+  mbar_wait(bar_r, 0);
+  for (int t = 0; t < n; ++t) {
+    const int s = t % kStages;
+    const uint32_t ph = (t / kStages) & 1;
+    const int left = p.n_stream - t * kT;  // valid streamed rows in this tile
+    // per-column statistics of the streamed queries (modes 1 / 2): columns 8 e + 2 (lane % 4) + {0, 1}
+    float lse_c[kT / 4], d_c[kT / 4];
+    if (mode != 0) {
+#pragma unroll
+      for (int e = 0; e < kT / 8; ++e)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int col = 8 * e + 2 * (lane & 3) + h;
+          lse_c[2 * e + h] = col < left ? __ldg(p.lse + stat_base + t * kT + col) : INFINITY;
+          d_c[2 * e + h] = col < left ? __ldg(p.dsum + stat_base + t * kT + col) : 0.f;
+        }
+    }
+    float sc[kT / 2], dp[kT / 2];
+    mbar_wait(bar_full + 8 * s, ph);
+    wgmma_fence();
+    for (int k = 0; k < dsteps; ++k) {
+      const uint32_t ro = static_cast<uint32_t>(k >> 2) * kRTile + roff + static_cast<uint32_t>(k & 3) * 32;
+      const uint32_t to = static_cast<uint32_t>(k >> 2) * kTChunk + static_cast<uint32_t>(k & 3) * 32;
+      wgmma_ss_t<kT>(sc, gmma_desc_sw128(sR1 + ro), gmma_desc_sw128(sT1 + s * kTBytes + to), k != 0);
+    }
+    if (need_dp) {
+      for (int k = 0; k < dsteps; ++k) {
+        const uint32_t ro = static_cast<uint32_t>(k >> 2) * kRTile + roff + static_cast<uint32_t>(k & 3) * 32;
+        const uint32_t to = static_cast<uint32_t>(k >> 2) * kTChunk + static_cast<uint32_t>(k & 3) * 32;
+        wgmma_ss_t<kT>(dp, gmma_desc_sw128(sR2 + ro), gmma_desc_sw128(sT2 + s * kTBytes + to), k != 0);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < kT / 2; ++i) {
+      reg_fence(sc[i]);
+      reg_fence(dp[i]);
+    }
+    uint32_t pa[kT / 16][4];  // P (mode 1) or dS as bf16 A fragments, one group of four registers per 16 streamed rows
+#pragma unroll
+    for (int i = 0; i < kT / 2; i += 2) {
+      const int r = (i >> 1) & 1;
+      const int cp = 2 * (i >> 2);  // index of this pair's first column in lse_c / d_c
+      float v[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int col = 8 * (i >> 2) + 2 * (lane & 3) + h;
+        float pv, dv;
+        if (mode == 0) {
+          pv = col < left ? bwd_exp2(fmaf(sc[i + h], p.scale_log2, -lse_r[r])) : 0.f;  // keys beyond Skv
+          dv = d_r[r];
+        } else {
+          pv = bwd_exp2(fmaf(sc[i + h], p.scale_log2, -lse_c[cp + h]));  // lse = inf beyond Sq: p = 0
+          dv = d_c[cp + h];
+        }
+        v[h] = mode == 1 ? pv : pv * (dp[i + h] - dv) * p.scale;
+      }
+      pa[i >> 3][(i >> 1) & 3] = pack_bf16x2(v[0], v[1]);
+    }
+    const uint32_t sB = (mode == 1 ? sT2 : sT1) + s * kTBytes;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kT / 16; ++kk) {
+#pragma unroll
+      for (int c = 0; c < ND; ++c) wgmma_rs_n64_tb(acc + 32 * c, pa[kk], gmma_desc_sw128(sB + c * kTChunk + kk * 2048), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < ND * 32; ++i) reg_fence(acc[i]);
+    if (signal) mbar_arrive(bar_empty + 8 * s);
+  }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, AttnBwdCfg<ND>::kTmemCols);
+  // ---- write the accumulator (first d columns of each padded head)
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int grow = row0 + 8 * r;
+    if (grow >= p.n_res) continue;
+    __nv_bfloat16* op = p.out + (static_cast<size_t>(b) * p.n_res + grow) * p.ld + static_cast<size_t>(head) * p.d;
+#pragma unroll
+    for (int c = 0; c < ND; ++c) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int col = c * 64 + 8 * e + 2 * (lane & 3);
+        if (col < p.d) {
+          const int i = 32 * c + 4 * e + 2 * r;
+          *reinterpret_cast<uint32_t*>(op + col) = pack_bf16x2(acc[i], acc[i + 1]);
+        }
+      }
+    }
   }
 }
 
@@ -341,6 +287,16 @@ static int launch_attention_bwd(cudaStream_t stream, const AttnBwdParams& p, dim
   SB200_CUDA_CHECK(launch_pdl(attention_bwd_kernel<ND>, grid, dim3(kBwdThreads), AttnBwdCfg<ND>::kSmem, stream, p));
   SB200_CUDA_CHECK(cudaGetLastError());
   return 0;
+}
+
+static int launch_attention_bwd_d(cudaStream_t stream, const AttnBwdParams& p, dim3 grid) {
+  if (p.d <= 64) return launch_attention_bwd<1>(stream, p, grid);
+  if (p.d <= 128) return launch_attention_bwd<2>(stream, p, grid);
+  return launch_attention_bwd<3>(stream, p, grid);
+}
+
+static int streamed_rows(int head_dim) {
+  return head_dim <= 64 ? AttnBwdCfg<1>::kT : (head_dim <= 128 ? AttnBwdCfg<2>::kT : AttnBwdCfg<3>::kT);
 }
 
 static int make_map(Ctx* ctx, CUtensorMap* m, const void* ptr, int ld, int d, int heads, int S, int B, uint32_t rows) {
@@ -388,38 +344,32 @@ extern "C" int sb200_attention_bwd(void* handle, void* stream, const void* q, in
   p.d = head_dim;
   p.scale = scale;
   p.scale_log2 = scale * 1.4426950408889634f;
+  const uint32_t trows = static_cast<uint32_t>(streamed_rows(head_dim));
   // ---- dQ: resident (Q, dO) tiles, streamed (K, V)
   p.mode = 0;
   p.n_res = Sq;
   p.n_stream = Skv;
-  p.out1 = static_cast<__nv_bfloat16*>(dq);
-  p.ld1 = lddq;
+  p.out = static_cast<__nv_bfloat16*>(dq);
+  p.ld = lddq;
   if ((st = make_map(ctx, &p.tmR1, q, ldq, head_dim, heads, Sq, B, 128))) return st;
   if ((st = make_map(ctx, &p.tmR2, dout, lddo, head_dim, heads, Sq, B, 128))) return st;
-  if ((st = make_map(ctx, &p.tmT1, k, ldk, head_dim, heads, Skv, B, 64))) return st;
-  if ((st = make_map(ctx, &p.tmT2, v, ldv, head_dim, heads, Skv, B, 64))) return st;
-  dim3 gq((Sq + 127) / 128, heads, B);
-  if (head_dim <= 64)
-    st = launch_attention_bwd<1>(s, p, gq);
-  else if (head_dim <= 128)
-    st = launch_attention_bwd<2>(s, p, gq);
-  else
-    st = launch_attention_bwd<3>(s, p, gq);
-  if (st || !dk) return st;
-  // ---- dK, dV: resident (K, V) tiles, streamed (Q, dO)
-  p.mode = 1;
+  if ((st = make_map(ctx, &p.tmT1, k, ldk, head_dim, heads, Skv, B, trows))) return st;
+  if ((st = make_map(ctx, &p.tmT2, v, ldv, head_dim, heads, Skv, B, trows))) return st;
+  if ((st = launch_attention_bwd_d(s, p, dim3((Sq + 127) / 128, heads, B))) || !dk) return st;
+  // ---- dV, then dK: resident (K, V) tiles, streamed (Q, dO)
   p.n_res = Skv;
   p.n_stream = Sq;
-  p.out1 = static_cast<__nv_bfloat16*>(dv);
-  p.ld1 = lddv;
-  p.out2 = static_cast<__nv_bfloat16*>(dk);
-  p.ld2 = lddk;
   if ((st = make_map(ctx, &p.tmR1, k, ldk, head_dim, heads, Skv, B, 128))) return st;
   if ((st = make_map(ctx, &p.tmR2, v, ldv, head_dim, heads, Skv, B, 128))) return st;
-  if ((st = make_map(ctx, &p.tmT1, q, ldq, head_dim, heads, Sq, B, 64))) return st;
-  if ((st = make_map(ctx, &p.tmT2, dout, lddo, head_dim, heads, Sq, B, 64))) return st;
-  dim3 gk((Skv + 127) / 128, heads, B);
-  if (head_dim <= 64) return launch_attention_bwd<1>(s, p, gk);
-  if (head_dim <= 128) return launch_attention_bwd<2>(s, p, gk);
-  return launch_attention_bwd<3>(s, p, gk);
+  if ((st = make_map(ctx, &p.tmT1, q, ldq, head_dim, heads, Sq, B, trows))) return st;
+  if ((st = make_map(ctx, &p.tmT2, dout, lddo, head_dim, heads, Sq, B, trows))) return st;
+  const dim3 gk((Skv + 127) / 128, heads, B);
+  p.mode = 1;
+  p.out = static_cast<__nv_bfloat16*>(dv);
+  p.ld = lddv;
+  if ((st = launch_attention_bwd_d(s, p, gk))) return st;
+  p.mode = 2;
+  p.out = static_cast<__nv_bfloat16*>(dk);
+  p.ld = lddk;
+  return launch_attention_bwd_d(s, p, gk);
 }

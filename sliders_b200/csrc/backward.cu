@@ -995,7 +995,7 @@ extern "C" int sb200_lora_proj(void* handle, void* stream, const void* A, int ld
 
 static int wgrad_chunks(Ctx* ctx, int rows, int cblocks, int* rows_per_block) {
   (void)ctx;
-  int chunks = (296 + cblocks - 1) / cblocks;  // fixed (not num_sms-derived) so callers can size `ws`: see sb200.h
+  int chunks = (264 + cblocks - 1) / cblocks;  // two per SM of an H100, fixed (not num_sms-derived) so callers can size `ws`: see sb200.h
   if (chunks > 256) chunks = 256;
   int rpb = (rows + chunks - 1) / chunks;
   if (rpb < 32) rpb = 32;

@@ -63,9 +63,6 @@ struct Ctx {
   EncodeTiledFn encode = nullptr;
   std::mutex mu;
   std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> tmaps;
-  bool gemm_attr_set = false;
-  bool gemm_stats_attr_set = false;
-  bool attn_attr_set = false;
 };
 
 // bf16 tensor map, 128-byte swizzle, zero OOB fill. dims/box innermost first; strides (bytes) for dims

@@ -1,31 +1,19 @@
-// LoRA-fused bf16 GEMM / implicit-GEMM 3x3 convolution for sm_100a.
+// LoRA-fused bf16 GEMM / implicit-GEMM 3x3 convolution for sm_90a.
 //
 //   out[M, N] = epilogue( A[M, K] . W[N, K]^T  [+ scale * (A . down^T) . up^T] )
 //
-// Persistent, warp-specialised kernel, one CTA per SM, in two flavours selected on the host:
-//   kCtas = 1   128 x bn output tile per CTA  (tcgen05.mma cta_group::1, UMMA 128 x (bn + rt) x 16)
-//   kCtas = 2   256 x bn tile per CTA PAIR    (cluster of 2, cta_group::2, UMMA 256 x (bn + rt) x 16): each CTA stages
-//               its own 128 A rows but only HALF of the W (and LoRA-down) rows, which halves the B-operand traffic
-//               through each SM's shared memory.
-// Warp roles (352 threads):
-//   warps 8, 9  TMA producers  — stream A / W / LoRA-down tiles through an mbarrier ring of smem stages (k-blocks dealt
-//                                 round-robin: one pass of the producer loop costs more issue cycles than a narrow tile's UMMAs)
-//   warp 10     MMA issuer     — (leader CTA only) tcgen05.mma into a double-buffered TMEM accumulator
-//   warps 0..7  epilogue       — two warps per TMEM lane quarter, interleaved over 32-column slabs: tcgen05.ld (one row
-//                                 per thread), rank-r LoRA up-projection, bias / time-embedding row bias / GEGLU /
-//                                 residual; residual tiles come in by cp.async and results leave through a swizzled
-//                                 smem staging tile so that global accesses are coalesced
-// Producer and issuer run as CONVERGED warps: every lane polls the mbarrier, an `elect.sync` region issues the
-// uniform-datapath instructions (UTMALDG / UTCHMMA / UTCBAR).  Round 1 ran them from a `lane == 0` branch, where ptxas
-// wraps each such instruction in an ELECT / R2UR.BROADCAST / BRA.U.ANY loop: ~125 issue-side cycles per UMMA
-// (tools/micro/issue_bench.cu: 126 clk per UMMA at any N <= 128 against 78 converged, 48 without the handshake), which
-// is what capped narrow tiles and made the CTA-pair kernel (longer per-k-block chain) issue-bound
-// (profiles/r02_gemm_issue.md).
-//
-// The LoRA down-projection rides in the tile's own UMMA: its rows are staged right behind the W rows of the stage, so
-// the instruction's N is bn + rt and t = A . down^T lands in spare accumulator columns.  For the CTA pair each CTA
-// appends its half of the down rows to its half of the W rows; the accumulator columns are then
-//   [ W cols 0..bn/2 | t 0..rt/2 | W cols bn/2..bn | t rt/2..rt ]   (acc_col / t_col below).
+// One CTA per 128 x BN output tile (BN = 64 or 128: a template parameter, picked on the host), 288 threads:
+//   warp 8      TMA producer — streams A / W / LoRA-down tiles (64-deep k-blocks) through an mbarrier ring of smem stages
+//   warps 0..7  two consumer warpgroups, rows 0..63 and 64..127 of the tile: wgmma m64 x BN x 16 from shared memory
+//               into registers; then the epilogue
+// The LoRA down-projection rides in the same k-block loop: its rows are staged right behind the W rows of the stage and
+// one more wgmma (N = rt) per k-step accumulates t = A . down^T.
+// Epilogue: both warpgroups park their accumulators in shared memory as an fp32 [128 x (BN + rt)] tile (over the stage
+// ring, which is free once the main loop has ended).  Each thread then owns one row: rank-r LoRA up-projection,
+// LayerNorm fold, bias / time-embedding row bias / GEGLU / residual; residual tiles come in by cp.async and results
+// leave through a swizzled smem staging tile so that global accesses are coalesced.
+// CTA pairs (kCtas = 2): a cluster of two CTAs on consecutive 128-row tiles of the same N tile.  Each CTA loads half
+// of the W (and LoRA-down) rows of a stage and multicasts them to both, which halves the weight traffic from L2.
 //
 // A-operand addressing modes:
 //   plain   2-D [M, K], optionally split along K over two sources (skip-connection concat, conv_shortcut)
@@ -45,47 +33,43 @@ namespace sb200 {
 
 constexpr int kBM = 128;  // rows per CTA
 constexpr int kBK = 64;
-constexpr int kEpiWarps = 16;
-constexpr int kEpiPerQuarter = kEpiWarps / 4;  // epilogue warps sharing one TMEM lane quarter (32 rows); slabs are dealt round-robin
-constexpr int kProducers = 2;  // TMA producer warps; k-blocks are dealt to them round-robin
-constexpr int kGemmThreads = 32 * (kEpiWarps + kProducers + 1);
-// Warp roles by index: the two single-instruction-stream roles get the HIGHEST warp ids.  A sub-partition's issue arbiter
-// favours the higher warp id (B300_MICROARCH.md: "hi-wid-first"), and each of these two warps shares its sub-partition
-// with two epilogue warps (warp id mod 4 fixes both the sub-partition and the TMEM lane quarter a warp may read, so the
-// epilogue has to sit on all four).  With the roles at warps 0 / 1 (round 1) an active epilogue starved the k-block loop:
-// the epilogue of tile i was not hidden behind the main loop of tile i + 1 (same-box: 8192x1280x1280 32.4 us with, 24.8 us
-// without epilogue, profiles/r02_gemm_tiles.txt).
+constexpr int kEpiWarps = 8;                   // the two consumer warpgroups
+constexpr int kEpiPerQuarter = kEpiWarps / 4;  // epilogue warps sharing one 32-row quarter; slabs are dealt round-robin
 constexpr int kProducerWarp = kEpiWarps;
-constexpr int kMmaWarp = kEpiWarps + kProducers;
+constexpr int kGemmThreads = 32 * (kEpiWarps + 1);
 constexpr int kMaxStages = 8;
 constexpr int kSmemBudget = 227 * 1024;
 constexpr int kBarRegion = 1024;
-constexpr uint32_t kDescHi = (1024u >> 4) | (1u << 14) | (2u << 29);  // UMMA smem descriptor, high word
+constexpr int kLoraCols = 32;         // accumulator columns kept for t = A . down^T (rt <= 32)
 constexpr int kSlab = 32;             // output columns staged per epilogue-warp iteration
 constexpr int kEpiBufBytes = 32 * 64; // [32 rows x 32 cols] bf16
-constexpr int kEpiBufs = 1;           // staging buffers per epilogue warp (with 4 warps per lane quarter the other warps of
-                                      // the sub-partition hide a slab's prefetch latency; a second buffer per warp would cost stages)
-constexpr int kEpiBytesPerWarp = kEpiBufs * kEpiBufBytes;  // + kEpiBufs x [32 cols][r] fp32 of lora_up rows when LoRA is fused
-constexpr int kEpiBytes = kEpiWarps * kEpiBytesPerWarp;
+constexpr int kEpiBytes = kEpiWarps * kEpiBufBytes;  // + kEpiWarps x [32 cols][r] fp32 of lora_up rows with LoRA
+constexpr int kConsumerBar = 5;       // named barrier of the 256 consumer threads (1..4: row-statistics reduction)
+
+// fp32 accumulator tile in shared memory: row stride BN + kLoraCols + 4 floats, so that the 32 rows a warp reads at
+// one column fall into distinct 16-byte bank groups
+__host__ __device__ constexpr int acc_stride(int bn) { return bn + kLoraCols + 4; }
+__host__ __device__ constexpr int acc_tile_bytes(int bn) { return kBM * acc_stride(bn) * 4; }
 
 struct GemmParams {
   CUtensorMap tmA[4];
   CUtensorMap tmB;
   CUtensorMap tmL;
   int M, N, K;
-  int bn;           // output columns of W per tile (UMMA N = bn + lora_rt), multiple of 16
+  int bn;           // output columns of W per tile (the kernel's BN)
   int ncols_out;    // output columns per tile (bn, or bn/2 with GEGLU)
   int Nout;         // output columns overall (N, or N/2 with GEGLU)
   int num_m_tiles, num_n_tiles;  // tiles of (128 * kCtas) x bn
-  int num_sub;      // 128-row sub-tiles along M (a CTA of a pair whose sub-tile index is >= num_sub idles through it)
+  int num_sub;      // 128-row sub-tiles along M (a CTA of a pair whose sub-tile index is >= num_sub computes zeros)
   int kblocks;      // K / 64 (conv: 9 * cb_total)
   int stages;
-  int stage_bytes;  // bytes of one smem stage of ONE CTA
+  int stage_bytes;  // bytes of one smem stage
+  int ring_bytes;   // stage ring, also holds the fp32 accumulator tile after the main loop
   int a_tx;         // bytes one A load deposits (box bytes; < 16 KB for conv patches smaller than 128 pixels)
-  int b_rows;       // W rows staged per CTA per k-block (bn / kCtas)
-  int l_rows;       // LoRA-down rows staged per CTA (rt / kCtas)
+  int b_rows;       // W rows one CTA loads per k-block (bn / kCtas)
+  int l_rows;       // LoRA-down rows one CTA loads per k-block (rt / kCtas)
   int up_buf_bytes; // per-warp staging of one slab's lora_up rows: 32 * r * 4 (0 without LoRA)
-  int n_fast;       // tile order: 1 = consecutive work units share the A row-tile and walk the N tiles (A is read from
+  int n_fast;       // tile order: 1 = consecutive CTAs share the A row-tile and walk the N tiles (A is read from
                     // DRAM once, W stays L2-resident); 0 = M fastest (A re-streamed once per N tile when it exceeds L2)
   int a_mode;       // 0 plain, 1 conv3x3 stride 1, 2 conv3x3 stride 2
   int kb_split;     // k-blocks (per tap) that come from source 0
@@ -94,10 +78,6 @@ struct GemmParams {
   int bw, bh, bb;   // conv patch of one sub-tile (bw * bh * bb <= 128 pixels)
   int tiles_w, tiles_h;
   int flags;
-  int quad;         // CTA pairs launched as 2x2 clusters: two pairs on the same rows, A tile multicast to both (tmA[2..3]
-                    // = half-height boxes); consecutive N tiles go to the two pairs of a cluster
-  int mma_unroll2;  // issue two k-blocks per elect region (SB200_MMA_UNROLL, default 1)
-  int debug;        // profiling experiments only: bit 0 skip W loads, bit 1 skip A loads, bit 3 skip the epilogue (garbage)
   const __nv_bfloat16* bias;
   const __nv_bfloat16* rowbias;
   int rows_per_batch;
@@ -148,30 +128,39 @@ __device__ __forceinline__ void lora_apply(float* f, const float* t, uint32_t up
   }
 }
 
-// Converged-warp mbarrier wait: every lane polls (the result is warp-uniform), a protocol bug traps instead of hanging.
-__device__ __forceinline__ void mbar_wait_warp(uint32_t bar, uint32_t parity) {
-  uint32_t spins = 0;
-  long long t0 = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 255u) == 0) {  // keep the common path lean: the clock is read once per 256 failed polls
-      if (t0 == 0) {
-        t0 = clock64();
-      } else if (clock64() - t0 > SB200_WATCHDOG_CYCLES) {
-        if ((threadIdx.x & 31) == 0)
-          printf("sb200: mbarrier watchdog (block %d warp %d bar 0x%x parity %u)\n", blockIdx.x, threadIdx.x >> 5, bar, parity);
-        __trap();
-      }
-    }
+// n consecutive fp32 of the shared accumulator tile (n multiple of 4)
+template <int n>
+__device__ __forceinline__ void ld_acc(uint32_t addr, uint32_t* v) {
+#pragma unroll
+  for (int i = 0; i < n / 4; ++i) {
+    const uint4 a = ld_shared_v4(addr + 16 * i);
+    v[4 * i] = a.x;
+    v[4 * i + 1] = a.y;
+    v[4 * i + 2] = a.z;
+    v[4 * i + 3] = a.w;
   }
 }
 
-// kStats builds write 8 int64 per CTA: {producer wait, producer total, issuer wait on full, issuer total, epilogue warp 0
-// wait on the accumulator, epilogue warp 0 total, issuer wait on the accumulator hand-back, -}.  The buffer travels in
-// the (otherwise unused) rowbias slot of a call without SB200_EPI_ROWBIAS; without one the head of `out` is used.
-__device__ __forceinline__ long long* stats_out(const GemmParams& p) {
-  return (p.rowbias != nullptr && !(p.flags & SB200_EPI_ROWBIAS))
-             ? reinterpret_cast<long long*>(const_cast<__nv_bfloat16*>(p.rowbias))
-             : reinterpret_cast<long long*>(p.out);
+// accumulator fragment of one warpgroup (m64 x N, see wgmma.cuh) -> rows row0.. of the shared fp32 tile
+template <int N>
+__device__ __forceinline__ void store_frag(const float* d, uint32_t tile, int row0, int col0, int stride) {
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  const int r = row0 + w * 16 + (lane >> 2);
+#pragma unroll
+  for (int i = 0; i < N / 2; i += 2) {
+    const int row = r + 8 * ((i >> 1) & 1);
+    const int col = col0 + 8 * (i >> 2) + 2 * (lane & 3);
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(tile + (row * stride + col) * 4), "f"(d[i]), "f"(d[i + 1])
+                 : "memory");
+  }
+}
+
+template <int BN>
+__device__ __forceinline__ void wgmma_main(float* d, uint64_t a, uint64_t b) {
+  if constexpr (BN == 64)
+    wgmma_ss_n64(d, a, b, 1u);
+  else
+    wgmma_ss_n128(d, a, b, 1u);
 }
 
 // First output pixel (b0, h0, w0) of conv sub-tile `st` (w fastest, then h, then batch).
@@ -184,33 +173,23 @@ __device__ __forceinline__ void conv_origin(const GemmParams& p, int st, int& b0
   b0 = (r / p.tiles_h) * p.bb;
 }
 
-// kStats (profiling builds of the same kernel, debug bit 5): the producer and the issuer accumulate the cycles they spend
-// blocked on their mbarriers and write {wait, total} per CTA over the head of `out` (combine with debug bit 3).
-template <int kCtas, bool kStats = false>
+template <int BN, int kCtas, int RT>
 __global__ void __launch_bounds__(kGemmThreads, 1) gemm_kernel(const __grid_constant__ GemmParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t base = (raw_addr + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024 B alignment
-  uint8_t* smem = smem_raw + (base - raw_addr);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t crank = kCtas == 2 ? cluster_ctarank() : 0u;   // rank in the cluster (0..1, or 0..3 in quad mode)
-  const uint32_t cta_rank = crank & 1u;                          // rank inside the CTA pair
-  const uint32_t pair_id = crank >> 1;                           // which pair of a 2x2 cluster
-  const uint32_t lead = crank & ~1u;                             // cluster rank of this pair's leader
-  const bool quad = kCtas == 2 && p.quad != 0;
-  const bool leader = cta_rank == 0;
+  const uint32_t cta_rank = kCtas == 2 ? cluster_ctarank() : 0u;
   const int S = p.stages;
-  const uint32_t bar_full = base;                 // S barriers (used in the leader CTA)
-  const uint32_t bar_empty = base + 8u * S;       // S barriers (every CTA)
-  const uint32_t bar_tfull = base + 16u * S;      // 2 barriers (every CTA)
-  const uint32_t bar_tempty = bar_tfull + 16u;    // 2 barriers (used in the leader CTA)
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + 512);
+  const uint32_t bar_full = base;            // S barriers
+  const uint32_t bar_empty = base + 8u * S;  // S barriers
   const uint32_t tiles = base + kBarRegion;
   const bool has_lora = (p.flags & SB200_EPI_LORA) != 0;
   const bool geglu = (p.flags & SB200_EPI_GEGLU) != 0;
+  constexpr int rt = RT;  // LoRA-down rows of a stage (0 without LoRA)
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tmA[0]);
@@ -220,608 +199,370 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_kernel(const __grid_cons
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < S; ++i) {
       mbar_init(bar_full + 8u * i, 1);
-      mbar_init(bar_empty + 8u * i, quad ? 2 : 1);  // quad: the stage is overwritten from both pairs, both must be done
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(bar_tfull + 8u * i, 1);
-      mbar_init(bar_tempty + 8u * i, kEpiWarps * kCtas);
+      mbar_init(bar_empty + 8u * i, 2 * kCtas);  // one arrival per consumer warpgroup of every CTA the stage feeds
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if constexpr (kCtas == 2) {
-      tmem_alloc_2cta(smem_u32(const_cast<uint32_t*>(tmem_slot)), 512);
-      tmem_relinquish_2cta();
-    } else {
-      tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), 512);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
   if constexpr (kCtas == 2) {
     cluster_sync_all();
   } else {
     __syncthreads();
   }
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();  // everything above overlapped the previous kernel's tail; global memory is touched only below
 
-  // persistent work unit: CTA, CTA pair, or (quad) a cluster of two pairs that walks PAIRS of adjacent N tiles
-  const int ctas_per_unit = quad ? 4 : kCtas;
-  const int unit = blockIdx.x / ctas_per_unit;
-  const int num_units = gridDim.x / ctas_per_unit;
-  const int num_n_tiles = quad ? p.num_n_tiles / 2 : p.num_n_tiles, num_m_tiles = p.num_m_tiles, n_fast = p.n_fast;
-  const int total_tiles = num_m_tiles * num_n_tiles;
-  const int nt_mul = quad ? 2 : 1, nt_add = quad ? static_cast<int>(pair_id) : 0;
+  const int t = blockIdx.x / kCtas;  // this CTA's (pair's) output tile
+  const int num_n_tiles = p.num_n_tiles, num_m_tiles = p.num_m_tiles;
+  const int mt = p.n_fast ? t / num_n_tiles : t % num_m_tiles;
+  const int nt = p.n_fast ? t % num_n_tiles : t / num_m_tiles;
+  const int st = mt * kCtas + static_cast<int>(cta_rank);  // this CTA's 128-row sub-tile
   const int kblocks = p.kblocks;
   const uint32_t stage_bytes = static_cast<uint32_t>(p.stage_bytes);
   const uint32_t a_bytes = kBM * 128;
-  const uint32_t b_bytes = static_cast<uint32_t>(p.b_rows) * 128;
-  const int bn = p.bn;
-  const int rt = has_lora ? p.lora_rt : 0;
+  const uint32_t b_bytes = static_cast<uint32_t>(BN) * 128;  // W rows of a stage (both halves for a pair)
 
-  if (warp >= kProducerWarp && warp < kProducerWarp + kProducers) {
-    // ------------------------------------------------------------------ TMA producers (every CTA), converged warps
-    // One pass of this loop (barrier wait, elect region, expect_tx, two or three UTMALDGs at ~60 issue cycles each) costs
-    // a warp ~410 cycles (measured with the kStats build, profiles/r02_gemm_tiles.txt) — more than a 128- or 192-wide
-    // tile's four UMMAs — so the k-blocks of the unit's whole tile sequence are dealt round-robin to kProducers warps.
-    // Warp w loads the k-blocks whose running index g satisfies g % kProducers == w into stage g % S; a stage's full
-    // barrier is armed (expect_tx) by the one warp that loads it.
-    const int pw = warp - kProducerWarp;
-    const bool skip_w = (p.debug & 1) != 0, skip_a = (p.debug & 2) != 0;
+  if (warp == kProducerWarp) {
+    // ------------------------------------------------------------------ TMA producer, converged warp
     const int a_mode = p.a_mode, kb_split = p.kb_split, cb_total = p.cb_total;
-    const uint32_t tx = (skip_a ? 0u : static_cast<uint32_t>(p.a_tx)) + (skip_w ? 0u : b_bytes) +
-                        static_cast<uint32_t>(p.l_rows) * 128u;
-    int stage = pw % S;
-    uint32_t phase = static_cast<uint32_t>(pw / S) & 1u;
-    long long st_wait = 0, st_t0 = kStats ? clock64() : 0;
-    int t = unit, kb = pw;           // position of this warp's next k-block: tile t, k-block kb inside it
-    while (kb >= kblocks) {
-      kb -= kblocks;
-      t += num_units;
+    const uint32_t tx = static_cast<uint32_t>(p.a_tx) + b_bytes + static_cast<uint32_t>(rt) * 128u;
+    const int m0 = st * kBM;
+    int b0 = 0, h0 = 0, w0 = 0;
+    if (a_mode != 0) {
+      if (st < p.num_sub)
+        conv_origin(p, st, b0, h0, w0);
+      else
+        b0 = p.B;  // phantom sub-tile of an odd pair: every box is out of bounds -> zero fill
     }
-    int cur_t = -1, nt = 0, m0 = 0, b0 = 0, h0 = 0, w0 = 0, brow = 0;
-    while (t < total_tiles) {
-      if (t != cur_t) {              // tile coordinates (once per tile and warp)
-        cur_t = t;
-        const int mt = n_fast ? t / num_n_tiles : t % num_m_tiles;
-        nt = (n_fast ? t % num_n_tiles : t / num_m_tiles) * nt_mul + nt_add;
-        const int st = mt * kCtas + static_cast<int>(cta_rank);  // this CTA's 128-row sub-tile
-        m0 = st * kBM;
-        b0 = h0 = w0 = 0;
-        if (a_mode != 0) {
-          if (st < p.num_sub) {
-            conv_origin(p, st, b0, h0, w0);
-          } else {
-            b0 = p.B;  // phantom sub-tile of an odd pair: every box is out of bounds -> zero fill
-          }
-        }
-        // W rows this CTA stages
-        if (geglu) {
-          const int half = bn >> 1;
-          brow = kCtas == 2 ? (cta_rank == 0 ? nt * half : (p.N >> 1) + nt * half) : nt * half;
-        } else {
-          brow = nt * bn + static_cast<int>(cta_rank) * p.b_rows;
-        }
-      }
+    // W rows this CTA loads (a pair: half each, multicast to both)
+    int brow;
+    if (geglu) {
+      const int half = BN >> 1;
+      brow = (kCtas == 2 && cta_rank == 1) ? (p.N >> 1) + nt * half : nt * half;
+    } else {
+      brow = nt * BN + static_cast<int>(cta_rank) * p.b_rows;
+    }
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int kb = 0; kb < kblocks; ++kb) {
       const uint32_t full_bar = bar_full + 8u * stage, empty_bar = bar_empty + 8u * stage;
-      {
-        const long long w0c = kStats ? clock64() : 0;
-        mbar_wait_warp(empty_bar, phase ^ 1u);
-        if (kStats) st_wait += clock64() - w0c;
-      }
+      mbar_wait(empty_bar, phase ^ 1u);
       if (elect_one()) {
-        uint32_t full = full_bar;
-        if constexpr (kCtas == 2) {
-          // Both CTAs' TMA bytes are counted on the LEADER's barrier; only the leader arrives (expecting the
-          // bytes of the pair).  The peer's bytes for this stage cannot land before the previous use of the
-          // stage completed (its empty barrier is released by the leader's commit after that phase), and a
-          // transiently negative tx-count inside the right phase is legal.
-          full = mapa_u32(full, lead);
-          if (leader) mbar_expect_tx(full_bar, 2u * tx);
-        } else {
-          mbar_expect_tx(full, tx);
-        }
+        mbar_expect_tx(full_bar, tx);
         const uint32_t sA = tiles + static_cast<uint32_t>(stage) * stage_bytes;
         const uint32_t sB = sA + a_bytes;
-        const CUtensorMap* amap;
-        int c0, c1, c2 = 0, c3 = 0;
         if (a_mode == 0) {
           const int src = kb < kb_split ? 0 : 1;
-          amap = &p.tmA[src];
-          c0 = (src ? kb - kb_split : kb) * kBK;
-          c1 = m0;
+          tma_load_2d(sA, &p.tmA[src], full_bar, (src ? kb - kb_split : kb) * kBK, m0);
         } else {
-          const int tap = kb / cb_total;   // filter tap and channel block of this k-block
+          const int tap = kb / cb_total;  // filter tap and channel block of this k-block
           const int cb = kb - tap * cb_total;
           const int kh = tap / 3;
           const int kw = tap - kh * 3;
           if (a_mode == 1) {
             const int src = cb < kb_split ? 0 : 1;
-            amap = &p.tmA[src];
-            c0 = (src ? cb - kb_split : cb) * kBK;
-            c1 = w0 + kw - 1;
-            c2 = h0 + kh - 1;
+            tma_load_4d(sA, &p.tmA[src], full_bar, (src ? cb - kb_split : cb) * kBK, w0 + kw - 1, h0 + kh - 1, b0);
           } else {
-            // input row 2*ho + kh - 1: kh=0 -> odd plane, row ho-1; kh=1 -> even plane, row ho;
-            // kh=2 -> odd plane, row ho
+            // input row 2*ho + kh - 1: kh=0 -> odd plane, row ho-1; kh=1 -> even plane, row ho; kh=2 -> odd plane, row ho
             const int ph = (kh == 1) ? 0 : 1;
             const int pwl = (kw == 1) ? 0 : 1;
-            amap = &p.tmA[ph * 2 + pwl];
-            c0 = cb * kBK;
-            c1 = w0 + ((kw == 0) ? -1 : 0);
-            c2 = h0 + ((kh == 0) ? -1 : 0);
+            tma_load_4d(sA, &p.tmA[ph * 2 + pwl], full_bar, cb * kBK, w0 + ((kw == 0) ? -1 : 0),
+                        h0 + ((kh == 0) ? -1 : 0), b0);
           }
-          c3 = b0;
         }
         if constexpr (kCtas == 2) {
-          if (!skip_a) {
-            if (quad) {
-              // the CTAs with this pair rank in both pairs need the same 128 rows: each loads 64 of them and multicasts
-              // to both (L2 -> SM traffic of A halves; the N = 1280 shapes are bound by it, DESIGN.md §8)
-              const int src = kb < kb_split ? 0 : 1;
-              tma_load_2d_2cta_mc(sA + pair_id * (a_bytes >> 1), &p.tmA[2 + src], full_bar & 0xFEFFFFFFu, c0,
-                                  c1 + static_cast<int>(pair_id) * (kBM / 2),
-                                  static_cast<uint16_t>((1u << cta_rank) | (4u << cta_rank)));
-            } else if (a_mode == 0) {
-              tma_load_2d_2cta(sA, amap, full, c0, c1);
-            } else {
-              tma_load_4d_2cta(sA, amap, full, c0, c1, c2, c3);
-            }
-          }
-          if (!skip_w) tma_load_2d_2cta(sB, &p.tmB, full, kb * kBK, brow);
-          if (has_lora) tma_load_2d_2cta(sB + b_bytes, &p.tmL, full, kb * kBK, static_cast<int>(cta_rank) * p.l_rows);
+          const uint32_t boff = cta_rank * static_cast<uint32_t>(p.b_rows) * 128u;
+          tma_load_2d_mc(sB + boff, &p.tmB, full_bar, kb * kBK, brow, 3);
+          if (has_lora)
+            tma_load_2d_mc(sB + b_bytes + cta_rank * static_cast<uint32_t>(p.l_rows) * 128u, &p.tmL, full_bar, kb * kBK,
+                           static_cast<int>(cta_rank) * p.l_rows, 3);
         } else {
-          if (!skip_a) {
-            if (a_mode == 0)
-              tma_load_2d(sA, amap, full, c0, c1);
-            else
-              tma_load_4d(sA, amap, full, c0, c1, c2, c3);
-          }
-          if (!skip_w) {
-            tma_load_2d(sB, &p.tmB, full, kb * kBK, brow);
-            if (geglu)
-              tma_load_2d(sB + static_cast<uint32_t>(bn >> 1) * 128, &p.tmB, full, kb * kBK, (p.N >> 1) + nt * (bn >> 1));
-          }
-          if (has_lora) tma_load_2d(sB + b_bytes, &p.tmL, full, kb * kBK, 0);
+          tma_load_2d(sB, &p.tmB, full_bar, kb * kBK, brow);
+          if (geglu) tma_load_2d(sB + (b_bytes >> 1), &p.tmB, full_bar, kb * kBK, (p.N >> 1) + nt * (BN >> 1));
+          if (has_lora) tma_load_2d(sB + b_bytes, &p.tmL, full_bar, kb * kBK, 0);
         }
       }
       __syncwarp();
-      kb += kProducers;
-      while (kb >= kblocks) {
-        kb -= kblocks;
-        t += num_units;
-      }
-      stage += kProducers;
-      if (stage >= S) {
-        stage -= S;
+      if (++stage == S) {
+        stage = 0;
         phase ^= 1u;
       }
     }
-    if (kStats && lane == 0 && pw == 0) {
-      long long* o = stats_out(p) + blockIdx.x * 8;
-      o[0] = st_wait;
-      o[1] = clock64() - st_t0;
-    }
-  } else if (warp == kMmaWarp) {
-    // ------------------------------------------------------------------ MMA issuer (leader CTA only), converged warp
-    if (leader) {
-      const uint32_t idesc = umma_idesc_bf16(kBM * kCtas, bn + rt);
-      const uint16_t pair_mask = static_cast<uint16_t>(3u << (2u * pair_id));    // this pair's two CTAs
-      const uint16_t empty_mask = quad ? static_cast<uint16_t>(0xF) : pair_mask;  // who refills this pair's stages
-      // The loop below is the issue-side critical path (one pass per 64-deep k-block has to fit inside the 4 UMMAs'
-      // tensor time: 2 (bn + rt) cycles), so everything it needs is a running register value: descriptor low words and
-      // barrier addresses advance by constants and wrap with the stage counter, nothing is recomputed from the stage
-      // index or re-read from the parameter bank.
-      // descriptor = {hi: SBO 1024 B | version 1 | SWIZZLE_128B, lo: (address >> 4)}; +2 per 16-element k-step
-      const uint32_t a_lo0 = (tiles & 0x3FFFF) >> 4;
-      const uint32_t sb16 = stage_bytes >> 4, ab16 = a_bytes >> 4;
-      const int unroll2 = p.mma_unroll2;
-      uint32_t a_lo = a_lo0, full_bar = bar_full, empty_bar = bar_empty;
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      long long st_wait = 0, st_twait = 0;
-      const long long st_t0 = kStats ? clock64() : 0;
-      auto wait_full = [&](uint32_t bar, uint32_t ph) {
-        const long long w0 = kStats ? clock64() : 0;
-        mbar_wait_warp(bar, ph);
-        if (kStats) st_wait += clock64() - w0;
-      };
-      auto issue_kblock = [&](uint32_t lo, uint32_t ebar, uint32_t first, uint32_t d_tmem) {
-#pragma unroll
-        for (int k = 0; k < kBK / 16; ++k) {
-          const uint64_t adesc = (static_cast<uint64_t>(kDescHi) << 32) | (lo + 2u * k);
-          const uint64_t bdesc = (static_cast<uint64_t>(kDescHi) << 32) | (lo + ab16 + 2u * k);
-          const uint32_t acc = (k != 0) ? 1u : first;
-          if constexpr (kCtas == 2)
-            umma_ss_2cta(d_tmem, adesc, bdesc, idesc, acc);
-          else
-            umma_ss(d_tmem, adesc, bdesc, idesc, acc);
-        }
-        // free the smem stage (in every CTA of the pair) once these MMAs retire
-        if constexpr (kCtas == 2)
-          umma_commit_2cta(ebar, empty_mask);
-        else
-          umma_commit(ebar);
-      };
-      auto advance = [&]() {
-        a_lo += sb16;
-        full_bar += 8u;
-        empty_bar += 8u;
-        if (++stage == S) {
-          stage = 0;
-          phase ^= 1u;
-          a_lo = a_lo0;
-          full_bar = bar_full;
-          empty_bar = bar_empty;
-        }
-      };
-      for (int t = unit; t < total_tiles; t += num_units) {
-        {
-          const long long w0 = kStats ? clock64() : 0;
-          mbar_wait_warp(bar_tempty + 8u * as, aphase ^ 1u);
-          if (kStats) st_twait += clock64() - w0;
-        }
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(as) * 256u;
-        int kb = 0;
-        if (unroll2) {
-          // two k-blocks per elect region: the region's fixed cost (reconvergence, operand-release wait) is paid once
-          // per 8 UMMAs
-          for (; kb + 1 < kblocks; kb += 2) {
-            const uint32_t lo0 = a_lo, eb0 = empty_bar;
-            wait_full(full_bar, phase);
-            advance();
-            const uint32_t lo1 = a_lo, eb1 = empty_bar;
-            wait_full(full_bar, phase);
-            advance();
-            tc_fence_after();
-            if (elect_one()) {
-              issue_kblock(lo0, eb0, kb != 0 ? 1u : 0u, d_tmem);
-              issue_kblock(lo1, eb1, 1u, d_tmem);
-            }
-            __syncwarp();
-          }
-        }
-        for (; kb < kblocks; ++kb) {
-          wait_full(full_bar, phase);
-          tc_fence_after();
-          if (elect_one()) issue_kblock(a_lo, empty_bar, kb != 0 ? 1u : 0u, d_tmem);
-          __syncwarp();
-          advance();
-        }
-        if (elect_one()) {  // accumulator complete once everything issued so far retires
-          if constexpr (kCtas == 2)
-            umma_commit_2cta(bar_tfull + 8u * as, pair_mask);
-          else
-            umma_commit(bar_tfull + 8u * as);
-        }
-        __syncwarp();
-        as ^= 1;
-        if (as == 0) aphase ^= 1u;
-      }
-      if (kStats && lane == 0) {
-        long long* o = stats_out(p) + blockIdx.x * 8;
-        o[2] = st_wait;
-        o[3] = clock64() - st_t0;
-        o[6] = st_twait;
-      }
-    }
   } else {
-    // ------------------------------------------------------------------ epilogue (warps 0..7, every CTA)
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int hsel = warp >> 2;             // which of the kEpiPerQuarter warps of this quarter (slab index mod that)
-    int as = 0;
-    uint32_t aphase = 0;
+    // ------------------------------------------------------------------ consumers: main loop
+    const int wg = warp >> 2;
+    float acc[BN / 2];
+    float accl[16];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) accl[i] = 0.f;
+    const bool signal = (threadIdx.x & 127) == 0;
+    const uint32_t peer_empty = kCtas == 2 ? mapa_u32(bar_empty, cta_rank ^ 1u) : 0u;
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int kb = 0; kb < kblocks; ++kb) {
+      mbar_wait(bar_full + 8u * stage, phase);
+      const uint32_t sA = tiles + static_cast<uint32_t>(stage) * stage_bytes + static_cast<uint32_t>(wg) * 64u * 128u;
+      const uint32_t sB = tiles + static_cast<uint32_t>(stage) * stage_bytes + a_bytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBK / 16; ++k) {
+        const uint64_t adesc = gmma_desc_sw128(sA + 32u * k);
+        wgmma_main<BN>(acc, adesc, gmma_desc_sw128(sB + 32u * k));
+        if constexpr (rt == 16)
+          wgmma_ss_n16(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
+        else if constexpr (rt == 32)
+          wgmma_ss_n32(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block's products have read their stage: hand it back to the producer(s)
+      if (kb > 0 && signal) {
+        mbar_arrive(bar_empty + 8u * prev);
+        if (kCtas == 2) mbar_arrive_cluster(peer_empty + 8u * prev);
+      }
+      prev = stage;
+      if (++stage == S) {
+        stage = 0;
+        phase ^= 1u;
+      }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
+#pragma unroll
+    for (int i = 0; i < 16; ++i) reg_fence(accl[i]);
+
+    // ------------------------------------------------------------------ epilogue
+    const uint32_t accs = tiles;  // fp32 accumulator tile, over the stage ring
+    constexpr int kStride = acc_stride(BN);
+    asm volatile("bar.sync %0, %1;" ::"n"(kConsumerBar), "n"(32 * kEpiWarps) : "memory");  // both warpgroups done reading
+    store_frag<BN>(acc, accs, wg * 64, 0, kStride);
+    if constexpr (rt == 16)
+      store_frag<16>(accl, accs, wg * 64, BN, kStride);
+    else if constexpr (rt == 32)
+      store_frag<32>(accl, accs, wg * 64, BN, kStride);
+    asm volatile("bar.sync %0, %1;" ::"n"(kConsumerBar), "n"(32 * kEpiWarps) : "memory");
+
+    const int q = warp & 3;      // 32-row quarter of the tile this warp writes
+    const int hsel = warp >> 2;  // which of the kEpiPerQuarter warps of this quarter (slab index mod that)
     const float lscale =
         has_lora ? (p.lora_scale_dev ? p.lora_scale * __ldg(p.lora_scale_dev) : p.lora_scale) : 0.f;
     const bool has_resid = (p.flags & SB200_EPI_RESID) != 0;
-    const bool skip_epi = (p.debug & 8) != 0;
-    const uint32_t tempty_leader = kCtas == 2 ? mapa_u32(bar_tempty, lead) : bar_tempty;
-    // accumulator column of output column c / of LoRA-down row j (see the header: the pair interleaves its halves)
-    const int half_cols = bn >> 1, lr_half = rt >> 1;
-    const bool pair_lora = kCtas == 2 && has_lora;
-    // per-warp staging buffers (2 x [32 rows x 32 cols] bf16, 64 B rows, 16-byte chunks XOR-swizzled by
-    // (row >> 1) & 3): residual tiles arrive here by cp.async with coalesced global reads, results leave from
-    // here with coalesced global writes; in between every thread touches only its own row.
-    const uint32_t ebuf = tiles + static_cast<uint32_t>(S) * stage_bytes +
-                          static_cast<uint32_t>(warp) * (kEpiBytesPerWarp + kEpiBufs * p.up_buf_bytes);
-    const uint32_t ubuf0 = ebuf + kEpiBufs * kEpiBufBytes;  // kEpiBufs x p.up_buf_bytes, same buffer parity as ebuf
-    int bufsel = 0;
-    long long st_wait = 0;
-    const long long st_t0 = kStats ? clock64() : 0;
-    for (int t = unit; t < total_tiles; t += num_units) {
-      const int mt = n_fast ? t / num_n_tiles : t % num_m_tiles;
-      const int nt = (n_fast ? t % num_n_tiles : t / num_m_tiles) * nt_mul + nt_add;
-      const int st = mt * kCtas + static_cast<int>(cta_rank);
-      // output row of this thread's accumulator row (q * 32 + lane), or -1 (padding row of the tile)
-      int my_row = -1, my_batch = 0;
-      {
-        const int r = q * 32 + lane;
-        if (p.a_mode == 0) {
-          const int m = st * kBM + r;
-          if (m < p.M) my_row = m;
-          my_batch = (p.flags & SB200_EPI_ROWBIAS) ? m / p.rows_per_batch : 0;
-        } else if (st < p.num_sub) {
-          int b0, h0, w0;
-          conv_origin(p, st, b0, h0, w0);
-          const int iw = r % p.bw;
-          const int t2 = r / p.bw;
-          const int ih = t2 % p.bh;
-          const int ib = t2 / p.bh;
-          const int b = b0 + ib, h = h0 + ih, w = w0 + iw;
-          if (ib < p.bb && b < p.B && h < p.H && w < p.W) my_row = (b * p.H + h) * p.W + w;
-          my_batch = b;
-        }
+    // per-warp staging buffer ([32 rows x 32 cols] bf16, 64 B rows, 16-byte chunks XOR-swizzled by (row >> 1) & 3):
+    // residual tiles arrive here by cp.async with coalesced global reads, results leave from here with coalesced global
+    // writes; in between every thread touches only its own row.
+    const uint32_t ebuf = tiles + static_cast<uint32_t>(p.ring_bytes) +
+                          static_cast<uint32_t>(warp) * (kEpiBufBytes + p.up_buf_bytes);
+    const uint32_t ubuf = ebuf + kEpiBufBytes;  // p.up_buf_bytes of lora_up rows
+    const uint32_t arow = accs + static_cast<uint32_t>((q * 32 + lane) * kStride) * 4u;
+    // output row of this thread's accumulator row (q * 32 + lane), or -1 (padding row of the tile)
+    int my_row = -1, my_batch = 0;
+    {
+      const int r = q * 32 + lane;
+      if (p.a_mode == 0) {
+        const int m = st * kBM + r;
+        if (m < p.M) my_row = m;
+        my_batch = (p.flags & SB200_EPI_ROWBIAS) ? m / p.rows_per_batch : 0;
+      } else if (st < p.num_sub) {
+        int b0, h0, w0;
+        conv_origin(p, st, b0, h0, w0);
+        const int iw = r % p.bw;
+        const int t2 = r / p.bw;
+        const int ih = t2 % p.bh;
+        const int ib = t2 / p.bh;
+        const int b = b0 + ib, h = h0 + ih, w = w0 + iw;
+        if (ib < p.bb && b < p.B && h < p.H && w < p.W) my_row = (b * p.H + h) * p.W + w;
+        my_batch = b;
       }
-      const bool row_ok = my_row >= 0;
-      // LayerNorm fold: (mean, rstd) of this thread's row of x from the producer's partial sums
-      // part-major [parts][M][2]: the 32 rows of a warp read consecutive addresses.  The first loads are issued here
-      // and summed after the accumulator wait, so their L2 latency hides behind it.
-      constexpr int kLnPre = 8;
-      float2 ln_pre[kLnPre];
-      const bool ln_on = p.ln_stats != nullptr && row_ok;
-      const float2* ln_sp = reinterpret_cast<const float2*>(p.ln_stats) + (ln_on ? my_row : 0);
-#pragma unroll
-      for (int i = 0; i < kLnPre; ++i)
-        ln_pre[i] = (ln_on && i < p.ln_parts) ? __ldg(ln_sp + static_cast<size_t>(i) * p.M) : make_float2(0.f, 0.f);
-      float rs1 = 0.f, rs2 = 0.f;  // row statistics of what this warp writes in this tile
-      const int n_base = nt * p.ncols_out;
-      const int ncols_valid = min(p.ncols_out, p.Nout - n_base);
-      const int nslabs = (ncols_valid + kSlab - 1) / kSlab;
-      const int my_slabs = skip_epi ? 0 : (nslabs - hsel + kEpiPerQuarter - 1) / kEpiPerQuarter;  // slabs hsel, hsel + kEpiPerQuarter, ...
-      auto prefetch_resid = [&](int col0, int sw, uint32_t buf) {
-        const int cpr = sw >> 3;  // 16-byte chunks per row
-        if (has_resid) {
-          for (int idx = lane; idx < 32 * cpr; idx += 32) {
-            const int row = cpr == 4 ? idx >> 2 : idx / cpr;
-            const int ch = idx - row * cpr;
-            const int mr = __shfl_sync(0xffffffffu, my_row, row);
-            if (mr >= 0)
-              cp_async_16(buf + row * 64 + ((ch ^ ((row >> 1) & 3)) << 4),
-                          p.resid + static_cast<size_t>(mr) * p.ldr + n_base + col0 + ch * 8);
-          }
-        }
-        if (has_lora && lane < sw) {
-          // this slab's lora_up rows ([r] fp32 per output column) travel with the residual: the rank-r update then
-          // reads them from shared memory instead of taking an L2 round trip per 16 columns inside the loop
-          const uint32_t ub = ubuf0 + (buf == ebuf ? 0u : static_cast<uint32_t>(p.up_buf_bytes)) + lane * p.lora_r * 4;
-          const float* src = p.lora_up + static_cast<size_t>(n_base + col0 + lane) * p.lora_r;
-          cp_async_16(ub, src);
-          if (p.lora_r == 8) cp_async_16(ub + 16, src + 4);
-        }
-        cp_async_commit();
-      };
-      const bool staged = has_resid || has_lora;
-      if (staged && my_slabs > 0)
-        prefetch_resid(hsel * kSlab, min(kSlab, ncols_valid - hsel * kSlab), ebuf + bufsel * kEpiBufBytes);
-      const __nv_bfloat16* rb =
-          (p.flags & SB200_EPI_ROWBIAS) ? p.rowbias + static_cast<size_t>(row_ok ? my_batch : 0) * p.Nout : nullptr;
-      {
-        const long long w0c = kStats ? clock64() : 0;
-        mbar_wait(bar_tfull + 8u * as, aphase);
-        if (kStats) st_wait += clock64() - w0c;
-      }
-      tc_fence_after();
-      const uint32_t taddr =
-          tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(as) * 256u;
-      // LayerNorm fold: (mean, rstd) of this thread's row of x from the producer's partial sums
-      float ln_rstd = 1.f, ln_rm = 0.f;
-      if (ln_on) {
-        float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-        for (int i = 0; i < kLnPre; ++i) {
-          s1 += ln_pre[i].x;
-          s2 += ln_pre[i].y;
-        }
-        for (int i = kLnPre; i < p.ln_parts; ++i) {
-          const float2 v2 = __ldg(ln_sp + static_cast<size_t>(i) * p.M);
-          s1 += v2.x;
-          s2 += v2.y;
-        }
-        const float mean = s1 * p.ln_inv_c;
-        ln_rstd = rsqrtf(fmaxf(s2 * p.ln_inv_c - mean * mean, 0.f) + p.ln_eps);
-        ln_rm = ln_rstd * mean;
-      }
-      float tl[8];
-      int group_lo = 0, group_hi = 0;  // output-column range of the adaptor whose t = A.down^T is held in tl
-      const uint32_t swz = static_cast<uint32_t>((lane >> 1) & 3);
-      for (int k = 0; k < my_slabs; ++k) {
-        const int col0 = (hsel + kEpiPerQuarter * k) * kSlab;
-        const int sw = min(kSlab, ncols_valid - col0);
-        const uint32_t buf = ebuf + bufsel * kEpiBufBytes;
-        const bool more = k + 1 < my_slabs;
-        if (kEpiBufs == 2 && staged && more) {
-          const int ncol0 = col0 + kEpiPerQuarter * kSlab;
-          prefetch_resid(ncol0, min(kSlab, ncols_valid - ncol0), ebuf + (bufsel ^ 1) * kEpiBufBytes);
-        }
-        for (int sub = 0; sub * 16 < sw; ++sub) {
-          const int c = col0 + sub * 16;
-          const int n = n_base + c;
-          uint32_t v[16];
-          uint32_t g[16];
-          tmem_ld_x16(taddr + c + ((pair_lora && c >= half_cols) ? lr_half : 0), v);
-          if (geglu) tmem_ld_x16(taddr + (bn >> 1) + c, g);
-          if (has_lora && (n < group_lo || n >= group_hi)) {
-            const int grp = n / p.lora_group_n;
-            group_lo = grp * p.lora_group_n;
-            group_hi = group_lo + p.lora_group_n;
-            {
-              uint32_t tv[8];
-              const int j = grp * p.lora_r;
-              tmem_ld_x8(taddr + ((pair_lora && j < lr_half) ? half_cols + j : bn + j), tv);
-              tmem_ld_wait();
-              if (p.ln_cl != nullptr) {
-#pragma unroll
-                for (int jj = 0; jj < 8; ++jj)
-                  tl[jj] = (jj < p.lora_r) ? fmaf(__uint_as_float(tv[jj]), ln_rstd,
-                                                  fmaf(-ln_rm, __ldg(p.ln_cl + j + jj), __ldg(p.ln_dl + j + jj))) * lscale
-                                           : 0.f;
-              } else {
-#pragma unroll
-                for (int jj = 0; jj < 8; ++jj) tl[jj] = __uint_as_float(tv[jj]) * lscale;
-              }
-            }
-          }
-          tmem_ld_wait();
-          float f[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]);
-          if (p.ln_stats != nullptr) {
-            // LN(x) . W^T + b = rstd * acc - rstd * mean * c[n] + d[n]
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              const float4 cc = __ldg(reinterpret_cast<const float4*>(p.ln_c + n) + j4);
-              const float4 dd = __ldg(reinterpret_cast<const float4*>(p.ln_d + n) + j4);
-              f[4 * j4 + 0] = fmaf(f[4 * j4 + 0], ln_rstd, fmaf(-ln_rm, cc.x, dd.x));
-              f[4 * j4 + 1] = fmaf(f[4 * j4 + 1], ln_rstd, fmaf(-ln_rm, cc.y, dd.y));
-              f[4 * j4 + 2] = fmaf(f[4 * j4 + 2], ln_rstd, fmaf(-ln_rm, cc.z, dd.z));
-              f[4 * j4 + 3] = fmaf(f[4 * j4 + 3], ln_rstd, fmaf(-ln_rm, cc.w, dd.w));
-            }
-          }
-          if (staged && sub == 0) {  // this slab's residual / lora_up rows have landed (the next slab's copy may be in flight)
-            if (kEpiBufs == 2 && more)
-              cp_async_wait<1>();
-            else
-              cp_async_wait<0>();
-            __syncwarp();
-          }
-          if (has_lora) {
-            const uint32_t up = ubuf0 + static_cast<uint32_t>(bufsel) * p.up_buf_bytes + sub * 16 * p.lora_r * 4;
-            if (p.lora_r == 4)
-              lora_apply<4>(f, tl, up);
-            else
-              lora_apply<8>(f, tl, up);
-          }
-          if (p.flags & SB200_EPI_BIAS) add_bf16x16(f, p.bias + n);
-          if (rb) add_bf16x16(f, rb + n);
-          if (geglu) {
-            float gb[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) gb[j] = __uint_as_float(g[j]);
-            if (p.ln_stats != nullptr) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                gb[j] = fmaf(gb[j], ln_rstd, fmaf(-ln_rm, __ldg(p.ln_c + p.Nout + n + j), __ldg(p.ln_d + p.Nout + n + j)));
-            }
-            if (p.flags & SB200_EPI_BIAS) add_bf16x16(gb, p.bias + p.Nout + n);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) f[j] *= gelu_erf_f(gb[j]);
-          }
-          const uint32_t a0 = buf + lane * 64 + (((2 * sub) ^ swz) << 4);
-          const uint32_t a1 = buf + lane * 64 + (((2 * sub + 1) ^ swz) << 4);
-          uint32_t o[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) o[j] = pack_bf16x2(f[2 * j], f[2 * j + 1]);
-          if (has_resid && row_ok) {
-            // the residual is added to the ROUNDED projection, in bf16, like the reference's separate elementwise
-            // `hidden_states = attn_output + hidden_states` on two bf16 tensors (8 packed adds instead of 32 fp32 ops)
-            const uint4 r0 = ld_shared_v4(a0), r1 = ld_shared_v4(a1);
-            const uint32_t rw[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-            for (int j = 0; j < 8; ++j) o[j] = add_bf16x2(o[j], rw[j]);
-          }
-          if (p.rs_out != nullptr) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float lo = bf16_lo(o[j]), hi = bf16_hi(o[j]);
-              rs1 += lo + hi;
-              rs2 = fmaf(lo, lo, fmaf(hi, hi, rs2));
-            }
-          }
-          st_shared_v4(a0, make_uint4(o[0], o[1], o[2], o[3]));
-          st_shared_v4(a1, make_uint4(o[4], o[5], o[6], o[7]));
-        }
-        if (!more) {
-          // the accumulator has been read completely: hand it back to the MMA warp before the last copy-out
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if constexpr (kCtas == 2)
-              mbar_arrive_cluster(tempty_leader + 8u * as);
-            else
-              mbar_arrive(bar_tempty + 8u * as);
-          }
-        }
-        __syncwarp();
-        {  // coalesced copy-out of the staged [32 x sw] tile
-          const int cpr = sw >> 3;
-          for (int idx = lane; idx < 32 * cpr; idx += 32) {
-            const int row = cpr == 4 ? idx >> 2 : idx / cpr;
-            const int ch = idx - row * cpr;
-            const int mr = __shfl_sync(0xffffffffu, my_row, row);
-            const uint4 val = ld_shared_v4(buf + row * 64 + ((ch ^ ((row >> 1) & 3)) << 4));
-            if (mr >= 0)
-              *reinterpret_cast<uint4*>(p.out + static_cast<size_t>(mr) * p.ldo + n_base + col0 + ch * 8) = val;
-          }
-        }
-        __syncwarp();
-        if (kEpiBufs == 2) {
-          bufsel ^= 1;
-        } else if (staged && more) {  // single buffer: the next slab's residual / lora_up rows replace what was just copied out
-          const int ncol0 = col0 + kEpiPerQuarter * kSlab;
-          prefetch_resid(ncol0, min(kSlab, ncols_valid - ncol0), ebuf);
-        }
-      }
-      if (my_slabs == 0) {  // nothing to read for this warp (narrow last tile): still release the accumulator
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if constexpr (kCtas == 2)
-            mbar_arrive_cluster(tempty_leader + 8u * as);
-          else
-            mbar_arrive(bar_tempty + 8u * as);
-        }
-      }
-      if (p.rs_out != nullptr) {
-        // The kEpiPerQuarter warps of a lane quarter hold partial sums of the SAME 32 rows (different slabs): combine
-        // them through the quarter's first warp's staging buffer (free between its last copy-out and its next
-        // prefetch), so that a row has one slot per N tile.  Named barrier 1 + q, 32 * kEpiPerQuarter threads.
-        const uint32_t red = tiles + static_cast<uint32_t>(S) * stage_bytes +
-                             static_cast<uint32_t>(q) * (kEpiBytesPerWarp + kEpiBufs * p.up_buf_bytes);
-        asm volatile("bar.sync %0, %1;" ::"r"(1 + q), "r"(32 * kEpiPerQuarter) : "memory");  // first warp done with its buffer
-        if (hsel != 0)
-          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(red + ((hsel - 1) * 32 + lane) * 8), "f"(rs1), "f"(rs2)
-                       : "memory");
-        asm volatile("bar.sync %0, %1;" ::"r"(1 + q), "r"(32 * kEpiPerQuarter) : "memory");
-        if (hsel == 0) {
-#pragma unroll
-          for (int w = 0; w < kEpiPerQuarter - 1; ++w) {
-            float a, b;
-            asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(a), "=f"(b) : "r"(red + (w * 32 + lane) * 8));
-            rs1 += a;
-            rs2 += b;
-          }
-          if (row_ok)
-            reinterpret_cast<float2*>(p.rs_out)[static_cast<size_t>(nt) * p.M + my_row] = make_float2(rs1, rs2);
-        }
-      }
-      as ^= 1;
-      if (as == 0) aphase ^= 1u;
     }
-    if (kStats && warp == 0 && lane == 0) {
-      long long* o = stats_out(p) + blockIdx.x * 8;
-      o[4] = st_wait;
-      o[5] = clock64() - st_t0;
+    const bool row_ok = my_row >= 0;
+    // LayerNorm fold: (mean, rstd) of this thread's row of x from the producer's partial sums, part-major
+    // [parts][M][2]: the 32 rows of a warp read consecutive addresses
+    float ln_rstd = 1.f, ln_rm = 0.f;
+    if (p.ln_stats != nullptr && row_ok) {
+      const float2* ln_sp = reinterpret_cast<const float2*>(p.ln_stats) + my_row;
+      float s1 = 0.f, s2 = 0.f;
+      for (int i = 0; i < p.ln_parts; ++i) {
+        const float2 v2 = __ldg(ln_sp + static_cast<size_t>(i) * p.M);
+        s1 += v2.x;
+        s2 += v2.y;
+      }
+      const float mean = s1 * p.ln_inv_c;
+      ln_rstd = rsqrtf(fmaxf(s2 * p.ln_inv_c - mean * mean, 0.f) + p.ln_eps);
+      ln_rm = ln_rstd * mean;
+    }
+    float rs1 = 0.f, rs2 = 0.f;  // row statistics of what this warp writes in this tile
+    const int n_base = nt * p.ncols_out;
+    const int ncols_valid = min(p.ncols_out, p.Nout - n_base);
+    const int nslabs = (ncols_valid + kSlab - 1) / kSlab;
+    const int my_slabs = (nslabs - hsel + kEpiPerQuarter - 1) / kEpiPerQuarter;  // slabs hsel, hsel + kEpiPerQuarter, ...
+    auto prefetch_resid = [&](int col0, int sw) {
+      const int cpr = sw >> 3;  // 16-byte chunks per row
+      if (has_resid) {
+        for (int idx = lane; idx < 32 * cpr; idx += 32) {
+          const int row = cpr == 4 ? idx >> 2 : idx / cpr;
+          const int ch = idx - row * cpr;
+          const int mr = __shfl_sync(0xffffffffu, my_row, row);
+          if (mr >= 0)
+            cp_async_16(ebuf + row * 64 + ((ch ^ ((row >> 1) & 3)) << 4),
+                        p.resid + static_cast<size_t>(mr) * p.ldr + n_base + col0 + ch * 8);
+        }
+      }
+      if (has_lora && lane < sw) {
+        // this slab's lora_up rows ([r] fp32 per output column) travel with the residual: the rank-r update then
+        // reads them from shared memory instead of taking an L2 round trip per 16 columns inside the loop
+        const uint32_t ub = ubuf + lane * p.lora_r * 4;
+        const float* src = p.lora_up + static_cast<size_t>(n_base + col0 + lane) * p.lora_r;
+        cp_async_16(ub, src);
+        if (p.lora_r == 8) cp_async_16(ub + 16, src + 4);
+      }
+      cp_async_commit();
+    };
+    const bool staged = has_resid || has_lora;
+    if (staged && my_slabs > 0) prefetch_resid(hsel * kSlab, min(kSlab, ncols_valid - hsel * kSlab));
+    const __nv_bfloat16* rb =
+        (p.flags & SB200_EPI_ROWBIAS) ? p.rowbias + static_cast<size_t>(row_ok ? my_batch : 0) * p.Nout : nullptr;
+    float tl[8];
+    int group_lo = 0, group_hi = 0;  // output-column range of the adaptor whose t = A.down^T is held in tl
+    const uint32_t swz = static_cast<uint32_t>((lane >> 1) & 3);
+    for (int k = 0; k < my_slabs; ++k) {
+      const int col0 = (hsel + kEpiPerQuarter * k) * kSlab;
+      const int sw = min(kSlab, ncols_valid - col0);
+      const bool more = k + 1 < my_slabs;
+      for (int sub = 0; sub * 16 < sw; ++sub) {
+        const int c = col0 + sub * 16;
+        const int n = n_base + c;
+        uint32_t v[16];
+        uint32_t g[16];
+        ld_acc<16>(arow + c * 4, v);
+        if (geglu) ld_acc<16>(arow + ((BN >> 1) + c) * 4, g);
+        if (has_lora && (n < group_lo || n >= group_hi)) {
+          const int grp = n / p.lora_group_n;
+          group_lo = grp * p.lora_group_n;
+          group_hi = group_lo + p.lora_group_n;
+          uint32_t tv[8];
+          const int j = grp * p.lora_r;
+          ld_acc<8>(arow + (BN + j) * 4, tv);
+          if (p.ln_cl != nullptr) {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+              tl[jj] = (jj < p.lora_r) ? fmaf(__uint_as_float(tv[jj]), ln_rstd,
+                                              fmaf(-ln_rm, __ldg(p.ln_cl + j + jj), __ldg(p.ln_dl + j + jj))) * lscale
+                                       : 0.f;
+          } else {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) tl[jj] = __uint_as_float(tv[jj]) * lscale;
+          }
+        }
+        float f[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]);
+        if (p.ln_stats != nullptr) {
+          // LN(x) . W^T + b = rstd * acc - rstd * mean * c[n] + d[n]
+#pragma unroll
+          for (int j4 = 0; j4 < 4; ++j4) {
+            const float4 cc = __ldg(reinterpret_cast<const float4*>(p.ln_c + n) + j4);
+            const float4 dd = __ldg(reinterpret_cast<const float4*>(p.ln_d + n) + j4);
+            f[4 * j4 + 0] = fmaf(f[4 * j4 + 0], ln_rstd, fmaf(-ln_rm, cc.x, dd.x));
+            f[4 * j4 + 1] = fmaf(f[4 * j4 + 1], ln_rstd, fmaf(-ln_rm, cc.y, dd.y));
+            f[4 * j4 + 2] = fmaf(f[4 * j4 + 2], ln_rstd, fmaf(-ln_rm, cc.z, dd.z));
+            f[4 * j4 + 3] = fmaf(f[4 * j4 + 3], ln_rstd, fmaf(-ln_rm, cc.w, dd.w));
+          }
+        }
+        if (staged && sub == 0) {  // this slab's residual / lora_up rows have landed
+          cp_async_wait<0>();
+          __syncwarp();
+        }
+        if (has_lora) {
+          const uint32_t up = ubuf + sub * 16 * p.lora_r * 4;
+          if (p.lora_r == 4)
+            lora_apply<4>(f, tl, up);
+          else
+            lora_apply<8>(f, tl, up);
+        }
+        if (p.flags & SB200_EPI_BIAS) add_bf16x16(f, p.bias + n);
+        if (rb) add_bf16x16(f, rb + n);
+        if (geglu) {
+          float gb[16];
+#pragma unroll
+          for (int j = 0; j < 16; ++j) gb[j] = __uint_as_float(g[j]);
+          if (p.ln_stats != nullptr) {
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+              gb[j] = fmaf(gb[j], ln_rstd, fmaf(-ln_rm, __ldg(p.ln_c + p.Nout + n + j), __ldg(p.ln_d + p.Nout + n + j)));
+          }
+          if (p.flags & SB200_EPI_BIAS) add_bf16x16(gb, p.bias + p.Nout + n);
+#pragma unroll
+          for (int j = 0; j < 16; ++j) f[j] *= gelu_erf_f(gb[j]);
+        }
+        const uint32_t a0 = ebuf + lane * 64 + (((2 * sub) ^ swz) << 4);
+        const uint32_t a1 = ebuf + lane * 64 + (((2 * sub + 1) ^ swz) << 4);
+        uint32_t o[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[j] = pack_bf16x2(f[2 * j], f[2 * j + 1]);
+        if (has_resid && row_ok) {
+          // the residual is added to the ROUNDED projection, in bf16, like the reference's separate elementwise
+          // `hidden_states = attn_output + hidden_states` on two bf16 tensors
+          const uint4 r0 = ld_shared_v4(a0), r1 = ld_shared_v4(a1);
+          const uint32_t rw[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
+#pragma unroll
+          for (int j = 0; j < 8; ++j) o[j] = add_bf16x2(o[j], rw[j]);
+        }
+        if (p.rs_out != nullptr) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float lo = bf16_lo(o[j]), hi = bf16_hi(o[j]);
+            rs1 += lo + hi;
+            rs2 = fmaf(lo, lo, fmaf(hi, hi, rs2));
+          }
+        }
+        st_shared_v4(a0, make_uint4(o[0], o[1], o[2], o[3]));
+        st_shared_v4(a1, make_uint4(o[4], o[5], o[6], o[7]));
+      }
+      __syncwarp();
+      {  // coalesced copy-out of the staged [32 x sw] tile
+        const int cpr = sw >> 3;
+        for (int idx = lane; idx < 32 * cpr; idx += 32) {
+          const int row = cpr == 4 ? idx >> 2 : idx / cpr;
+          const int ch = idx - row * cpr;
+          const int mr = __shfl_sync(0xffffffffu, my_row, row);
+          const uint4 val = ld_shared_v4(ebuf + row * 64 + ((ch ^ ((row >> 1) & 3)) << 4));
+          if (mr >= 0)
+            *reinterpret_cast<uint4*>(p.out + static_cast<size_t>(mr) * p.ldo + n_base + col0 + ch * 8) = val;
+        }
+      }
+      __syncwarp();
+      if (staged && more) {  // the next slab's residual / lora_up rows replace what was just copied out
+        const int ncol0 = col0 + kEpiPerQuarter * kSlab;
+        prefetch_resid(ncol0, min(kSlab, ncols_valid - ncol0));
+      }
+    }
+    if (p.rs_out != nullptr) {
+      // The kEpiPerQuarter warps of a quarter hold partial sums of the SAME 32 rows (different slabs): combine them
+      // through the quarter's first warp's staging buffer (free after its last copy-out), so that a row has one slot
+      // per N tile.  Named barrier 1 + q, 32 * kEpiPerQuarter threads.
+      const uint32_t red = tiles + static_cast<uint32_t>(p.ring_bytes) +
+                           static_cast<uint32_t>(q) * (kEpiBufBytes + p.up_buf_bytes);
+      asm volatile("bar.sync %0, %1;" ::"r"(1 + q), "r"(32 * kEpiPerQuarter) : "memory");  // first warp done with its buffer
+      if (hsel != 0)
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(red + ((hsel - 1) * 32 + lane) * 8), "f"(rs1), "f"(rs2)
+                     : "memory");
+      asm volatile("bar.sync %0, %1;" ::"r"(1 + q), "r"(32 * kEpiPerQuarter) : "memory");
+      if (hsel == 0) {
+#pragma unroll
+        for (int w = 0; w < kEpiPerQuarter - 1; ++w) {
+          float a, b;
+          asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(a), "=f"(b) : "r"(red + (w * 32 + lane) * 8));
+          rs1 += a;
+          rs2 += b;
+        }
+        if (row_ok) reinterpret_cast<float2*>(p.rs_out)[static_cast<size_t>(nt) * p.M + my_row] = make_float2(rs1, rs2);
+      }
     }
   }
 
-  __syncwarp();
-  tc_fence_before();
   if constexpr (kCtas == 2) {
-    cluster_sync_all();  // the peer's barriers / smem must outlive every multicast arrive aimed at them
-  } else {
-    __syncthreads();
-  }
-  if (warp == 2) {
-    tc_fence_after();
-    if constexpr (kCtas == 2)
-      tmem_dealloc_2cta(tmem_base, 512);
-    else
-      tmem_dealloc(tmem_base, 512);
+    __syncwarp();
+    cluster_sync_all();  // the peer's barriers / smem must outlive every multicast and remote arrive aimed at them
   }
 }
 
@@ -838,59 +579,75 @@ static int env_int(const char* name, int dflt) {
   return (e && e[0]) ? atoi(e) : dflt;
 }
 
-// SB200_PAIR: 0 = never use the CTA-pair kernel, 1 = whenever the cost model prefers it (default), 2 = always.
-static int pair_policy() {
-  static const int v = env_int("SB200_PAIR", 1);
+// SB200_PAIR=2 runs every GEMM / conv as CTA pairs; otherwise pairs run only where the caller forces them (bit 12 of
+// bn).  Pairs are opt-in: they halve the weight traffic from L2, but they never need fewer waves than single CTAs (a
+// pair is two CTAs on two row tiles), and these tiles are not L2-bound: on an H100 at 400 W, 8192 x 1280 x 1280 takes
+// 69 us single / 105 us paired, 8192 x 10240 x 1280 576 / 1056 us, 2048 x 640 x 640 20.5 / 21.9 us.
+static bool pairs_always() {
+  static const bool v = env_int("SB200_PAIR", 0) == 2;
   return v;
 }
 
-// Cost model in SM cycles, fitted to the round-2 same-box measurements (profiles/r02_gemm_matrix_v2_two_producers.log,
-// r02_gemm_stats_two_producers.log: cycles per 64-deep k-block from the kStats build):
-//   CTA pair    max(2 (bn + rt), ~325)      tensor-bound from bn = 176 up, below that the two producer warps' issue
-//               rate (3 TMA instructions per k-block with LoRA: +40)
-//   single CTA  ~390 + (bn + rt) / 2        (524 at 256, 456 at 128, 415 at 64)
-// A tile costs kblocks of those plus ~600 cycles of hand-over; its epilogue (~14 cycles per output column, more with a
-// residual / LoRA / GEGLU) overlaps the next tile's main loop unless it is longer; work is dealt in waves over the
-// persistent units; a launch pays its prologue, the last tile's epilogue and, for the pair, cluster launch / sync.
-static TileChoice pick_tile(int M, int ncols, int max_bn, int step, int num_sms, int kblocks, int lora_rt,
-                            int force_ctas, int sub_tiles, int flags) {
+// Tile widths the kernel is instantiated for (a 256-wide accumulator does not fit the registers of 288 threads).
+static bool bn_supported(int bn) { return bn == 64 || bn == 128; }
+
+// Tile width from a cost model in SM cycles.  A 128 x bn tile's 64-deep k-block takes 4 bn cycles of tensor work (m64
+// wgmmas of two warpgroups at 4096 bf16 FLOP / clk / SM) plus the LoRA columns; a tile pays ~2000 cycles of prologue
+// and pipeline fill and an epilogue of ~14 cycles per output column (more with a residual / LoRA / GEGLU).  One CTA per
+// SM: work is dealt in waves of num_sms tiles.
+static TileChoice pick_tile(int ncols, int num_sms, int kblocks, int lora_rt, int force_ctas, int sub_tiles, int flags) {
   double best = -1;
-  TileChoice bc{1, step};
-  const int pol = pair_policy();
+  TileChoice bc{1, 64};
+  const int ctas = force_ctas ? force_ctas : (pairs_always() ? 2 : 1);
   const bool geglu = (flags & SB200_EPI_GEGLU) != 0;
   const double epi_per_col = 14.0 + ((flags & SB200_EPI_RESID) ? 5.0 : 0.0) + (lora_rt ? 6.0 : 0.0) + (geglu ? 10.0 : 0.0);
-  for (int ctas = 1; ctas <= 2; ++ctas) {
-    if (force_ctas ? ctas != force_ctas : ((pol == 0 && ctas == 2) || (pol == 2 && ctas == 1))) continue;
-    const int m_tiles = (sub_tiles + ctas - 1) / ctas;
-    const int units = num_sms / ctas;
-    const int bstep = (ctas == 2 && (lora_rt || step == 32)) ? 32 : step;
-    for (int bn = bstep; bn <= max_bn; bn += bstep) {
-      const int n_tiles = (ncols + bn - 1) / bn;
-      const long tiles = static_cast<long>(m_tiles) * n_tiles;
-      const long waves = (tiles + units - 1) / units;
-      const double wide = 2.0 * (bn + lora_rt);
-      const double perkb = ctas == 2 ? (wide > 325.0 + (lora_rt ? 40.0 : 0.0) ? wide : 325.0 + (lora_rt ? 40.0 : 0.0))
-                                     : 390.0 + 0.25 * wide;
-      const double epi = 400.0 + epi_per_col * (geglu ? bn / 2 : bn);
-      const double main_loop = kblocks * perkb + 600.0;
-      const double tile = main_loop > epi ? main_loop : epi;
-      const double cost = waves * tile + 4000.0 + epi + (ctas == 2 ? 3000.0 : 0.0);
-      if (best < 0 || cost < best - 1e-9 || (cost < best + 1e-9 && bn > bc.bn)) {
-        best = cost;
-        bc = TileChoice{ctas, bn};
-      }
+  for (int bn = 64; bn <= 128; bn *= 2) {
+    const long tiles = static_cast<long>(sub_tiles) * ((ncols + bn - 1) / bn);
+    const long waves = (tiles + num_sms - 1) / num_sms;
+    const double perkb = 4.0 * (bn + lora_rt) + 64.0;
+    const double cost = waves * (kblocks * perkb + 2000.0 + epi_per_col * (geglu ? bn / 2 : bn));
+    if (best < 0 || cost < best - 1e-9 || (cost < best + 1e-9 && bn > bc.bn)) {
+      best = cost;
+      bc = TileChoice{ctas, bn};
     }
   }
-  (void)M;
   return bc;
 }
 
 static bool n_fast_default() {
   static const bool v = [] {
-    const char* e = getenv("SB200_TILE_ORDER");  // "m" restores the M-fastest order (same-box A/B)
+    const char* e = getenv("SB200_TILE_ORDER");  // "m" restores the M-fastest order
     return !(e && e[0] == 'm');
   }();
   return v;
+}
+
+template <int BN, int kCtas, int RT>
+static int launch_gemm_bn(Ctx* ctx, cudaStream_t stream, const GemmParams& p, int smem) {
+  static bool attr_set = false;  // one flag per instantiation
+  if (!attr_set) {
+    SB200_CUDA_CHECK(
+        cudaFuncSetAttribute(gemm_kernel<BN, kCtas, RT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
+    attr_set = true;
+  }
+  const int total = p.num_m_tiles * p.num_n_tiles;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(total * kCtas);
+  cfg.blockDim = dim3(kGemmThreads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = (pdl_mode() == 2 || (pdl_mode() == 1 && pdl_hint())) ? 1 : 0;
+  attr[1].id = cudaLaunchAttributeClusterDimension;
+  attr[1].val.clusterDim.x = kCtas;
+  attr[1].val.clusterDim.y = 1;
+  attr[1].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = kCtas == 2 ? 2 : 1;
+  SB200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_kernel<BN, kCtas, RT>, p));
+  (void)ctx;
+  return 0;
 }
 
 static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
@@ -900,97 +657,42 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
   {
     const double w_bytes = 2.0 * p.N * p.K;
     const double a_bytes_total = 2.0 * p.M * (p.a_mode == 0 ? p.K : p.K / 9);
-    p.n_fast = (n_fast_default() && !(w_bytes > a_bytes_total && w_bytes > 64e6)) ? 1 : 0;
+    p.n_fast = (n_fast_default() && !(w_bytes > a_bytes_total && w_bytes > 32e6)) ? 1 : 0;
   }
-  // two k-blocks per elect region pays for tiles whose 4 UMMAs (2 (bn + rt) cycles) are shorter than one pass of the
-  // issue loop; wide tiles run better with one (same-box A/B, profiles/r02_gemm_tiles.txt)
-  static const int unroll_env = env_int("SB200_MMA_UNROLL", -1);
-  const int unroll2 = unroll_env >= 0 ? unroll_env : (p.bn + p.lora_rt <= 160 ? 1 : 0);
-  p.mma_unroll2 = (unroll2 != 0) != ((p.debug & 16) != 0);  // debug bit 4 flips it (same-box A/B)
   const bool has_lora = p.flags & SB200_EPI_LORA;
   p.b_rows = p.bn / ctas;
   p.l_rows = has_lora ? p.lora_rt / ctas : 0;
-  p.stage_bytes = kBM * 128 + p.b_rows * 128 + p.l_rows * 128;
+  p.stage_bytes = kBM * 128 + p.bn * 128 + (has_lora ? p.lora_rt * 128 : 0);
   p.up_buf_bytes = has_lora ? kSlab * p.lora_r * 4 : 0;
-  const int epi_bytes = kEpiBytes + kEpiWarps * kEpiBufs * p.up_buf_bytes;
+  const int epi_bytes = kEpiBytes + kEpiWarps * p.up_buf_bytes;
   int stages = (kSmemBudget - kBarRegion - 1024 - epi_bytes) / p.stage_bytes;
   if (stages > kMaxStages) stages = kMaxStages;
   if (stages < 2) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
   p.stages = stages;
-  const int smem = kBarRegion + 1024 + stages * p.stage_bytes + epi_bytes;
-  if (!ctx->gemm_attr_set) {
-    SB200_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
-    SB200_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
-    ctx->gemm_attr_set = true;
+  p.ring_bytes = stages * p.stage_bytes;
+  if (p.ring_bytes < acc_tile_bytes(p.bn)) p.ring_bytes = acc_tile_bytes(p.bn);
+  const int smem = kBarRegion + 1024 + p.ring_bytes + epi_bytes;
+  if (smem > kSmemBudget) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
+  pdl_hint() = p.num_m_tiles * p.num_n_tiles * ctas <= 2 * ctx->num_sms;
+  const int rt = has_lora ? p.lora_rt : 0;
+  const int variant = (ctas == 2 ? 6 : 0) + (p.bn == 128 ? 3 : 0) + (rt == 16 ? 1 : (rt == 32 ? 2 : 0));
+  cudaStream_t s = stream;
+  int st;
+  switch (variant) {
+    case 0: st = launch_gemm_bn<64, 1, 0>(ctx, s, p, smem); break;
+    case 1: st = launch_gemm_bn<64, 1, 16>(ctx, s, p, smem); break;
+    case 2: st = launch_gemm_bn<64, 1, 32>(ctx, s, p, smem); break;
+    case 3: st = launch_gemm_bn<128, 1, 0>(ctx, s, p, smem); break;
+    case 4: st = launch_gemm_bn<128, 1, 16>(ctx, s, p, smem); break;
+    case 5: st = launch_gemm_bn<128, 1, 32>(ctx, s, p, smem); break;
+    case 6: st = launch_gemm_bn<64, 2, 0>(ctx, s, p, smem); break;
+    case 7: st = launch_gemm_bn<64, 2, 16>(ctx, s, p, smem); break;
+    case 8: st = launch_gemm_bn<64, 2, 32>(ctx, s, p, smem); break;
+    case 9: st = launch_gemm_bn<128, 2, 0>(ctx, s, p, smem); break;
+    case 10: st = launch_gemm_bn<128, 2, 16>(ctx, s, p, smem); break;
+    default: st = launch_gemm_bn<128, 2, 32>(ctx, s, p, smem); break;
   }
-  const int total = p.num_m_tiles * p.num_n_tiles;
-  pdl_hint() = total <= 2 * ctx->num_sms;
-  const bool stats = (p.debug & 32) != 0;
-  if (stats && !ctx->gemm_stats_attr_set) {
-    SB200_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
-    SB200_CUDA_CHECK(cudaFuncSetAttribute(gemm_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
-    ctx->gemm_stats_attr_set = true;
-  }
-  if (ctas == 1) {
-    const int grid = total < ctx->num_sms ? total : ctx->num_sms;
-    if (stats)
-      SB200_CUDA_CHECK(launch_pdl(gemm_kernel<1, true>, dim3(grid), dim3(kGemmThreads), smem, stream, p));
-    else
-      SB200_CUDA_CHECK(launch_pdl(gemm_kernel<1>, dim3(grid), dim3(kGemmThreads), smem, stream, p));
-  } else {
-    const int csize = p.quad ? 4 : 2;
-    int units = ctx->num_sms / csize;
-    int work = total;
-    if (p.quad) {
-      // clusters of four must fit inside a GPC: ask the driver how many are resident at once (once per context)
-      static int quad_clusters = 0;
-      if (quad_clusters == 0) {
-        cudaLaunchConfig_t qc;
-        memset(&qc, 0, sizeof(qc));
-        qc.gridDim = dim3(4 * (ctx->num_sms / 4));
-        qc.blockDim = dim3(kGemmThreads);
-        qc.dynamicSmemBytes = kSmemBudget;
-        cudaLaunchAttribute qa;
-        qa.id = cudaLaunchAttributeClusterDimension;
-        qa.val.clusterDim.x = 4;
-        qa.val.clusterDim.y = 1;
-        qa.val.clusterDim.z = 1;
-        qc.attrs = &qa;
-        qc.numAttrs = 1;
-        int n = 0;
-        if (cudaOccupancyMaxActiveClusters(&n, gemm_kernel<2>, &qc) != cudaSuccess || n <= 0) {
-          cudaGetLastError();
-          n = ctx->num_sms / 4;
-        }
-        quad_clusters = n < ctx->num_sms / 4 ? n : ctx->num_sms / 4;
-      }
-      units = quad_clusters;
-      work = p.num_m_tiles * (p.num_n_tiles / 2);
-    }
-    const int grid = csize * (work < units ? work : units);
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kGemmThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = csize;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    // programmatic dependent launch like launch_pdl() gives the single-CTA kernel (SB200_PDL_PAIR=0: same-box A/B)
-    static const int pdl_pair = env_int("SB200_PDL_PAIR", 1);
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed =
-        (pdl_pair && (pdl_mode() == 2 || (pdl_mode() == 1 && pdl_hint()))) ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 2;
-    if (stats)
-      SB200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_kernel<2, true>, p));
-    else
-      SB200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_kernel<2>, p));
-  }
+  if (st) return st;
   SB200_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -1005,10 +707,9 @@ static int check_lora(const sb200_lora* l, int N) {
   return 0;
 }
 
-// bn encodes an explicit choice when > 0: low 12 bits = tile width, bit 12 set = force the CTA-pair kernel,
-// bit 13 set = force the single-CTA kernel (used by the tests to cover both), bits 14.. = debug bits.
-static void decode_bn(int bn_arg, int* bn, int* force_ctas, int* debug = nullptr) {
-  if (debug) *debug = bn_arg > 0 ? (bn_arg >> 14) & 63 : 0;
+// bn encodes an explicit choice when > 0: low 12 bits = tile width, bit 12 set = force CTA pairs, bit 13 set = force
+// single CTAs (used by the tests to cover both).
+static void decode_bn(int bn_arg, int* bn, int* force_ctas) {
   *force_ctas = (bn_arg > 0 && (bn_arg & 0x1000)) ? 2 : ((bn_arg > 0 && (bn_arg & 0x2000)) ? 1 : 0);
   *bn = bn_arg > 0 ? (bn_arg & 0xFFF) : 0;
 }
@@ -1071,22 +772,17 @@ extern "C" int sb200_gemm_ln(void* handle, void* stream, const void* x0, int ldx
   p.cb_total = p.kblocks;
   p.a_tx = kBM * 128;
   p.num_sub = (M + kBM - 1) / kBM;
-  int max_bn = 256;
   if (has_lora) {
     int st = check_lora(lora, N);
     if (st) return st;
-    max_bn = 256 - lora->rt;
     fill_lora(p, lora);
   }
-  const int step = geglu ? 32 : 16;
   int bn, force_ctas;
-  decode_bn(bn_arg, &bn, &force_ctas, &p.debug);
-  TileChoice tc = pick_tile(M, N, max_bn, step, ctx->num_sms, p.kblocks, has_lora ? lora->rt : 0, force_ctas, p.num_sub, flags);
+  decode_bn(bn_arg, &bn, &force_ctas);
+  TileChoice tc = pick_tile(N, ctx->num_sms, p.kblocks, has_lora ? lora->rt : 0, force_ctas, p.num_sub, flags);
   if (bn > 0) tc.bn = bn;
   if (force_ctas) tc.ctas = force_ctas;
-  const int need = (tc.ctas == 2 && (has_lora || geglu)) ? 32 : step;
-  SB200_REQUIRE(tc.bn % need == 0 && tc.bn >= need && tc.bn <= max_bn, "gemm: bn=%d invalid (step %d, max %d)",
-                tc.bn, need, max_bn);
+  SB200_REQUIRE(bn_supported(tc.bn), "gemm: bn=%d invalid (64 or 128)", tc.bn);
   p.bn = tc.bn;
   p.ncols_out = geglu ? tc.bn / 2 : tc.bn;
   p.num_m_tiles = (p.num_sub + tc.ctas - 1) / tc.ctas;
@@ -1144,26 +840,6 @@ extern "C" int sb200_gemm_ln(void* handle, void* stream, const void* x0, int ldx
     const uint64_t strides[1] = {static_cast<uint64_t>(K) * 2};
     const uint32_t box[2] = {kBK, static_cast<uint32_t>(lora->rt / tc.ctas)};
     if ((st = make_tmap_bf16(ctx, &p.tmL, lora->down, 2, dims, strides, box))) return st;
-  }
-  // 2x2 clusters with the A tile multicast to both pairs: for shapes that stream more bytes from L2 than the tensor
-  // pipe can cover (narrow tiles: the N = 1280 projections).  SB200_QUAD: 0 off, 1 = tiles up to 192 wide, 2 = always.
-  {
-    static const int quad_env = env_int("SB200_QUAD", 0);
-    const bool want = quad_env >= 2 || (quad_env == 1 && tc.bn + (has_lora ? lora->rt : 0) <= 208);
-    if (want && tc.ctas == 2 && !geglu && p.num_n_tiles % 2 == 0 && p.num_n_tiles >= 2) {
-      p.quad = 1;
-      const uint32_t hbox[2] = {kBK, kBM / 2};
-      {
-        const uint64_t dims[2] = {static_cast<uint64_t>(K0), static_cast<uint64_t>(M)};
-        const uint64_t strides[1] = {static_cast<uint64_t>(ldx0) * 2};
-        if ((st = make_tmap_bf16(ctx, &p.tmA[2], x0, 2, dims, strides, hbox))) return st;
-      }
-      if (split) {
-        const uint64_t dims[2] = {static_cast<uint64_t>(K - K0), static_cast<uint64_t>(M)};
-        const uint64_t strides[1] = {static_cast<uint64_t>(ldx1) * 2};
-        if ((st = make_tmap_bf16(ctx, &p.tmA[3], x1, 2, dims, strides, hbox))) return st;
-      }
-    }
   }
   return launch_gemm(ctx, static_cast<cudaStream_t>(stream), p, tc.ctas);
 }
@@ -1240,20 +916,17 @@ extern "C" int sb200_conv3x3(void* handle, void* stream, const void* x0, int ldx
   p.tiles_h = (H + bh - 1) / bh;
   p.num_sub = p.tiles_w * p.tiles_h * ((B + bb - 1) / bb);
   p.a_tx = bw * bh * bb * 128;
-  int max_bn = 256;
   if (has_lora) {
     int st = check_lora(lora, Cout);
     if (st) return st;
-    max_bn = 256 - lora->rt;
     fill_lora(p, lora);
   }
   int bn, force_ctas;
-  decode_bn(bn_arg, &bn, &force_ctas, &p.debug);
-  TileChoice tc = pick_tile(M, Cout, max_bn, 16, ctx->num_sms, p.kblocks, has_lora ? lora->rt : 0, force_ctas, p.num_sub, flags);
+  decode_bn(bn_arg, &bn, &force_ctas);
+  TileChoice tc = pick_tile(Cout, ctx->num_sms, p.kblocks, has_lora ? lora->rt : 0, force_ctas, p.num_sub, flags);
   if (bn > 0) tc.bn = bn;
   if (force_ctas) tc.ctas = force_ctas;
-  const int need = (tc.ctas == 2 && has_lora) ? 32 : 16;
-  SB200_REQUIRE(tc.bn % need == 0 && tc.bn >= need && tc.bn <= max_bn, "conv3x3: bn=%d invalid (step %d)", tc.bn, need);
+  SB200_REQUIRE(bn_supported(tc.bn), "conv3x3: bn=%d invalid (64 or 128)", tc.bn);
   p.bn = tc.bn;
   p.ncols_out = tc.bn;
   p.num_m_tiles = (p.num_sub + tc.ctas - 1) / tc.ctas;

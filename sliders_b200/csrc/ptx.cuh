@@ -1,11 +1,13 @@
-// sm_100a PTX primitives shared by the sliders_b200 kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / st) and the UMMA shared-memory + instruction descriptors.
+// sm_90a PTX primitives shared by the sliders_b200 kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma fences and
+// shared-memory descriptors (the instructions themselves are in wgmma.cuh), cluster multicast.
 // Everything here is inline PTX; there is no CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace sb200 {
 
@@ -25,7 +27,7 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 // start while its stream predecessor is still running; pdl_wait() blocks until the predecessor grid has completed and
 // its writes are visible (a no-op for ordinary launches), pdl_trigger() lets the successor's CTAs be scheduled early.
 // Every kernel calls pdl_trigger() first and pdl_wait() before its first global-memory access, so only the prologue
-// (barrier init, TMEM allocation, descriptor prefetch) and the launch latency overlap the predecessor's tail.
+// (barrier init, descriptor prefetch) and the launch latency overlap the predecessor's tail.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
@@ -73,16 +75,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Blocking wait with a watchdog: a protocol bug becomes a trapped launch, not a hung GPU.
+// Blocking wait with a watchdog: a protocol bug becomes a trapped launch (an unspecified launch failure on the host),
+// not a hung GPU.  No printf here: a call inside a warpgroup's MMA loop makes ptxas serialise its wgmma instructions.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > SB200_WATCHDOG_CYCLES) {
-      printf("sb200: mbarrier watchdog (block %d thread %d bar 0x%x parity %u)\n", blockIdx.x,
-             threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (clock64() - t0 > SB200_WATCHDOG_CYCLES) __trap();
   }
 }
 
@@ -122,140 +121,30 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* m, 
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05: tensor memory allocation, MMA issue, commit, loads/stores
+// wgmma (warpgroup MMA): fences, commit / wait groups and the shared-memory matrix descriptor
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_slot),
-               "r"(ncols)
-               : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]; A is read from tensor memory (K-major only).
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n"
-      :
-      : "r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once every MMA issued so far by this thread has completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   bar)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
+// Keeps the compiler from moving accumulator accesses across a wgmma wait.
+__device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
-// 32 lanes x 32 bit, N consecutive columns: thread t of the warp receives lane (base_lane + t).
-__device__ __forceinline__ void tmem_ld_x8(uint32_t taddr, uint32_t* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-                 "=r"(v[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      :
-      : "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]),
-        "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]),
-        "r"(v[15])
-      : "memory");
+// Descriptor of a 128-byte-swizzled tile whose rows are 128 B (64 bf16), as TMA writes it with SWIZZLE_128B:
+//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4 (unused by these layouts: 1)
+//   bits [32,46) stride byte offset >> 4   bits [62,64) layout type (1 = SWIZZLE_128B)
+// K-major operand (rows = M or N, 64 K-elements per row): SBO = 1024 B (one 8-row swizzle atom); a 16-element k-step
+// inside the row adds 32 B to the start address.  MN-major operand (rows = K, 64 MN-elements per row): SBO = 1024 B
+// between groups of 8 K-rows; a 16-row k-step adds 2048 B.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) {
+  return static_cast<uint64_t>((saddr & 0x3FFFF) >> 4) | (static_cast<uint64_t>(1) << 16) |
+         (static_cast<uint64_t>(1024 >> 4) << 32) | (static_cast<uint64_t>(1) << 62);
 }
 
 // ---------------------------------------------------------------------------------------------
-// UMMA descriptors
-// ---------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a 128-byte-swizzled tile whose rows are 128 B (64 bf16):
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1 (Blackwell)
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
-// K-major operand (rows = M or N, 64 K-elements per row): SBO = 1024 B (one 8-row swizzle atom),
-// LBO unused. MN-major operand (rows = K, 64 MN-elements per row): SBO = 1024 B between groups of
-// 8 K-rows, LBO = stride between 64-element MN atoms (unused when the MN extent is 64).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes = 0) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// Instruction descriptor, kind::f16: bf16 x bf16 -> fp32.
-//   [4,6) D format (1 = f32)   [7,10) A format (1 = bf16)   [10,13) B format (1 = bf16)
-//   [15] A major (0 = K)       [16] B major (0 = K, 1 = MN)
-//   [17,23) N >> 3             [24,29) M >> 4
-__host__ __device__ __forceinline__ uint32_t umma_idesc_bf16(int m, int n, int b_mn_major = 0) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(b_mn_major) << 16) |
-         (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-
-// ---------------------------------------------------------------------------------------------
-// CTA pairs (thread-block cluster of 2, tcgen05 cta_group::2): one UMMA spans both SMs' tensor memory
-// (rows 0..127 in the leader CTA, 128..255 in the peer), each CTA stages its own A rows and HALF of the
-// B tile, which is what lifts the per-SM shared-memory fill rate below the tensor-core rate.
+// Thread-block clusters: a pair of CTAs shares the weight tile, each loads half of it and multicasts it to both.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -263,7 +152,7 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
   return r;
 }
 __device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 // shared::cluster address of the same smem offset in CTA `rank` of the cluster
 __device__ __forceinline__ uint32_t mapa_u32(uint32_t saddr, uint32_t rank) {
@@ -272,72 +161,17 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t saddr, uint32_t rank) {
   return r;
 }
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
 }
-// 2-CTA TMA loads: data lands in the issuing CTA's smem, the transaction bytes are signalled on the
-// mbarrier at `cluster_bar` (the LEADER CTA's barrier, a shared::cluster address).
-__device__ __forceinline__ void tma_load_2d_2cta(uint32_t dst, const CUtensorMap* m, uint32_t cluster_bar,
-                                                 int c0, int c1) {
+// The box lands at offset `dst` in every CTA of `cta_mask`; each destination's transaction bytes are signalled on the
+// mbarrier at offset `bar` in that CTA.
+__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1,
+                                               uint16_t cta_mask) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      :
-      : "r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(cluster_bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-// The same load multicast to the CTAs in `cta_mask`: the box lands at offset `dst` in each of them and each
-// destination's transaction bytes are signalled at the barrier offset / peer bit given by `bar` inside the DESTINATION's
-// own CTA pair (so `bar` = this CTA's barrier address with the peer bit cleared = "the leader of the pair").
-__device__ __forceinline__ void tma_load_2d_2cta_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1,
-                                                    uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
       " [%0], [%1, {%4, %5}], [%2], %3;"
       :
       : "r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "h"(cta_mask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2cta(uint32_t dst, const CUtensorMap* m, uint32_t cluster_bar,
-                                                 int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      :
-      : "r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(cluster_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_slot),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2cta() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// D[tmem of both CTAs] (+)= A[smem, 128 rows per CTA] * B[smem, N/2 rows per CTA]; issued by ONE thread
-// of the leader CTA.
-__device__ __forceinline__ void umma_ss_2cta(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive (once the MMAs issued so far retire) on the mbarrier at this smem offset in every CTA of `mask`.
-__device__ __forceinline__ void umma_commit_2cta(uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          bar),
-      "h"(mask)
       : "memory");
 }
 

@@ -72,7 +72,7 @@ class LoRAModule(nn.Module):
     def forward(self, x):
         raise RuntimeError(
             f"{self.lora_name}: the adapted leaf was called through PyTorch.  In sliders_b200 the LoRA delta is "
-            "fused into the tcgen05 GEMM/conv kernels (UNet2DConditionModel.forward); there is no eager path.")
+            "fused into the wgmma GEMM/conv kernels (UNet2DConditionModel.forward); there is no eager path.")
 
 
 class LoRANetwork(nn.Module):

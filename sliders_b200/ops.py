@@ -29,7 +29,7 @@ def _stream() -> C.c_void_p:
 
 def _ctx(t: torch.Tensor):
     if not t.is_cuda:
-        raise _cabi.Sb200Error("sliders_b200 kernels need CUDA tensors on a B200 (no CPU fallback)")
+        raise _cabi.Sb200Error("sliders_b200 kernels need CUDA tensors on an H100 (no CPU fallback)")
     return _cabi.handle(t.device.index if t.device.index is not None else torch.cuda.current_device())
 
 
@@ -132,7 +132,7 @@ def gemm(x: torch.Tensor, w: torch.Tensor, *, bias=None, rowbias=None, rows_per_
          geglu: bool = False, lora: Optional[Lora] = None, x1: Optional[torch.Tensor] = None,
          out: Optional[torch.Tensor] = None, bn: int = 0, ln: Optional[LnFold] = None,
          rowstats: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """out[M,N] = epilogue([x | x1] @ w.T): one tcgen05 `gemm_kernel` launch.  `ln`: the rows of x are un-normalised and
+    """out[M,N] = epilogue([x | x1] @ w.T): one wgmma `gemm_kernel` launch.  `ln`: the rows of x are un-normalised and
     w is gamma-scaled (LayerNorm fold); `rowstats` [M, cap, 2] fp32: leave per-row partial (sum, sum of squares) of the
     output for a later `ln` (the number of slots used is `ops.last_rowstats_parts`)."""
     M, K0 = x.shape
@@ -460,7 +460,7 @@ def colsum(dy: torch.Tensor) -> torch.Tensor:
 
 def _wgrad_ws(Cc: int, r: int, device) -> torch.Tensor:
     cblocks = (Cc // 8 + 31) // 32
-    chunks = min(256, (296 + cblocks - 1) // cblocks)
+    chunks = min(256, (264 + cblocks - 1) // cblocks)
     return torch.empty(chunks * Cc * r, device=device, dtype=torch.float32)
 
 

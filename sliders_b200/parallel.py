@@ -1,5 +1,5 @@
 """Multi-GPU fan-out of conditioned eps-predictions (SURVEY.md §8e): one process per GPU (torchrun),
-`torch.distributed` for the plumbing (NCCL over NVLink on the B200 box, gloo in the CPU tests).
+`torch.distributed` for the plumbing (NCCL over NVLink between GPUs, gloo in the CPU tests).
 
 The reference is single-process (`--device N`, train_lora_xl.py:414).  What shards naturally is the batch of
 *independent* conditioned passes: the 4 predictions x CFG halves of a text-slider iteration

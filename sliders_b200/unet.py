@@ -1,10 +1,10 @@
-"""B200-native replacement for the `unet(...)` call of the reference slider trainers / samplers.
+"""H100-native replacement for the `unet(...)` call of the reference slider trainers / samplers.
 
 `UNet2DConditionModel` here is NOT the diffusers network: it is a parameter container whose module tree,
 attribute names and class names mirror diffusers 0.20.2 exactly (so that `LoRANetwork.create_modules`,
 reference trainscripts/textsliders/lora.py:164-218, discovers the same 346 / 150 leaves and writes the same
 checkpoint keys, and so that Hugging Face `unet/diffusion_pytorch_model.safetensors` state dicts load with
-`load_state_dict`), plus a forward that runs entirely in the hand-written sm_100a kernels of libsb200.so
+`load_state_dict`), plus a forward that runs entirely in the hand-written sm_90a kernels of libsb200.so
 (ops.py).  None of the leaf modules' own `forward`s are ever executed.
 
 Call-site compatibility (reference): `unet(sample, timestep, encoder_hidden_states=…,
@@ -697,7 +697,7 @@ class UNet2DConditionModel(nn.Module):
 
     def _forward_nograd(self, sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict, train=False):
         if not sample.is_cuda:
-            raise RuntimeError("sliders_b200.UNet2DConditionModel runs only on a CUDA (sm_100) device; "
+            raise RuntimeError("sliders_b200.UNet2DConditionModel runs only on a CUDA (sm_90) device; "
                                "there is no CPU path (the CPU oracle lives under oracle/ for tests)")
         B = sample.shape[0]
         dev = sample.device

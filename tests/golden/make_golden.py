@@ -27,6 +27,35 @@ OUT = os.path.dirname(os.path.abspath(__file__))
 WEIGHT_SEED, LORA_SEED = 11, 12
 
 
+MAX_FIXTURE_BYTES = 1_000_000
+
+
+def save_grad_subset(fx, path):
+    """torch.save(fx) with the per-adaptor gradient dicts ("grads", and "delta_sign" where present) cut to every
+    stride-th adaptor (sorted names, both lora_down and lora_up of a kept adaptor), the smallest stride that keeps the
+    file under MAX_FIXTURE_BYTES.  "grad_keys" keeps the full key list for the adaptor-set checks."""
+    import io
+
+    def adaptor(k):
+        return k.rsplit(".lora_", 1)[0]
+
+    keys = list(fx["grads"].keys())
+    names = sorted({adaptor(k) for k in keys})
+    for stride in range(1, len(names) + 1):
+        keep = {n for i, n in enumerate(names) if i % stride == 0}
+        out = dict(fx, grad_keys=keys)
+        for field in ("grads", "delta_sign"):
+            if field in fx:
+                out[field] = {k: v for k, v in fx[field].items() if adaptor(k) in keep}
+        buf = io.BytesIO()
+        torch.save(out, buf)
+        if buf.tell() < MAX_FIXTURE_BYTES:
+            break
+    with open(path, "wb") as f:
+        f.write(buf.getvalue())
+    return stride
+
+
 def build(cfg_name, lora, rank, alpha, method):
     cfg = getattr(ounet.UNetConfig, cfg_name)()
     torch.manual_seed(0)

@@ -42,7 +42,7 @@ def main():
     out = {"loss": loss.detach(), "target": target.detach(),
            "grads": {k: p.grad.to(torch.bfloat16) for k, p in net.named_parameters()}}
     assert all(torch.isfinite(g).all() and g.abs().sum() > 0 for g in out["grads"].values())
-    torch.save(out, os.path.join(HERE, "tiny_xl_grads.pt"))
+    mg.save_grad_subset(out, os.path.join(HERE, "tiny_xl_grads.pt"))
     print("tiny_xl_grads:", len(out["grads"]), "tensors, loss", float(loss))
 
     fx = torch.load(os.path.join(HERE, "tiny_sd.pt"))
@@ -59,7 +59,7 @@ def main():
     out = {"loss": loss.detach(), "pred": pred.detach(), "noise": noise,
            "grads": {k: p.grad.to(torch.bfloat16) for k, p in net.named_parameters()}}
     assert all(torch.isfinite(g).all() and g.abs().sum() > 0 for g in out["grads"].values())
-    torch.save(out, os.path.join(HERE, "tiny_sd_grads.pt"))
+    mg.save_grad_subset(out, os.path.join(HERE, "tiny_sd_grads.pt"))
     print("tiny_sd_grads:", len(out["grads"]), "tensors, loss", float(loss))
 
 

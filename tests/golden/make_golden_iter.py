@@ -210,7 +210,7 @@ def main():
         # regenerated from the seeds by the tests (make_golden.build)
         before, after = fx.pop("lora_before"), fx.pop("lora_after")
         fx["delta_sign"] = {k: torch.sign(after[k] - before[k]).to(torch.int8) for k in after if "alpha" not in k}
-        torch.save(fx, os.path.join(HERE, name + ".pt"))
+        mg.save_grad_subset(fx, os.path.join(HERE, name + ".pt"))
         gn = sum(float(g.float().pow(2).sum()) for g in fx["grads"].values()) ** 0.5
         print(name, "seed", fx["seed"], "timesteps_to", fx["timesteps_to"], "t", fx["current_timestep"],
               {k: float(fx[k]) for k in fx if k.startswith("loss")}, "grad norm", gn, "tensors", len(fx["grads"]))

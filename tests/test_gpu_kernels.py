@@ -1,8 +1,8 @@
-"""GPU parity tests of the individual sm_100a kernels, called through the C ABI (sliders_b200.ops) and compared
+"""GPU parity tests of the individual sm_90a kernels, called through the C ABI (sliders_b200.ops) and compared
 with fp32 torch math on the same bf16 inputs.  Tolerances: outputs are bf16 (relative rounding 2^-9 = 0.2 %), so
 rel-RMS <= 1e-2 catches any indexing / accumulation error while allowing output rounding; attention additionally
-rounds P to bf16 (standard flash attention), tolerance 2e-2.  Both GEMM kernels (single-CTA and the cta_group::2
-CTA-pair) are forced explicitly."""
+rounds P to bf16 (standard flash attention), tolerance 2e-2.  Both GEMM flavours (single CTA and the
+two-CTA cluster that multicasts the weight tile) are forced explicitly."""
 import math
 
 import pytest

@@ -1,7 +1,7 @@
 """CPU tests that pin the oracle (oracle/unet.py, oracle/ddim.py) — the reference has no tests of its own
 (SURVEY.md §4), so the restatement is pinned by known answers of the published architecture, by the golden
-vectors produced with the reference's own unmodified lora.py / train_util.py (tests/golden/make_golden.py) and,
-when /root/reference is present, by running those reference modules live."""
+vectors produced with the reference's own unmodified lora.py / train_util.py (tests/golden/make_golden.py) and by
+the answers those reference modules gave (tests/golden/make_golden_reference.py -> reference_answers.pt)."""
 import os
 
 import pytest
@@ -9,12 +9,14 @@ import torch
 
 from conftest import c3lier
 from oracle import ddim as oddim
-from oracle import reference_bridge as rb
 from oracle import unet as ounet
 from sliders_b200 import synthetic
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
-needs_ref = pytest.mark.skipif(not rb.available(), reason="/root/reference not present (GPU box)")
+
+
+def _reference_answers():
+    return torch.load(os.path.join(GOLDEN, "reference_answers.pt"))
 
 
 # ---------------------------------------------------------------------------------------- structure KATs
@@ -46,24 +48,29 @@ def test_hf_key_names():
     assert sd1.state_dict()["down_blocks.0.attentions.0.proj_in.weight"].shape == (320, 320, 1, 1)  # conv projection
 
 
-@needs_ref
 @pytest.mark.parametrize("name,n_leaves,n_params,rank", [("sdxl", 346, 4_320_000, 4), ("sdxl", 346, 8_640_000, 8),
                                                          ("sd15", 150, 2_906_880, 4)])
 def test_reference_lora_injection_counts(name, n_leaves, n_params, rank):
-    lora = rb.load("lora")
-    with torch.device("meta"):
-        m = ounet.UNet2DConditionModel(getattr(ounet.UNetConfig, name)())
-        with c3lier(lora):
-            net = lora.LoRANetwork(m, rank=rank, multiplier=1.0, alpha=1.0, train_method="noxattn")
-    assert len(net.unet_loras) == n_leaves
-    assert sum(p.numel() for p in net.parameters()) == n_params
-    names = {l.lora_name for l in net.unet_loras}
+    """The reference's LoRANetwork (noxattn + c3lier) on the oracle UNet injected these leaves (stored answers), and
+    the product's LoRANetwork on the product UNet injects the same leaves, in the same order."""
+    from sliders_b200 import lora as plora
+    from sliders_b200.unet import UNet2DConditionModel as PU, UNetConfig as PC
+
+    ref = _reference_answers()["injection"]
+    names = ref[name]
+    assert len(names) == n_leaves and ref[(name, rank)]["n_params"] == n_params
     for k in ("lora_unet_down_blocks_0_resnets_0_conv1", "lora_unet_down_blocks_0_resnets_0_time_emb_proj",
               "lora_unet_down_blocks_0_downsamplers_0_conv", "lora_unet_up_blocks_2_resnets_2_conv_shortcut",
               "lora_unet_mid_block_attentions_0_transformer_blocks_0_attn1_to_out_0"):
         if name == "sdxl":
             assert k in names, k
     assert not any("attn2" in n for n in names)
+    with torch.device("meta"):
+        m = PU(getattr(PC, name)())
+        with c3lier(plora):
+            net = plora.LoRANetwork(m, rank=rank, multiplier=1.0, alpha=1.0, train_method="noxattn")
+    assert [l.lora_name for l in net.unet_loras] == names
+    assert sum(p.numel() for p in net.parameters()) == n_params
 
 
 # ---------------------------------------------------------------------------------------- scheduler KATs
@@ -191,59 +198,62 @@ def test_golden_loss_formula():
     assert torch.allclose(want, fx["loss_enhance_g4"], rtol=1e-5)
 
 
-# ---------------------------------------------------------------------------------------- live reference
-@needs_ref
+# ---------------------------------------------------------------------------------------- reference answers
 def test_zero_init_identity_and_multiplier_semantics_with_reference_lora():
-    lora = rb.load("lora")
-    tu = rb.load("train_util")
-    mu = rb.load("model_util")
-    m = _tiny("tiny_xl")
+    """oracle/port.py's copy of the reference's LoRA hook on the tiny oracle UNet reproduces what the reference's own
+    lora.py + train_util.predict_noise_xl returned (stored answers): a fresh network is the identity (lora_up == 0,
+    lora.py:97-98), multiplier 0 outside `with network:`, the adaptor delta inside it, guidance 1 == the text half."""
+    from oracle import port
+
+    fx = _reference_answers()["hook_semantics"]
+    m = _tiny("tiny_xl", seed=fx["weight_seed"])
     m.requires_grad_(False)
-    g = torch.Generator().manual_seed(5)
-    lat = torch.randn(1, 4, 16, 16, generator=g)
-    ehs = torch.randn(2, 77, 256, generator=g)
-    pooled = torch.randn(2, 128, generator=g)
-    tids = torch.tensor([[128., 128, 0, 0, 128, 128]] * 2)
-    sched = mu.create_noise_scheduler("ddim")
+    x = fx["inputs"]
+    lat, ehs, pooled, tids, t = (x["latents"], x["text_embeddings"], x["add_text_embeddings"], x["add_time_ids"],
+                                 x["timestep"])
+    sched = _ddim()
     sched.set_timesteps(1000)
     with torch.no_grad():
-        base = tu.predict_noise_xl(m, sched, 500, lat, ehs, pooled, tids, guidance_scale=1)
-        with c3lier(lora):
-            net = lora.LoRANetwork(m, rank=4, multiplier=1.0, alpha=1.0, train_method="noxattn")
-        with net:  # fresh LoRA: lora_up == 0  ->  identity (lora.py:97-98)
-            fresh = tu.predict_noise_xl(m, sched, 500, lat, ehs, pooled, tids, guidance_scale=1)
-        assert torch.equal(fresh, base)
-        synthetic.init_lora_nonzero_(net, seed=1, up_std=0.05)
-        off = tu.predict_noise_xl(m, sched, 500, lat, ehs, pooled, tids, guidance_scale=1)  # multiplier 0 after exit
-        assert torch.allclose(off, base, atol=1e-6)
+        base = port.predict_noise_xl(m, sched, t, lat, ehs, pooled, tids, guidance_scale=1)
+        assert torch.allclose(base, fx["base"], rtol=1e-5, atol=1e-6)
+        net = port.LoRAHooks(m, rank=4, alpha=1.0, c3lier=True)
+        net.__exit__()
+        with net:  # fresh LoRA: lora_up == 0  ->  identity
+            fresh = port.predict_noise_xl(m, sched, t, lat, ehs, pooled, tids, guidance_scale=1)
+        assert torch.equal(fresh, base) and torch.equal(fx["fresh"], fx["base"])
+        synthetic.init_lora_nonzero_(net, seed=fx["lora_seed"], up_std=fx["lora_up_std"], reseed_down=True)
+        off = port.predict_noise_xl(m, sched, t, lat, ehs, pooled, tids, guidance_scale=1)  # multiplier 0 after exit
+        assert torch.allclose(off, base, atol=1e-6) and torch.allclose(fx["off"], fx["base"], atol=1e-6)
         with net:
-            on = tu.predict_noise_xl(m, sched, 500, lat, ehs, pooled, tids, guidance_scale=1)
-        assert (on - base).abs().max() > 1e-3
+            on = port.predict_noise_xl(m, sched, t, lat, ehs, pooled, tids, guidance_scale=1)
+        assert (fx["on"] - fx["base"]).abs().max() > 1e-3
+        assert torch.allclose(on, fx["on"], rtol=1e-5, atol=1e-6)
         # guidance_scale = 1  =>  guided == text half (train_util.py:250-253)
-        out = m(torch.cat([lat] * 2), 500, ehs, added_cond_kwargs={"text_embeds": pooled, "time_ids": tids}).sample
+        out = m(torch.cat([lat] * 2), t, ehs, added_cond_kwargs={"text_embeds": pooled, "time_ids": tids}).sample
         assert torch.allclose(base, out.chunk(2)[1], atol=1e-6)
 
 
-@needs_ref
 def test_reference_state_dict_keys_match_ours():
+    """Slider checkpoint compatibility: for every train_method the product's LoRANetwork has the state-dict keys, in
+    order, that the reference's LoRANetwork had on the oracle UNet (stored as SHA-256 of the joined key list)."""
+    import hashlib
+
     from sliders_b200 import lora as plora
     from sliders_b200.unet import UNet2DConditionModel as PU, UNetConfig as PC
 
-    lora = rb.load("lora")
-    for cfg_o, cfg_p in ((ounet.UNetConfig.sdxl(), PC.sdxl()), (ounet.UNetConfig.sd15(), PC.sd15())):
+    ref = _reference_answers()["state_dict_keys"]
+    for name, cfg_o, cfg_p in (("sdxl", ounet.UNetConfig.sdxl(), PC.sdxl()), ("sd15", ounet.UNetConfig.sd15(), PC.sd15())):
         with torch.device("meta"):
             mo, mp = ounet.UNet2DConditionModel(cfg_o), PU(cfg_p)
             assert list(mo.state_dict().keys()) == list(mp.state_dict().keys())
             assert [tuple(v.shape) for v in mo.state_dict().values()] == [tuple(v.shape) for v in mp.state_dict().values()]
             for method in ("noxattn", "full", "xattn", "selfattn", "innoxattn", "xattn-strict", "noxattn-hspace",
                            "noxattn-hspace-last"):
-                with c3lier(lora):
-                    a = lora.LoRANetwork(mo, rank=4, multiplier=1.0, alpha=1.0, train_method=method)
                 with c3lier(plora):
                     b = plora.LoRANetwork(mp, rank=4, multiplier=1.0, alpha=1.0, train_method=method)
-                assert list(a.state_dict().keys()) == list(b.state_dict().keys()), method
-                # re-create fresh models: injection swaps the leaf forwards
-                mo, mp = ounet.UNet2DConditionModel(cfg_o), PU(cfg_p)
+                keys = list(b.state_dict().keys())
+                assert (hashlib.sha256("\n".join(keys).encode()).hexdigest(), len(keys)) == ref[(name, method)], method
+                mp = PU(cfg_p)  # a fresh model: injection swaps the leaf forwards
 
 
 def test_euler_discrete_known_answers_and_ddim_equivalence():
@@ -360,7 +370,7 @@ def test_stochastic_sampler_identities():
 
 
 def test_port_reproduces_the_reference_loop_golden():
-    """oracle/port.py (the CPU port bench.py falls back to where /root/reference is absent) against the fixture the
+    """oracle/port.py (the CPU port bench.py times for its CPU baseline) against the fixture the
     reference's own loop source produced (tests/golden/iter_text_xl.pt): same adaptor set, same loss, same gradients."""
     import os
 
@@ -374,7 +384,8 @@ def test_port_reproduces_the_reference_loop_golden():
     om.requires_grad_(False).eval()
     net = port.LoRAHooks(om, rank=fx["rank"], alpha=fx["alpha"], c3lier=True)
     assert len(net.unet_loras) == fx["n_lora"]
-    assert {k for k, _ in net.named_parameters()} == set(fx["grads"])
+    assert {k for k, _ in net.named_parameters()} == set(fx["grad_keys"])
+    assert set(fx["grads"]) <= set(fx["grad_keys"])  # the fixture stores the gradients of a fixed subset of adaptors
     synthetic.init_lora_nonzero_(net, seed=fx["lora_seed"], up_std=fx["up_std"], reseed_down=True)
     net.__exit__()
     sched = oddim.DDIMScheduler(beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
@@ -389,6 +400,8 @@ def test_port_reproduces_the_reference_loop_golden():
     num = den = 0.0
     for k, p in net.named_parameters():
         # (the optimizer step ran after backward; .grad is untouched by it)
+        if k not in fx["grads"]:
+            continue
         num += (p.grad - fx["grads"][k].float()).pow(2).sum().item()
         den += fx["grads"][k].float().pow(2).sum().item()
     assert (num / den) ** 0.5 < 5e-3   # the fixture stores bf16-rounded gradients

@@ -1,4 +1,4 @@
-"""2-GPU check of the sharded text-slider step (BASELINE config 3), run under torchrun on a B200 x2 box:
+"""2-GPU check of the sharded text-slider step (BASELINE config 3), run under torchrun on two H100s:
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29512 \
         tools/gpu_check_sharded.py

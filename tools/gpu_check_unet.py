@@ -1,4 +1,4 @@
-"""End-to-end bring-up on a B200: product UNet (sliders_b200 kernels) vs the fp32 oracle on identical
+"""End-to-end bring-up on an H100: product UNet (sliders_b200 kernels) vs the fp32 oracle on identical
 weights / inputs, with and without LoRA, eager and CUDA-graph; then a first timing."""
 import os
 import sys

@@ -32,4 +32,4 @@ for fold in ([False, True, 1280] if os.environ.get("AB_LNFOLD") else [unet.fuse_
           torch.cuda.synchronize()
       ms = e0.elapsed_time(e1) / n
       print(f"B={B}: {ms:.2f} ms/forward -> {B / ms * 1e3:.1f} passes/s "
-            f"[SB200_PAIR={os.environ.get('SB200_PAIR', '1')} lnfold={fold}]", flush=True)
+            f"[SB200_PAIR={os.environ.get('SB200_PAIR', '0')} lnfold={fold}]", flush=True)

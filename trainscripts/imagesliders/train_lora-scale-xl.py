@@ -4,7 +4,7 @@
         --config_file 'trainscripts/imagesliders/data/config-xl.yaml' --folder_main 'datasets/eyesize/' \
         --folders 'bigsize, smallsize' --scales '1, -1'
 
-`folder_main/<folder>/` holds VAE-encoded latents (`<name>.pt`), see sliders_b200/cli.py.  Needs a B200."""
+`folder_main/<folder>/` holds VAE-encoded latents (`<name>.pt`), see sliders_b200/cli.py.  Needs an H100."""
 import os
 import sys
 

@@ -3,7 +3,7 @@
     python trainscripts/textsliders/train_lora.py --attributes 'male, female' --name 'ageslider' --rank 4 --alpha 1 \
         --config_file 'trainscripts/textsliders/data/config.yaml'
 
-The loop runs in sliders_b200 (sm_100a kernels; needs a B200).  See sliders_b200/cli.py for the offline flags."""
+The loop runs in sliders_b200 (sm_90a kernels; needs an H100).  See sliders_b200/cli.py for the offline flags."""
 import os
 import sys
 

@@ -4,7 +4,7 @@
         --alpha 1 --config_file 'trainscripts/textsliders/data/config-xl.yaml'
     torchrun --nproc-per-node 4 trainscripts/textsliders/train_lora_xl.py ...     # one conditioned prediction per GPU
 
-The loop runs in sliders_b200 (sm_100a kernels; needs a B200).  See sliders_b200/cli.py for the offline flags."""
+The loop runs in sliders_b200 (sm_90a kernels; needs an H100).  See sliders_b200/cli.py for the offline flags."""
 import os
 import sys
 
