@@ -145,6 +145,40 @@ int sb200_attention_bwd(void* handle, void* stream, const void* q, int ldq, cons
                         void* dq, int lddq, void* dk, int lddk, void* dv, int lddv, int B, int heads, int Sq,
                         int Skv, int head_dim, float scale);
 
+/* sb200_attention_bwd with caller scratch for a query-split dK / dV.  When the keys fit one resident tile (Skv <= 128)
+ * and heads * B leaves most of the 132 SMs of an H100 idle (cross-attention: 8 CTAs for SD1.x at batch 1), the dV and
+ * dK launches run SB200_ATTN_BWD_SPLITS query ranges per (head, batch) as separate CTAs that write fp32 partial tiles to
+ * ws, and a reduction sums them in split order (no atomics: bit-reproducible).  Other shapes take the unsplit path and
+ * leave ws untouched.  dQ is computed exactly as by sb200_attention_bwd.  The split count depends on the shape only.
+ * ws: SB200_ATTN_BWD_WS_FLOATS(B, heads, Sq, Skv, head_dim) floats. */
+#define SB200_ATTN_BWD_SPLITS_WANT(B, heads, Sq) \
+  ((132 + (B) * (heads) - 1) / ((B) * (heads)) < ((Sq) + 63) / 64 ? (132 + (B) * (heads) - 1) / ((B) * (heads)) : ((Sq) + 63) / 64)
+#define SB200_ATTN_BWD_SPLITS(B, heads, Sq, Skv) \
+  (((Skv) <= 128 && 2 * (B) * (heads) <= 132) ? SB200_ATTN_BWD_SPLITS_WANT(B, heads, Sq) : 1)
+#define SB200_ATTN_BWD_WS_FLOATS(B, heads, Sq, Skv, head_dim) \
+  ((size_t)2 * SB200_ATTN_BWD_SPLITS(B, heads, Sq, Skv) * (B) * (Skv) * (heads) * (head_dim))
+int sb200_attention_bwd_ws(void* handle, void* stream, const void* q, int ldq, const void* k, int ldk, const void* v,
+                           int ldv, const void* o, int ldo, const void* dout, int lddo, const float* lse, float* dsum,
+                           void* dq, int lddq, void* dk, int lddk, void* dv, int lddv, int B, int heads, int Sq,
+                           int Skv, int head_dim, float scale, float* ws, size_t ws_floats);
+
+/* out[M, N] (fp32, row stride ldo) = X[M, K] . W[N, K]^T as a split-K GEMM for few rows and a long K: the gradient
+ * w.r.t. encoder_hidden_states, d_ctx = dKV_all . W_kv, where K runs over the stacked to_k | to_v rows of every
+ * cross-attention block (77 * B rows, K up to 166 400 for SDXL).  Each CTA of the wgmma GEMM owns one 128 x bn tile
+ * and one range of SB200_GEMM_SPLITK_KB k-blocks (64 deep) and stores its fp32 accumulator tile to ws; a reduction
+ * sums the splits in order (no atomics: bit-reproducible).  The split depends on the shape only, sized for about one
+ * wave on 132 SMs.  N a multiple of 16, K and the leading dims multiples of 8.
+ * ws: SB200_GEMM_SPLITK_WS_FLOATS(M, N, K) floats. */
+#define SB200_GEMM_SPLITK_TILES(M, N) ((((M) + 127) / 128) * ((N) % 128 == 0 ? (N) / 128 : ((N) + 63) / 64))
+#define SB200_GEMM_SPLITK_KB_(M, N, K) \
+  ((((K) + 63) / 64 + (132 + SB200_GEMM_SPLITK_TILES(M, N) - 1) / SB200_GEMM_SPLITK_TILES(M, N) - 1) / \
+   ((132 + SB200_GEMM_SPLITK_TILES(M, N) - 1) / SB200_GEMM_SPLITK_TILES(M, N)))
+#define SB200_GEMM_SPLITK_KB(M, N, K) (SB200_GEMM_SPLITK_KB_(M, N, K) < 8 ? 8 : SB200_GEMM_SPLITK_KB_(M, N, K))
+#define SB200_GEMM_SPLITK_SPLITS(M, N, K) ((((K) + 63) / 64 + SB200_GEMM_SPLITK_KB(M, N, K) - 1) / SB200_GEMM_SPLITK_KB(M, N, K))
+#define SB200_GEMM_SPLITK_WS_FLOATS(M, N, K) ((size_t)SB200_GEMM_SPLITK_SPLITS(M, N, K) * (M) * (N))
+int sb200_gemm_splitk_f32(void* handle, void* stream, const void* x, int ldx, const void* w, int ldw, float* out,
+                          int ldo, int M, int N, int K, float* ws, size_t ws_floats);
+
 /* GroupNorm(+SiLU) backward w.r.t. the input (gamma / beta are frozen).  fwd_stats: the [B][groups][2] (mean, rstd)
  * block the forward left at stats_ws + SB200_GN_STATS_OFFSET(B, groups); ws: SB200_GN_WS_FLOATS scratch.
  * dx = dGN(dy) (+ add), written as the channel concat [B, HW, C0 + C1] with row stride lddx. */
@@ -206,6 +240,12 @@ int sb200_lora_conv_rank_update(void* handle, void* stream, void* dX, const floa
 int sb200_adamw(void* handle, void* stream, const void* table, int n_tensors, long long max_numel, double lr,
                 double beta1, double beta2, double eps, double weight_decay, int step);
 
+/* torch.optim.Adam step (L2 weight decay folded into the gradient, no amsgrad) on fp32 parameters with fp32
+ * moments: the optimiser of null-text inversion over the [1, 77, D] unconditional embedding.  table: device array of
+ * n_tensors records {p, g, m, v: fp32 device pointers; n: int64}. */
+int sb200_adam_f32(void* handle, void* stream, const void* table, int n_tensors, long long max_numel, double lr,
+                   double beta1, double beta2, double eps, double weight_decay, int step);
+
 /* GroupNorm (+ optional SiLU) over an NHWC tensor that may be the channel concat of two sources.
  * Replaces torch GroupNorm + SiLU in ResnetBlock2D / Transformer2DModel / conv_norm_out.
  * stats_ws: caller-owned fp32 scratch of at least SB200_GN_WS_FLOATS(B, groups) floats. The reduction is
@@ -255,6 +295,16 @@ int sb200_cfg_ddim(void* handle, void* stream, const void* eps2, int eps_is_f32,
  * carries): cx = 1, ce = sigma_next - sigma. */
 int sb200_cfg_step(void* handle, void* stream, const void* eps2, int eps_is_f32, float g, const void* x, float cx,
                    float ce, void* x_prev, void* eps_out, int out_is_f32, int64_t n);
+
+/* Loss of one null-text inversion inner step (fp32, n elements each):
+ *   eps = eps_u + g (eps_c - eps_u);  x_rec = cx x + ce eps  (a scheduler step affine in (x, eps));
+ *   loss = mean((x_rec - target)^2)
+ * mode 0 writes *loss (two-stage reduction over SB200_GUIDED_LOSS_BLOCKS(n) partial sums in ws, no atomics);
+ * mode 1 writes d_eps_u = dloss[0] (1 - g) ce 2 (x_rec - target) / n, dloss a device scalar (the incoming gradient). */
+#define SB200_GUIDED_LOSS_BLOCKS(n) ((n) / 2048 + 1 > 256 ? 256 : (n) / 2048 + 1)
+int sb200_guided_step_loss(void* handle, void* stream, const float* eps_u, const float* eps_c, float g, const float* x,
+                           float cx, float ce, const float* target, int64_t n, int mode, float* loss, float* ws,
+                           const float* dloss, float* d_eps_u);
 
 #ifdef __cplusplus
 }

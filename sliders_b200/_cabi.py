@@ -64,6 +64,11 @@ SIGNATURES = {
     "sb200_attention": [_p, _p, _p, _i, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _i, _f, _p],
     "sb200_attention_bwd": [_p, _p, _p, _i, _p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _p, _i, _p, _i, _p, _i,
                             _i, _i, _i, _i, _i, _f],
+    "sb200_attention_bwd_ws": [_p, _p, _p, _i, _p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _p, _i, _p, _i, _p, _i,
+                               _i, _i, _i, _i, _i, _f, _p, C.c_size_t],
+    "sb200_gemm_splitk_f32": [_p, _p, _p, _i, _p, _i, _p, _i, _i, _i, _i, _p, C.c_size_t],
+    "sb200_adam_f32": [_p, _p, _p, _i, C.c_longlong, _d, _d, _d, _d, _d, _i],
+    "sb200_guided_step_loss": [_p, _p, _p, _p, _f, _p, _f, _f, _p, _i64, _i, _p, _p, _p, _p],
     "sb200_groupnorm_bwd": [_p, _p, _p, _i, _i, _p, _i, _i, _p, _p, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _p, _p],
     "sb200_layernorm_bwd": [_p, _p, _p, _i, _p, _p, _i, _p, _i, _p, _i, _i, _i, _f],
     "sb200_geglu": [_p, _p, _p, _i, _p, _i, _i, _i],

@@ -8,8 +8,14 @@ The frozen weights need no gradient, so the pass is
   * per adapted leaf  y = W x + s up (down x):  d_up = s dY^T (x down^T),  d_down = s (dY up)^T x,  dX += s (dY up) down
     as rank-r reductions (csrc/backward.cu).
 `UNet2DConditionModel.forward` routes here (through `_UNetFunction`) whenever autograd is enabled and an active
-adaptor requires grad; otherwise the inference forward runs.  The training forward keeps the activations the backward
-needs (about 7 GB for an SDXL CFG pair at 1024 px) and applies GEGLU unfused so its pre-activation can be kept.
+adaptor requires grad or `encoder_hidden_states` requires grad; otherwise the inference forward runs.  The training
+forward keeps the activations the backward needs (about 7 GB for an SDXL CFG pair at 1024 px) and applies GEGLU unfused
+so its pre-activation can be kept.
+The gradient w.r.t. `encoder_hidden_states` (null-text inversion optimises the unconditional text embedding through the
+UNet) is the transpose of the batched cross-attention K / V projection of the forward (`unet._kv_plan`): every
+cross-attention block's dK | dV lands in its columns of one [B * 77, sum 2C] matrix, and one fp32 split-K GEMM against
+the stacked to_k | to_v weights gives d_ctx = dKV_all . W_kv.  Frozen active adaptors (a slider applied while the
+embedding is optimised) contribute to the input gradients; only trainable ones get weight gradients.
 The gradient w.r.t. the latents is not produced (the reference detaches them: train_lora_xl.py:207-229 runs the
 denoising under no_grad) — `sample.grad` stays None.
 """
@@ -63,16 +69,25 @@ def _w_dgrad(unet, conv) -> torch.Tensor:
 # LoRA leaf gradients
 # ----------------------------------------------------------------------------------------------------------------
 class _Grads:
-    """fp32 gradient buffers per adaptor parameter, keyed by id(parameter), plus the (adaptor, multiplier * alpha / r)
-    of every leaf as it was when the FORWARD ran: `loss.backward()` is called after `with network:` has reset the
-    multipliers to 0 (train_lora_xl.py:299-345, lora.py:256-258)."""
+    """fp32 gradient buffers per adaptor parameter, keyed by id(parameter), plus the (adaptor, multiplier * alpha / r,
+    trainable) of every active leaf as it was when the FORWARD ran: `loss.backward()` is called after `with network:`
+    has reset the multipliers to 0 (train_lora_xl.py:299-345, lora.py:256-258).  `dkv` / `kv_off`: the cross-attention
+    dK | dV matrix of the encoder_hidden_states gradient and each block's column offset in it (None without it)."""
 
     def __init__(self, scales: Dict[int, tuple]):
         self.by_param: Dict[int, torch.Tensor] = {}
         self.scales = scales
+        self.dkv: Optional[torch.Tensor] = None
+        self.kv_off: Dict[int, int] = {}
 
     def active(self, leaf):
-        return self.scales.get(id(leaf), (None, 0.0))
+        return self.scales.get(id(leaf), (None, 0.0, False))[:2]
+
+    def trainable(self, leaf) -> bool:
+        return self.scales.get(id(leaf), (None, 0.0, False))[2]
+
+    def any_trainable(self) -> bool:
+        return any(v[2] for v in self.scales.values())
 
     def buf(self, param: torch.Tensor, shape) -> Tuple[torch.Tensor, bool]:
         g = self.by_param.get(id(param))
@@ -87,8 +102,8 @@ def _snapshot_scales(unet) -> Dict[int, tuple]:
     out = {}
     for leaf, a in unet._adapted_leaves():
         s = float(a.multiplier) * float(a.scale)
-        if s != 0.0 and a.lora_down.weight.requires_grad:
-            out[id(leaf)] = (a, s)
+        if s != 0.0:
+            out[id(leaf)] = (a, s, bool(a.lora_down.weight.requires_grad))
     return out
 
 
@@ -96,11 +111,15 @@ def _lora_linear_bwd(unet, grads: _Grads, leaf, xs: List[torch.Tensor], dY: torc
                      dX: Optional[torch.Tensor]) -> None:
     """xs: the leaf's 2-D input as one or two column blocks ([x0 | x1]); dY [M, N]; dX [M, K] updated in place."""
     a, s = grads.active(leaf)
-    if a is None:
+    train = grads.trainable(leaf)
+    if a is None or (not train and dX is None):
         return
     down = a.lora_down.weight.detach().reshape(a.lora_down.weight.shape[0], -1).to(BF16)   # [r, K]
     up = a.lora_up.weight.detach().reshape(a.lora_up.weight.shape[0], -1).to(BF16)         # [N, r]
     r, K = down.shape
+    if not train:  # frozen adaptor: its share of the input gradient only
+        ops.lora_rank_update(dX, ops.lora_proj(dY, up.t().contiguous()), down, s)
+        return
     t = None
     k0 = 0
     for x in xs:
@@ -122,12 +141,16 @@ def _lora_conv_bwd(unet, grads: _Grads, conv, x: torch.Tensor, dY: torch.Tensor,
                    stride: int = 1) -> None:
     """x [B,H,W,Cin] NHWC input of the 3x3 leaf; dY [B,Ho,Wo,Cout]; dX [B,H,W,Cin] updated in place."""
     a, s = grads.active(conv)
-    if a is None:
+    train = grads.trainable(conv)
+    if a is None or (not train and dX is None):
         return
     D = a.lora_down.weight.detach().permute(0, 2, 3, 1).to(BF16).contiguous()             # [r, 3, 3, Cin]
     up = a.lora_up.weight.detach().reshape(a.lora_up.weight.shape[0], -1).to(BF16)        # [Cout, r]
     r = D.shape[0]
     dY2 = dY.reshape(-1, dY.shape[-1])
+    if not train:  # frozen adaptor: its share of the input gradient only
+        ops.lora_conv_rank_update(dX, ops.lora_proj(dY2, up.t().contiguous()), D, s, stride)
+        return
     t = ops.lora_conv_proj(x, D, stride)
     u = ops.lora_proj(dY2, up.t().contiguous())
     g_up, acc = grads.buf(a.lora_up.weight, (up.shape[0], r))
@@ -173,7 +196,7 @@ def _resnet_bwd(unet, grads, rec, d_out, need_dx=True):
     _lora_conv_bwd(unet, grads, blk.conv2, h3, d_out, d_h3)
     d_h2 = ops.groupnorm_bwd(h2, *unet._w_norm(n2), n2.num_groups, True, d_h3, ws2)
     # time_emb_proj: its output is broadcast over the pixels of conv1's output
-    if grads.active(blk.time_emb_proj)[0] is not None:
+    if grads.trainable(blk.time_emb_proj):
         d_temb = ops.colsum(d_h2).to(BF16)
         _lora_linear_bwd(unet, grads, blk.time_emb_proj, [emb_act], d_temb, None)
     # conv1
@@ -247,13 +270,18 @@ def _attn_bwd(unet, grads, attn, rec, x_norm, d_h, B, S):
             _lora_linear_bwd(unet, grads, leaf, [x_norm], dqkv[:, i * C_:(i + 1) * C_], d_n)
         return d_n
     dq = torch.empty((B * S, C_), device=d_h.device, dtype=BF16)
-    if any(grads.active(l)[0] is not None for l in (attn.to_k, attn.to_v)):
+    if any(grads.trainable(l) for l in (attn.to_k, attn.to_v)):
         # train methods `xattn` / `full`: the text-side projections are adapted; encoder_hidden_states needs no grad
         dkv = torch.empty((B * Skv, 2 * C_), device=d_h.device, dtype=BF16)
-        ops.attention_bwd(q, k, v, o, d_o, lse, B, attn.heads, S, Skv, scale, attn.dim_head, dq, dkv[:, :C_],
-                          dkv[:, C_:])
+        ops.attention_bwd_split(q, k, v, o, d_o, lse, B, attn.heads, S, Skv, scale, attn.dim_head, dq, dkv[:, :C_],
+                                dkv[:, C_:])
         _lora_linear_bwd(unet, grads, attn.to_k, [ctx], dkv[:, :C_], None)
         _lora_linear_bwd(unet, grads, attn.to_v, [ctx], dkv[:, C_:], None)
+    elif grads.dkv is not None:
+        # encoder_hidden_states needs a gradient: dK | dV into this block's columns of the batched K / V layout
+        off = grads.kv_off[id(attn)]
+        ops.attention_bwd_split(q, k, v, o, d_o, lse, B, attn.heads, S, Skv, scale, attn.dim_head, dq,
+                                grads.dkv[:, off:off + C_], grads.dkv[:, off + C_:off + 2 * C_])
     else:
         ops.attention_bwd(q, k, v, o, d_o, lse, B, attn.heads, S, Skv, scale, attn.dim_head, dq)
     d_n = ops.gemm(dq, _wt(unet, attn.to_q))
@@ -299,13 +327,13 @@ def _transformer_bwd(unet, grads, rec, d_out):
         ffp, ffo = blk.ff.net[0].proj, blk.ff.net[2]
         # feed-forward
         d_f = ops.gemm(d_h, _wt(unet, ffo))
-        if grads.active(ffo)[0] is not None:
-            _lora_linear_bwd(unet, grads, ffo, [ops.geglu(pre)], d_h, d_f)
+        if grads.active(ffo)[0] is not None:  # a frozen adaptor needs only dY: its input is not rebuilt
+            _lora_linear_bwd(unet, grads, ffo, [ops.geglu(pre)] if grads.trainable(ffo) else [], d_h, d_f)
         d_pre = ops.geglu_bwd(pre, d_f)
         d_n = ops.gemm(d_pre, _wt(unet, ffp))
         if grads.active(ffp)[0] is not None:
-            n3 = ops.layernorm(h3, *unet._w_norm(blk.norm3), eps=blk.norm3.eps)
-            _lora_linear_bwd(unet, grads, ffp, [n3], d_pre, d_n)
+            n3 = ops.layernorm(h3, *unet._w_norm(blk.norm3), eps=blk.norm3.eps) if grads.trainable(ffp) else None
+            _lora_linear_bwd(unet, grads, ffp, [n3] if n3 is not None else [], d_pre, d_n)
         d_h = ops.layernorm_bwd(h3, unet._w_norm(blk.norm3)[0], d_n, blk.norm3.eps, add=d_h)
         # cross-attention
         n2 = ops.layernorm(h2, *unet._w_norm(blk.norm2), eps=blk.norm2.eps)
@@ -329,7 +357,7 @@ def forward_train(unet, sample, timesteps_f32, ehs, added_cond_kwargs, out_dtype
     kv_all = unet._cross_kv(ctx)
     emb = unet._embeddings(timesteps_f32, B, added_cond_kwargs)
     h = ops.conv_in(sample, unet._w(unet.conv_in), unet._b(unet.conv_in))
-    tape = [("scales", _snapshot_scales(unet))]
+    tape = [("scales", _snapshot_scales(unet)), ("ctx", Sctx)]
     skips = [h]
     for blk in unet.down_blocks:
         attns = getattr(blk, "attentions", None)
@@ -395,13 +423,39 @@ def slice_tape(obj, lo: int, hi: int, B: int):
     return obj  # modules, ints, None, the scales snapshot
 
 
-def backward(unet, tape, d_eps: torch.Tensor) -> Dict[int, torch.Tensor]:
-    """Runs the tape in reverse; returns {id(parameter): fp32 gradient in the packed kernel layout}."""
+def _kv_plan_t(unet) -> Tuple[torch.Tensor, Dict[int, int]]:
+    """The stacked to_k | to_v weights of every cross-attention block, all channel widths in `_kv_plan` order, transposed
+    to [D_ctx, sum 2C] (packed once, like `_wt`), and each block's column offset in that order."""
+    ent = unet._packed.get("kvplan_t")
+    if ent is None:
+        plan = unet._kv_plan()
+        offs, base, ws = {}, 0, []
+        for C_, (w, o, _) in plan.items():
+            for aid, off in o.items():
+                offs[aid] = base + off
+            base += w.shape[0]
+            ws.append(w)
+        ent = (torch.cat(ws, 0).t().contiguous(), offs)
+        unet._packed["kvplan_t"] = ent
+    return ent
+
+
+def backward(unet, tape, d_eps: torch.Tensor, need_ehs: bool = False) -> Dict:
+    """Runs the tape in reverse; returns {id(parameter): fp32 gradient in the packed kernel layout}, plus under the key
+    "ehs" the fp32 [B * 77, D_ctx] gradient w.r.t. encoder_hidden_states when `need_ehs`."""
     assert tape[0][0] == "scales"
     grads = _Grads(tape[0][1])
     d_skips: List[torch.Tensor] = []
     d_h = None
     first_res = next(i for i, (kind, _) in enumerate(tape) if kind == "res")
+    stop_at = -1
+    if need_ehs:
+        first_tr = next(i for i, (kind, _) in enumerate(tape) if kind == "tr")
+        if not grads.any_trainable():
+            stop_at = first_tr  # nothing below the first transformer block needs a gradient
+        Sctx = next(rec for kind, rec in tape if kind == "ctx")  # tokens per sample of encoder_hidden_states
+        wt, grads.kv_off = _kv_plan_t(unet)
+        grads.dkv = torch.empty((d_eps.shape[0] * Sctx, wt.shape[1]), device=d_eps.device, dtype=BF16)
     for idx in range(len(tape) - 1, -1, -1):
         kind, rec = tape[idx]
         if kind == "out":
@@ -433,6 +487,10 @@ def backward(unet, tape, d_eps: torch.Tensor) -> Dict[int, torch.Tensor]:
             d_h = ops.add(d_h.reshape(-1, shp[-1]), ds.reshape(-1, shp[-1])).view(shp)
         if d_h is None and kind == "res":
             break  # first resnet: nothing upstream carries an adaptor
+        if idx == stop_at:
+            break
+    if need_ehs:
+        grads.by_param["ehs"] = ops.gemm_splitk_f32(grads.dkv, _kv_plan_t(unet)[0])
     return grads.by_param
 
 
@@ -453,8 +511,9 @@ class _TrainCapture:
     of all adaptor weights are static buffers.  The forward reads the slider factor from the device scalar the
     inference graphs use; the backward bakes it in, so the factor is part of the cache key."""
 
-    def __init__(self, unet, sample, t, ehs, added, out_dtype, params, keys):
+    def __init__(self, unet, sample, t, ehs, added, out_dtype, params, keys, need_ehs=False):
         self.x, self.t, self.ehs = sample.clone(), t.clone(), ehs.clone()
+        self.need_ehs = need_ehs
         self.added = None
         if added is not None:
             self.added = {"text_embeds": added["text_embeds"].to(device=sample.device, dtype=BF16).clone(),
@@ -467,7 +526,7 @@ class _TrainCapture:
         stream.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(stream):  # warm-up: weight / LoRA packing caches, transposed weights, TMA descriptors
             out, tape = forward_train(unet, self.x, self.t, self.ehs, self.added, out_dtype)
-            backward(unet, tape, torch.zeros_like(out))
+            backward(unet, tape, torch.zeros_like(out), need_ehs)
             del tape
         torch.cuda.current_stream().wait_stream(stream)
         torch.cuda.synchronize()
@@ -480,7 +539,7 @@ class _TrainCapture:
             unet._capturing = False
         self.d_out = torch.zeros_like(self.out)
         self.unet = unet
-        self.bwd = {}  # dead leading samples -> (graph, flat fp32 gradient of every adaptor weight)
+        self.bwd = {}  # dead leading samples -> (graph, flat fp32 gradient of every adaptor weight, d_ehs or None)
 
     def _capture_backward(self, dead: int):
         unet = self.unet
@@ -490,19 +549,19 @@ class _TrainCapture:
         stream = torch.cuda.Stream(device=self.x.device)
         stream.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(stream):
-            backward(unet, tape, d_live)  # warm-up of this variant
+            backward(unet, tape, d_live, self.need_ehs)  # warm-up of this variant
         torch.cuda.current_stream().wait_stream(stream)
         torch.cuda.synchronize()
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph, pool=self.gf.pool()):
-            by_param = backward(unet, tape, d_live)
+            by_param = backward(unet, tape, d_live, self.need_ehs)
             pieces = []
             for key, (shape, dtype) in zip(self.keys, self.meta):
                 g = by_param.get(key)
                 g = _param_grad(shape, dtype, g) if g is not None else torch.zeros(shape, device=self.x.device, dtype=dtype)
                 pieces.append(g.reshape(-1).to(torch.float32))
-            flat = torch.cat(pieces)
-        self.bwd[dead] = (graph, flat)
+            flat = torch.cat(pieces) if pieces else None
+        self.bwd[dead] = (graph, flat, by_param.get("ehs"))
 
     def run_forward(self, unet, x, t, ehs, added):
         self.x.copy_(x)
@@ -523,9 +582,12 @@ class _TrainCapture:
         self.d_out.copy_(d_out)
         if dead not in self.bwd:
             self._capture_backward(dead)
-        graph, flat_static = self.bwd[dead]
+        graph, flat_static, d_ehs = self.bwd[dead]
         graph.replay()
         self.pending = False
+        d_ehs = d_ehs.clone() if d_ehs is not None else None
+        if flat_static is None:
+            return [], d_ehs
         flat = flat_static.clone()
         grads, off = [], 0
         by_dtype = {}
@@ -538,28 +600,28 @@ class _TrainCapture:
                 src = by_dtype[dtype] = flat if dtype == torch.float32 else flat.to(dtype)
             grads.append(src[off:off + n].view(shape))
             off += n
-        return grads
+        return grads, d_ehs
 
 
-def _capture_for(unet, sample, t, ehs, added, out_dtype, params, keys):
+def _capture_for(unet, sample, t, ehs, added, out_dtype, params, keys, need_ehs=False):
     """Cached _TrainCapture for this call signature, or None when graphs are off / the signature cannot be captured
     (adaptors with different factors, or a second forward before the first one's backward)."""
     if not getattr(unet, "use_cuda_graph", False):
         return None
     sig, common = unet._lora_signature()
-    if common is None:
+    if common is None and any(sig[0]):
         return None
     addk = None
     if added is not None:
         addk = (tuple(added["text_embeds"].shape), tuple(added["time_ids"].shape))
-    key = ("train", tuple(sample.shape), sample.dtype, tuple(ehs.shape), addk, out_dtype, sig, round(common, 9),
-           tuple(keys))
+    key = ("train", tuple(sample.shape), sample.dtype, tuple(ehs.shape), addk, out_dtype, sig,
+           round(common, 9) if common is not None else None, tuple(keys), bool(need_ehs))
     cache = unet.__dict__.setdefault("_train_graphs", {})
     cap = cache.get(key)
     if cap is None:
         while len(cache) >= getattr(unet, "train_graph_max", 2):  # each capture pins its activations (19 GB at SDXL)
             cache.pop(next(iter(cache)))
-        cap = _TrainCapture(unet, sample, t, ehs, added, out_dtype, params, keys)
+        cap = _TrainCapture(unet, sample, t, ehs, added, out_dtype, params, keys, need_ehs)
         cache[key] = cap
     if cap.pending and cap.pending_token is not None and cap.pending_token() is None:
         # the autograd node of the forward that was never back-propagated is gone (exception, loss only logged, skipped
@@ -586,11 +648,13 @@ class _Token:
 
 class _UNetFunction(torch.autograd.Function):
     @staticmethod
-    def forward(fctx, unet, call, *params):
-        sample, t, ehs, added, out_dtype, keys = call
-        fctx.unet, fctx.keys = unet, keys
+    def forward(fctx, unet, call, ehs_in, *params):
+        sample, t, added, out_dtype, keys, need_ehs = call
+        ehs = ehs_in.detach().to(device=sample.device, dtype=BF16).contiguous()
+        fctx.unet, fctx.keys, fctx.need_ehs = unet, keys, need_ehs
+        fctx.ehs_meta = (tuple(ehs_in.shape), ehs_in.dtype, ehs_in.device)
         fctx.meta = [(tuple(p.shape), p.dtype) for p in params]
-        fctx.cap = _capture_for(unet, sample, t, ehs, added, out_dtype, params, keys)
+        fctx.cap = _capture_for(unet, sample, t, ehs, added, out_dtype, params, keys, need_ehs)
         if fctx.cap is not None:
             fctx.tape = True
             fctx.token = _Token()
@@ -606,21 +670,37 @@ class _UNetFunction(torch.autograd.Function):
         dead = int(getattr(fctx, "zero_rows", 0) or 0)  # leading samples whose incoming gradient is exactly zero
         if fctx.cap is not None:
             with torch.no_grad():
-                grads = fctx.cap.run_backward(d_out, dead)
+                grads, d_ctx = fctx.cap.run_backward(d_out, dead)
+                d_ehs = _ehs_grad(fctx, d_ctx, dead)
             fctx.tape = None
-            return (None, None, *grads)
+            return (None, None, d_ehs, *grads)
         with torch.no_grad():
             tape, d_live = fctx.tape, d_out.contiguous()
             if dead:
                 B = d_out.shape[0]
                 tape, d_live = slice_tape(tape, dead, B, B), d_live[dead:]
-            by_param = backward(fctx.unet, tape, d_live)
+            by_param = backward(fctx.unet, tape, d_live, fctx.need_ehs)
+            d_ehs = _ehs_grad(fctx, by_param.get("ehs"), dead)
         fctx.tape = None  # free the activations
-        out = [None, None]
+        out = [None, None, d_ehs]
         for key, (shape, dtype) in zip(fctx.keys, fctx.meta):
             g = by_param.get(key)
             out.append(_param_grad(shape, dtype, g) if g is not None else None)
         return tuple(out)
+
+
+def _ehs_grad(fctx, d_ctx: Optional[torch.Tensor], dead: int) -> Optional[torch.Tensor]:
+    """fp32 [B_live * 77, D] -> the gradient in encoder_hidden_states' own shape / dtype / device; the `dead` leading
+    samples (exactly-zero incoming gradient) get zeros."""
+    if not fctx.need_ehs:
+        return None
+    shape, dtype, device = fctx.ehs_meta
+    if dead:
+        full = torch.zeros(shape, device=d_ctx.device, dtype=torch.float32)
+        full[dead:].copy_(d_ctx.view((shape[0] - dead,) + shape[1:]))
+        d_ctx = full
+    return d_ctx.view(shape).to(device=device, dtype=dtype)
+
 
 
 def trainable_lora_params(unet) -> List[torch.Tensor]:
@@ -631,7 +711,11 @@ def trainable_lora_params(unet) -> List[torch.Tensor]:
     return ps
 
 
-def apply(unet, sample, t, ehs, added, out_dtype):
+def apply(unet, sample, t, ehs, added, out_dtype, need_ehs: bool = False):
+    """ehs: encoder_hidden_states as the caller passed it (any float dtype); with `need_ehs` it is an autograd input
+    and its gradient comes back in its own dtype, shape and device."""
     params = trainable_lora_params(unet)
     keys = [id(p) for p in params]  # the backward files gradients under id(adaptor parameter)
-    return _UNetFunction.apply(unet, (sample, t, ehs, added, out_dtype, keys), *params)
+    if not need_ehs:
+        ehs = ehs.detach()
+    return _UNetFunction.apply(unet, (sample, t, added, out_dtype, keys, need_ehs), ehs, *params)

@@ -17,6 +17,11 @@
 // The log-sum-exp comes from the forward kernel (attention.cu, `lse`), D from attn_bwd_prep_kernel.  Modes 1 / 2 read
 // lse / D per streamed column, mode 0 per resident row.  Head dim padded to ND x 64 columns by TMA zero fill as in
 // the forward.  Deterministic: no atomics (each output tile has one owner CTA).
+//
+// Query split (sb200_attention_bwd_ws): cross-attention has one 77-row resident tile per (head, batch), so modes 1 / 2
+// would run heads x B CTAs (8 for SD1.x at batch 1) that each stream every query.  With a scratch buffer, modes 1 / 2
+// instead run a (nsplit, heads, B) grid: CTA s streams queries [s q_split, (s + 1) q_split) and stores its fp32 partial
+// dV / dK tile to the scratch; attn_bwd_reduce_kernel sums the nsplit partials in split order into the bf16 outputs.
 #include "common.h"
 #include "ptx.cuh"
 
@@ -47,6 +52,9 @@ struct AttnBwdParams {
   int d;
   int mode;
   float scale_log2, scale;
+  float* ws;    // modes 1 / 2 query split: [nsplit][B * n_res][ld_ws] fp32 partials (NULL: one CTA per resident tile)
+  int q_split;  // streamed rows per split (a multiple of 64)
+  int ld_ws;    // heads * d
 };
 
 __device__ __forceinline__ float bwd_exp2(float x) {
@@ -77,7 +85,10 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attention_bwd_kernel(const __g
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int rt = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
+  const bool split = p.ws != nullptr;
+  const int rt = split ? 0 : blockIdx.x, head = blockIdx.y, b = blockIdx.z;
+  const int q0 = split ? blockIdx.x * p.q_split : 0;                       // first streamed row
+  const int n_str = split ? min(p.q_split, p.n_stream - q0) : p.n_stream;  // streamed rows of this CTA
   const int mode = p.mode;
   const bool need_dp = mode != 1;
 
@@ -106,7 +117,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attention_bwd_kernel(const __g
   }
   __syncthreads();
   pdl_wait();
-  const int n = (p.n_stream + kT - 1) / kT;
+  const int n = (n_str + kT - 1) / kT;
   const size_t stat_base = (static_cast<size_t>(b) * gridDim.y + head) * p.Sq;
 
   if (warp == 8) {
@@ -128,8 +139,8 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attention_bwd_kernel(const __g
         mbar_expect_tx(bar_full + 8 * s, 2 * kTBytes);
 #pragma unroll
         for (int i = 0; i < ND; ++i) {
-          tma_load_4d(sT1 + s * kTBytes + i * kTChunk, &p.tmT1, bar_full + 8 * s, i * 64, head, t * kT, b);
-          tma_load_4d(sT2 + s * kTBytes + i * kTChunk, &p.tmT2, bar_full + 8 * s, i * 64, head, t * kT, b);
+          tma_load_4d(sT1 + s * kTBytes + i * kTChunk, &p.tmT1, bar_full + 8 * s, i * 64, head, q0 + t * kT, b);
+          tma_load_4d(sT2 + s * kTBytes + i * kTChunk, &p.tmT2, bar_full + 8 * s, i * 64, head, q0 + t * kT, b);
         }
       }
       __syncwarp();
@@ -160,7 +171,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attention_bwd_kernel(const __g
   for (int t = 0; t < n; ++t) {
     const int s = t % kStages;
     const uint32_t ph = (t / kStages) & 1;
-    const int left = p.n_stream - t * kT;  // valid streamed rows in this tile
+    const int left = n_str - t * kT;  // valid streamed rows in this tile
     // per-column statistics of the streamed queries (modes 1 / 2): columns 8 e + 2 (lane % 4) + {0, 1}
     float lse_c[kT / 4], d_c[kT / 4];
     if (mode != 0) {
@@ -169,8 +180,8 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attention_bwd_kernel(const __g
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int col = 8 * e + 2 * (lane & 3) + h;
-          lse_c[2 * e + h] = col < left ? __ldg(p.lse + stat_base + t * kT + col) : INFINITY;
-          d_c[2 * e + h] = col < left ? __ldg(p.dsum + stat_base + t * kT + col) : 0.f;
+          lse_c[2 * e + h] = col < left ? __ldg(p.lse + stat_base + q0 + t * kT + col) : INFINITY;
+          d_c[2 * e + h] = col < left ? __ldg(p.dsum + stat_base + q0 + t * kT + col) : 0.f;
         }
     }
     float sc[kT / 2], dp[kT / 2];
@@ -231,6 +242,27 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attention_bwd_kernel(const __g
   }
 
   // ---- write the accumulator (first d columns of each padded head)
+  if (split) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int grow = row0 + 8 * r;
+      if (grow >= p.n_res) continue;
+      float* wp = p.ws + ((static_cast<size_t>(blockIdx.x) * gridDim.z + b) * p.n_res + grow) * p.ld_ws +
+                  static_cast<size_t>(head) * p.d;
+#pragma unroll
+      for (int c = 0; c < ND; ++c) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          const int col = c * 64 + 8 * e + 2 * (lane & 3);
+          if (col < p.d) {
+            const int i = 32 * c + 4 * e + 2 * r;
+            *reinterpret_cast<float2*>(wp + col) = make_float2(acc[i], acc[i + 1]);
+          }
+        }
+      }
+    }
+    return;
+  }
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int grow = row0 + 8 * r;
@@ -276,6 +308,31 @@ __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, int ld
   dsum[(static_cast<size_t>(bq) * heads + h) * Sq + qi] = acc;
 }
 
+// out[row, j] = sum over s (in order) of ws[s][row][j]; blockIdx.y: 0 = dV (first half of the scratch), 1 = dK.
+// Four columns per thread (cols is a multiple of 8).
+__global__ void attn_bwd_reduce_kernel(const float* __restrict__ ws, int nsplit, int rows, int cols,
+                                       __nv_bfloat16* __restrict__ dv, int lddv, __nv_bfloat16* __restrict__ dk,
+                                       int lddk) {
+  pdl_trigger();
+  pdl_wait();
+  const size_t part = static_cast<size_t>(rows) * cols;
+  const size_t idx = (static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x) * 4;
+  if (idx >= part) return;
+  const float* src = ws + static_cast<size_t>(blockIdx.y) * nsplit * part + idx;
+  float4 a = __ldg(reinterpret_cast<const float4*>(src));
+  for (int s = 1; s < nsplit; ++s) {
+    const float4 v = __ldg(reinterpret_cast<const float4*>(src + s * part));
+    a.x += v.x;
+    a.y += v.y;
+    a.z += v.z;
+    a.w += v.w;
+  }
+  const int row = static_cast<int>(idx / cols), col = static_cast<int>(idx % cols);
+  __nv_bfloat16* o =
+      blockIdx.y == 0 ? dv + static_cast<size_t>(row) * lddv + col : dk + static_cast<size_t>(row) * lddk + col;
+  *reinterpret_cast<uint2*>(o) = make_uint2(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w));
+}
+
 template <int ND>
 static int launch_attention_bwd(cudaStream_t stream, const AttnBwdParams& p, dim3 grid) {
   static bool attr_set = false;
@@ -308,14 +365,25 @@ static int make_map(Ctx* ctx, CUtensorMap* m, const void* ptr, int ld, int d, in
   return make_tmap_bf16(ctx, m, ptr, 4, dims, strides, box);
 }
 
+// Query splits of the dK / dV launches (include/sb200.h: SB200_ATTN_BWD_SPLITS bounds the result, which sizes the
+// scratch); *q_split receives the streamed rows per split.  1 = no split.
+static int attention_bwd_nsplit(int B, int heads, int Sq, int Skv, int* q_split) {
+  const int want = SB200_ATTN_BWD_SPLITS(B, heads, Sq, Skv);
+  if (want <= 1) return 1;
+  const int per = ((Sq + want - 1) / want + 63) / 64 * 64;
+  *q_split = per;
+  return (Sq + per - 1) / per;
+}
+
 }  // namespace sb200
 
 using namespace sb200;
 
-extern "C" int sb200_attention_bwd(void* handle, void* stream, const void* q, int ldq, const void* k, int ldk,
-                                   const void* v, int ldv, const void* o, int ldo, const void* dout, int lddo,
-                                   const float* lse, float* dsum, void* dq, int lddq, void* dk, int lddk, void* dv,
-                                   int lddv, int B, int heads, int Sq, int Skv, int head_dim, float scale) {
+static int attention_bwd_impl(void* handle, void* stream, const void* q, int ldq, const void* k, int ldk,
+                              const void* v, int ldv, const void* o, int ldo, const void* dout, int lddo,
+                              const float* lse, float* dsum, void* dq, int lddq, void* dk, int lddk, void* dv,
+                              int lddv, int B, int heads, int Sq, int Skv, int head_dim, float scale, float* ws,
+                              size_t ws_floats) {
   pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx, "attention_bwd: NULL handle");
@@ -363,6 +431,25 @@ extern "C" int sb200_attention_bwd(void* handle, void* stream, const void* q, in
   if ((st = make_map(ctx, &p.tmR2, v, ldv, head_dim, heads, Skv, B, 128))) return st;
   if ((st = make_map(ctx, &p.tmT1, q, ldq, head_dim, heads, Sq, B, trows))) return st;
   if ((st = make_map(ctx, &p.tmT2, dout, lddo, head_dim, heads, Sq, B, trows))) return st;
+  const int nsplit = ws ? attention_bwd_nsplit(B, heads, Sq, Skv, &p.q_split) : 1;
+  if (nsplit > 1) {
+    const size_t part = static_cast<size_t>(nsplit) * B * Skv * heads * head_dim;
+    SB200_REQUIRE(ws_floats >= 2 * part, "attention_bwd: scratch of %zu floats, %zu needed", ws_floats, 2 * part);
+    const dim3 gs(nsplit, heads, B);
+    p.ld_ws = heads * head_dim;
+    p.mode = 1;
+    p.ws = ws;
+    if ((st = launch_attention_bwd_d(s, p, gs))) return st;
+    p.mode = 2;
+    p.ws = ws + part;
+    if ((st = launch_attention_bwd_d(s, p, gs))) return st;
+    const size_t quads = static_cast<size_t>(B) * Skv * heads * head_dim / 4;
+    SB200_CUDA_CHECK(launch_pdl(attn_bwd_reduce_kernel, dim3(static_cast<unsigned>((quads + 255) / 256), 2), dim3(256),
+                                0, s, static_cast<const float*>(ws), nsplit, B * Skv, heads * head_dim,
+                                static_cast<__nv_bfloat16*>(dv), lddv, static_cast<__nv_bfloat16*>(dk), lddk));
+    SB200_CUDA_CHECK(cudaGetLastError());
+    return 0;
+  }
   const dim3 gk((Skv + 127) / 128, heads, B);
   p.mode = 1;
   p.out = static_cast<__nv_bfloat16*>(dv);
@@ -372,4 +459,22 @@ extern "C" int sb200_attention_bwd(void* handle, void* stream, const void* q, in
   p.out = static_cast<__nv_bfloat16*>(dk);
   p.ld = lddk;
   return launch_attention_bwd_d(s, p, gk);
+}
+
+extern "C" int sb200_attention_bwd(void* handle, void* stream, const void* q, int ldq, const void* k, int ldk,
+                                   const void* v, int ldv, const void* o, int ldo, const void* dout, int lddo,
+                                   const float* lse, float* dsum, void* dq, int lddq, void* dk, int lddk, void* dv,
+                                   int lddv, int B, int heads, int Sq, int Skv, int head_dim, float scale) {
+  return attention_bwd_impl(handle, stream, q, ldq, k, ldk, v, ldv, o, ldo, dout, lddo, lse, dsum, dq, lddq, dk, lddk,
+                            dv, lddv, B, heads, Sq, Skv, head_dim, scale, nullptr, 0);
+}
+
+extern "C" int sb200_attention_bwd_ws(void* handle, void* stream, const void* q, int ldq, const void* k, int ldk,
+                                      const void* v, int ldv, const void* o, int ldo, const void* dout, int lddo,
+                                      const float* lse, float* dsum, void* dq, int lddq, void* dk, int lddk, void* dv,
+                                      int lddv, int B, int heads, int Sq, int Skv, int head_dim, float scale, float* ws,
+                                      size_t ws_floats) {
+  SB200_REQUIRE(ws || ws_floats == 0, "attention_bwd_ws: NULL scratch");
+  return attention_bwd_impl(handle, stream, q, ldq, k, ldk, v, ldv, o, ldo, dout, lddo, lse, dsum, dq, lddq, dk, lddk,
+                            dv, lddv, B, heads, Sq, Skv, head_dim, scale, ws, ws_floats);
 }

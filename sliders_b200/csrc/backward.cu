@@ -818,6 +818,34 @@ __global__ void adamw_kernel(const AdamTensor* __restrict__ table, float decay, 
   }
 }
 
+// torch.optim.Adam (foreach / single-tensor, amsgrad off) on fp32 parameters and moments: the null-text embedding
+struct AdamTensorF32 {
+  float* p;
+  const float* g;
+  float* m;
+  float* v;
+  long long n;
+};
+
+__global__ void adam_f32_kernel(const AdamTensorF32* __restrict__ table, float weight_decay, float one_m_beta1,
+                                float beta2, float one_m_beta2, float eps, float neg_step_size, float bc2_sqrt) {
+  pdl_trigger();
+  pdl_wait();
+  const AdamTensorF32 t = table[blockIdx.y];
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < t.n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float p = t.p[i];
+    const float g = t.g[i] + weight_decay * p;          // grad.add(param, alpha=weight_decay)
+    const float m = t.m[i] + one_m_beta1 * (g - t.m[i]);  // exp_avg.lerp_(grad, 1 - beta1)
+    const float v = t.v[i] * beta2 + one_m_beta2 * g * g; // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2)
+    const float denom = sqrtf(v) / bc2_sqrt + eps;       // (exp_avg_sq.sqrt() / bias_correction2_sqrt).add_(eps)
+    p += neg_step_size * (m / denom);                    // param.addcdiv_(exp_avg, denom, value=-step_size)
+    t.p[i] = p;
+    t.m[i] = m;
+    t.v[i] = v;
+  }
+}
+
 static inline int grid_for(size_t work, int threads, int sms) {
   size_t b = (work + threads - 1) / threads;
   const size_t cap = static_cast<size_t>(sms) * 16;
@@ -1127,5 +1155,21 @@ extern "C" int sb200_adamw(void* handle, void* stream, const void* table, int n_
       static_cast<const AdamTensor*>(table), static_cast<float>(1.0 - lr * weight_decay),
       static_cast<float>(1.0 - beta1), static_cast<float>(beta2), static_cast<float>(1.0 - beta2),
       static_cast<float>(eps), static_cast<float>(-(lr / bc1)), static_cast<float>(sqrt(bc2))));
+  return 0;
+}
+
+extern "C" int sb200_adam_f32(void* handle, void* stream, const void* table, int n_tensors, long long max_numel,
+                              double lr, double beta1, double beta2, double eps, double weight_decay, int step) {
+  pdl_hint() = true;
+  Ctx* ctx = as_ctx(handle);
+  SB200_REQUIRE(ctx && table && n_tensors > 0 && max_numel > 0 && step >= 1, "adam_f32: arguments");
+  const double bc1 = 1.0 - pow(beta1, step), bc2 = 1.0 - pow(beta2, step);
+  const int bx = grid_for(static_cast<size_t>(max_numel), 256, ctx->num_sms);
+  SB200_CUDA_CHECK(launch_pdl(adam_f32_kernel, dim3(bx, n_tensors), dim3(256), 0, static_cast<cudaStream_t>(stream),
+                              static_cast<const AdamTensorF32*>(table), static_cast<float>(weight_decay),
+                              static_cast<float>(1.0 - beta1), static_cast<float>(beta2),
+                              static_cast<float>(1.0 - beta2), static_cast<float>(eps), static_cast<float>(-lr / bc1),
+                              static_cast<float>(sqrt(bc2))));
+  SB200_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

@@ -290,9 +290,86 @@ __global__ void cfg_ddim_kernel(const TE* __restrict__ eps2, float g, const TO* 
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// null-text inversion inner-step loss: x_rec = cx x + ce (eps_u + g (eps_c - eps_u)), loss = mean((x_rec - target)^2)
+constexpr int kLossThreads = 256;
+
+__device__ __forceinline__ float guided_residual(const float* eps_u, const float* eps_c, float g, const float* x,
+                                                 float cx, float ce, const float* target, int64_t i) {
+  const float eu = eps_u[i];
+  const float e = eu + g * (eps_c[i] - eu);
+  return cx * x[i] + ce * e - target[i];
+}
+
+// mode 0: block b sums the squared residuals of its grid-stride share into ws[b] (fixed order: strided per thread,
+// then a shared-memory tree); mode 1: d_eps_u = dloss (1 - g) ce 2 r / n
+__global__ void __launch_bounds__(kLossThreads) guided_loss_kernel(const float* __restrict__ eps_u,
+                                                                    const float* __restrict__ eps_c, float g,
+                                                                    const float* __restrict__ x, float cx, float ce,
+                                                                    const float* __restrict__ target, int64_t n,
+                                                                    int mode, float* __restrict__ ws,
+                                                                    const float* __restrict__ dloss,
+                                                                    float* __restrict__ d_eps_u) {
+  pdl_trigger();
+  pdl_wait();
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  if (mode == 1) {
+    const float k = __ldg(dloss) * (1.f - g) * ce * 2.f / static_cast<float>(n);
+    for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n; i += stride)
+      d_eps_u[i] = k * guided_residual(eps_u, eps_c, g, x, cx, ce, target, i);
+    return;
+  }
+  float acc = 0.f;
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n; i += stride) {
+    const float r = guided_residual(eps_u, eps_c, g, x, cx, ce, target, i);
+    acc = fmaf(r, r, acc);
+  }
+  __shared__ float red[kLossThreads];
+  red[threadIdx.x] = acc;
+  __syncthreads();
+  for (int w = kLossThreads / 2; w > 0; w >>= 1) {
+    if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) ws[blockIdx.x] = red[0];
+}
+
+__global__ void __launch_bounds__(kLossThreads) guided_loss_finalize_kernel(const float* __restrict__ ws, int parts,
+                                                                             int64_t n, float* __restrict__ loss) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ float red[kLossThreads];
+  red[threadIdx.x] = threadIdx.x < parts ? ws[threadIdx.x] : 0.f;
+  __syncthreads();
+  for (int w = kLossThreads / 2; w > 0; w >>= 1) {
+    if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *loss = red[0] / static_cast<float>(n);
+}
+
 }  // namespace sb200
 
 using namespace sb200;
+
+extern "C" int sb200_guided_step_loss(void* handle, void* stream, const float* eps_u, const float* eps_c, float g,
+                                      const float* x, float cx, float ce, const float* target, int64_t n, int mode,
+                                      float* loss, float* ws, const float* dloss, float* d_eps_u) {
+  pdl_hint() = true;
+  SB200_REQUIRE(handle && eps_u && eps_c && x && target && n > 0, "guided_step_loss: NULL argument");
+  SB200_REQUIRE(mode == 0 ? (loss && ws) : (mode == 1 && dloss && d_eps_u), "guided_step_loss: mode %d outputs", mode);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int parts = SB200_GUIDED_LOSS_BLOCKS(n);
+  const int blocks = mode == 0 ? parts : static_cast<int>((n + kLossThreads - 1) / kLossThreads < 1024
+                                                               ? (n + kLossThreads - 1) / kLossThreads : 1024);
+  SB200_CUDA_CHECK(launch_pdl(guided_loss_kernel, dim3(blocks), dim3(kLossThreads), 0, s, eps_u, eps_c, g, x, cx, ce,
+                              target, n, mode, ws, dloss, d_eps_u));
+  if (mode == 0)
+    SB200_CUDA_CHECK(launch_pdl(guided_loss_finalize_kernel, dim3(1), dim3(kLossThreads), 0, s,
+                                static_cast<const float*>(ws), parts, n, loss));
+  SB200_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
 
 extern "C" int sb200_sinusoid(void* handle, void* stream, const float* values, int n, int dim, void* out,
                               int ldo) {

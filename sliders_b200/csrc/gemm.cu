@@ -99,6 +99,10 @@ struct GemmParams {
   const float* ln_dl;
   float* rs_out;
   int rs_parts;
+  // split-K (sb200_gemm_splitk_f32): grid y = split index; split s runs k-blocks [s * sk_kb, (s + 1) * sk_kb) and stores
+  // its raw fp32 tile to sk_ws[s][M][N] instead of running the epilogue
+  float* sk_ws;
+  int sk_kb, sk_splits;
 };
 
 __device__ __forceinline__ void add_bf16x16(float* f, const __nv_bfloat16* src) {
@@ -215,7 +219,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_kernel(const __grid_cons
   const int mt = p.n_fast ? t / num_n_tiles : t % num_m_tiles;
   const int nt = p.n_fast ? t % num_n_tiles : t / num_m_tiles;
   const int st = mt * kCtas + static_cast<int>(cta_rank);  // this CTA's 128-row sub-tile
-  const int kblocks = p.kblocks;
+  const int kb_lo = p.sk_ws ? static_cast<int>(blockIdx.y) * p.sk_kb : 0;
+  const int kb_hi = p.sk_ws ? min(p.kblocks, kb_lo + p.sk_kb) : p.kblocks;
   const uint32_t stage_bytes = static_cast<uint32_t>(p.stage_bytes);
   const uint32_t a_bytes = kBM * 128;
   const uint32_t b_bytes = static_cast<uint32_t>(BN) * 128;  // W rows of a stage (both halves for a pair)
@@ -242,7 +247,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_kernel(const __grid_cons
     }
     int stage = 0;
     uint32_t phase = 0;
-    for (int kb = 0; kb < kblocks; ++kb) {
+    for (int kb = kb_lo; kb < kb_hi; ++kb) {
       const uint32_t full_bar = bar_full + 8u * stage, empty_bar = bar_empty + 8u * stage;
       mbar_wait(empty_bar, phase ^ 1u);
       if (elect_one()) {
@@ -299,7 +304,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_kernel(const __grid_cons
     const uint32_t peer_empty = kCtas == 2 ? mapa_u32(bar_empty, cta_rank ^ 1u) : 0u;
     int stage = 0, prev = 0;
     uint32_t phase = 0;
-    for (int kb = 0; kb < kblocks; ++kb) {
+    for (int kb = kb_lo; kb < kb_hi; ++kb) {
       mbar_wait(bar_full + 8u * stage, phase);
       const uint32_t sA = tiles + static_cast<uint32_t>(stage) * stage_bytes + static_cast<uint32_t>(wg) * 64u * 128u;
       const uint32_t sB = tiles + static_cast<uint32_t>(stage) * stage_bytes + a_bytes;
@@ -315,7 +320,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_kernel(const __grid_cons
       }
       wgmma_commit();
       wgmma_wait<1>();  // the previous k-block's products have read their stage: hand it back to the producer(s)
-      if (kb > 0 && signal) {
+      if (kb > kb_lo && signal) {
         mbar_arrive(bar_empty + 8u * prev);
         if (kCtas == 2) mbar_arrive_cluster(peer_empty + 8u * prev);
       }
@@ -341,6 +346,19 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_kernel(const __grid_cons
     else if constexpr (rt == 32)
       store_frag<32>(accl, accs, wg * 64, BN, kStride);
     asm volatile("bar.sync %0, %1;" ::"n"(kConsumerBar), "n"(32 * kEpiWarps) : "memory");
+    if (p.sk_ws != nullptr) {
+      // split-K: this split's raw fp32 tile, row-coalesced; sb200_gemm_splitk_f32's reduction sums the splits
+      float* dst = p.sk_ws + static_cast<size_t>(blockIdx.y) * p.M * p.N;
+      constexpr int kQuads = BN / 4;
+      for (int idx = threadIdx.x; idx < kBM * kQuads; idx += 32 * kEpiWarps) {
+        const int row = idx / kQuads, c = (idx - row * kQuads) * 4;
+        const int m = st * kBM + row, n = nt * BN + c;
+        if (m < p.M && n < p.N)
+          *reinterpret_cast<uint4*>(dst + static_cast<size_t>(m) * p.N + n) =
+              ld_shared_v4(accs + static_cast<uint32_t>(row * kStride + c) * 4u);
+      }
+      return;
+    }
 
     const int q = warp & 3;      // 32-row quarter of the tile this warp writes
     const int hsel = warp >> 2;  // which of the kEpiPerQuarter warps of this quarter (slab index mod that)
@@ -632,7 +650,7 @@ static int launch_gemm_bn(Ctx* ctx, cudaStream_t stream, const GemmParams& p, in
   }
   const int total = p.num_m_tiles * p.num_n_tiles;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(total * kCtas);
+  cfg.gridDim = dim3(total * kCtas, p.sk_ws ? p.sk_splits : 1);
   cfg.blockDim = dim3(kGemmThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
@@ -673,7 +691,7 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
   if (p.ring_bytes < acc_tile_bytes(p.bn)) p.ring_bytes = acc_tile_bytes(p.bn);
   const int smem = kBarRegion + 1024 + p.ring_bytes + epi_bytes;
   if (smem > kSmemBudget) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
-  pdl_hint() = p.num_m_tiles * p.num_n_tiles * ctas <= 2 * ctx->num_sms;
+  pdl_hint() = p.num_m_tiles * p.num_n_tiles * ctas * (p.sk_ws ? p.sk_splits : 1) <= 2 * ctx->num_sms;
   const int rt = has_lora ? p.lora_rt : 0;
   const int variant = (ctas == 2 ? 6 : 0) + (p.bn == 128 ? 3 : 0) + (rt == 16 ? 1 : (rt == 32 ? 2 : 0));
   cudaStream_t s = stream;
@@ -723,9 +741,78 @@ static void fill_lora(GemmParams& p, const sb200_lora* lora) {
   p.lora_scale_dev = lora->scale_dev;
 }
 
+// out[m, n] = sum over s (in order) of ws[s][m][n]; four columns per thread
+__global__ void splitk_reduce_kernel(const float* __restrict__ ws, int splits, int M, int N, float* __restrict__ out,
+                                     int ldo) {
+  pdl_trigger();
+  pdl_wait();
+  const size_t part = static_cast<size_t>(M) * N;
+  const size_t idx = (static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x) * 4;
+  if (idx >= part) return;
+  float4 a = __ldg(reinterpret_cast<const float4*>(ws + idx));
+  for (int s = 1; s < splits; ++s) {
+    const float4 v = __ldg(reinterpret_cast<const float4*>(ws + s * part + idx));
+    a.x += v.x;
+    a.y += v.y;
+    a.z += v.z;
+    a.w += v.w;
+  }
+  const size_t m = idx / N, n = idx % N;
+  *reinterpret_cast<float4*>(out + m * ldo + n) = a;
+}
+
 }  // namespace sb200
 
 using namespace sb200;
+
+extern "C" int sb200_gemm_splitk_f32(void* handle, void* stream, const void* x, int ldx, const void* w, int ldw,
+                                     float* out, int ldo, int M, int N, int K, float* ws, size_t ws_floats) {
+  Ctx* ctx = as_ctx(handle);
+  SB200_REQUIRE(ctx && x && w && out && ws, "gemm_splitk_f32: NULL argument");
+  SB200_REQUIRE(M > 0 && N > 0 && K > 0 && N % 16 == 0, "gemm_splitk_f32: bad dims M=%d N=%d K=%d", M, N, K);
+  SB200_REQUIRE(K % 8 == 0 && ldx % 8 == 0 && ldw % 8 == 0 && ldo % 4 == 0,
+                "gemm_splitk_f32: K and the bf16 leading dims must be multiples of 8, ldo of 4");
+  const size_t need = SB200_GEMM_SPLITK_WS_FLOATS(M, N, K);
+  SB200_REQUIRE(ws_floats >= need, "gemm_splitk_f32: scratch of %zu floats, %zu needed", ws_floats, need);
+  GemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.M = M;
+  p.N = N;
+  p.K = K;
+  p.Nout = N;
+  p.kblocks = (K + kBK - 1) / kBK;
+  p.kb_split = p.kblocks;
+  p.cb_total = p.kblocks;
+  p.a_tx = kBM * 128;
+  p.num_sub = (M + kBM - 1) / kBM;
+  p.bn = N % 128 == 0 ? 128 : 64;
+  p.ncols_out = p.bn;
+  p.num_m_tiles = p.num_sub;
+  p.num_n_tiles = (N + p.bn - 1) / p.bn;
+  p.sk_ws = ws;
+  p.sk_kb = SB200_GEMM_SPLITK_KB(M, N, K);
+  p.sk_splits = SB200_GEMM_SPLITK_SPLITS(M, N, K);
+  int st;
+  {
+    const uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(M)};
+    const uint64_t strides[1] = {static_cast<uint64_t>(ldx) * 2};
+    const uint32_t box[2] = {kBK, kBM};
+    if ((st = make_tmap_bf16(ctx, &p.tmA[0], x, 2, dims, strides, box))) return st;
+  }
+  {
+    const uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(N)};
+    const uint64_t strides[1] = {static_cast<uint64_t>(ldw) * 2};
+    const uint32_t box[2] = {kBK, static_cast<uint32_t>(p.bn)};
+    if ((st = make_tmap_bf16(ctx, &p.tmB, w, 2, dims, strides, box))) return st;
+  }
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if ((st = launch_gemm(ctx, s, p, 1))) return st;
+  const size_t quads = static_cast<size_t>(M) * N / 4;
+  SB200_CUDA_CHECK(launch_pdl(splitk_reduce_kernel, dim3(static_cast<unsigned>((quads + 255) / 256)), dim3(256), 0, s,
+                              static_cast<const float*>(ws), p.sk_splits, M, N, out, ldo));
+  SB200_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
 
 extern "C" int sb200_gemm(void* handle, void* stream, const void* x0, int ldx0, const void* x1, int ldx1,
                           int K0, const void* w, int ldw, void* out, int ldo, int M, int N, int K,

@@ -353,6 +353,109 @@ def attention_bwd(q, k, v, o, dout, lse, B: int, heads: int, Sq: int, Skv: int, 
     _count("attention_bwd", (6.0 if dk is None else 14.0) * B * heads * Sq * Skv * head_dim)
 
 
+def attn_bwd_splits(B: int, heads: int, Sq: int, Skv: int) -> int:
+    """SB200_ATTN_BWD_SPLITS: the query-split count bound of `attention_bwd_split` (1 = the unsplit launches)."""
+    if Skv > 128 or 2 * B * heads > 132:
+        return 1
+    return min((132 + B * heads - 1) // (B * heads), (Sq + 63) // 64)
+
+
+def attention_bwd_split(q, k, v, o, dout, lse, B: int, heads: int, Sq: int, Skv: int, scale: float, head_dim: int,
+                        dq: torch.Tensor, dk: torch.Tensor, dv: torch.Tensor) -> None:
+    """`attention_bwd` with dK / dV through `sb200_attention_bwd_ws`: for a short key sequence on few (head, batch)
+    pairs (cross-attention) the dV and dK launches split the queries over SB200_ATTN_BWD_SPLITS CTAs per pair, and
+    `attn_bwd_reduce_kernel` sums their fp32 partials in order.  Other shapes run exactly as `attention_bwd`."""
+    dsum = torch.empty(B * heads * Sq, device=q.device, dtype=torch.float32)
+    nsplit = attn_bwd_splits(B, heads, Sq, Skv)
+    ws_n = 2 * nsplit * B * Skv * heads * head_dim if nsplit > 1 else 0
+    ws = torch.empty(max(ws_n, 1), device=q.device, dtype=torch.float32)
+    lib = _begin()
+    _cabi.check(lib.sb200_attention_bwd_ws(
+        _ctx(q), _stream(), _p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(o), o.stride(0),
+        _p(dout), dout.stride(0), _p(lse), _p(dsum), _p(dq), dq.stride(0), _p(dk), dk.stride(0), _p(dv), dv.stride(0),
+        B, heads, Sq, Skv, int(head_dim), float(scale), _p(ws), ws_n))
+    global launch_count
+    launch_count += 2 if nsplit == 1 else 3
+    _count("attention_bwd", 14.0 * B * heads * Sq * Skv * head_dim)
+
+
+def splitk_ws_floats(M: int, N: int, K: int) -> int:
+    """SB200_GEMM_SPLITK_WS_FLOATS."""
+    tiles = ((M + 127) // 128) * (N // 128 if N % 128 == 0 else (N + 63) // 64)
+    want = (132 + tiles - 1) // tiles
+    kbs = (K + 63) // 64
+    kb = max(8, (kbs + want - 1) // want)
+    return ((kbs + kb - 1) // kb) * M * N
+
+
+def gemm_splitk_f32(x: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp32 out[M, N] = x[M, K] @ w[N, K].T (bf16 operands): `gemm_kernel` in split-K mode + `splitk_reduce_kernel`."""
+    M, K = x.shape
+    N = w.shape[0]
+    assert w.shape[1] == K
+    if out is None:
+        out = torch.empty((M, N), device=x.device, dtype=torch.float32)
+    n_ws = splitk_ws_floats(M, N, K)
+    ws = torch.empty(n_ws, device=x.device, dtype=torch.float32)
+    lib = _begin()
+    _cabi.check(lib.sb200_gemm_splitk_f32(_ctx(x), _stream(), _p(x), x.stride(0), _p(w), w.stride(0), _p(out),
+                                          out.stride(0), M, N, K, _p(ws), n_ws))
+    global launch_count
+    launch_count += 1
+    _count("gemm", 2.0 * M * N * K)
+    return out
+
+
+def guided_step_loss_fwd(eps_u, eps_c, g: float, x, cx: float, ce: float, target) -> torch.Tensor:
+    """fp32 scalar mean((cx x + ce (eps_u + g (eps_c - eps_u)) - target)^2): `guided_loss_kernel` + finalize."""
+    n = eps_u.numel()
+    parts = min(256, n // 2048 + 1)  # SB200_GUIDED_LOSS_BLOCKS
+    ws = torch.empty(parts, device=eps_u.device, dtype=torch.float32)
+    loss = torch.empty((), device=eps_u.device, dtype=torch.float32)
+    lib = _begin()
+    _cabi.check(lib.sb200_guided_step_loss(_ctx(eps_u), _stream(), _p(eps_u), _p(eps_c), float(g), _p(x), float(cx),
+                                           float(ce), _p(target), n, 0, _p(loss), _p(ws), None, None))
+    global launch_count
+    launch_count += 1
+    _count()
+    return loss
+
+
+def guided_step_loss_bwd(eps_u, eps_c, g: float, x, cx: float, ce: float, target, dloss) -> torch.Tensor:
+    """d loss / d eps_u scaled by the device scalar dloss: one `guided_loss_kernel` launch."""
+    d = torch.empty_like(eps_u)
+    lib = _begin()
+    _cabi.check(lib.sb200_guided_step_loss(_ctx(eps_u), _stream(), _p(eps_u), _p(eps_c), float(g), _p(x), float(cx),
+                                           float(ce), _p(target), eps_u.numel(), 1, None, None, _p(dloss), _p(d)))
+    _count()
+    return d
+
+
+class GuidedStepLoss(torch.autograd.Function):
+    """loss = mse(cx x + ce (eps_u + g (eps_c - eps_u)), target) with a gradient for eps_u only (the null-text inner
+    step: eps_c, x and target are constants).  All tensors fp32 CUDA, contiguous, of one shape."""
+
+    @staticmethod
+    def forward(fctx, eps_u, eps_c, g, x, cx, ce, target):
+        for t in (eps_u, eps_c, x, target):
+            if t.dtype != torch.float32 or not t.is_contiguous() or t.shape != eps_u.shape:
+                raise ValueError("guided_step_loss: eps_u, eps_c, x and target must be contiguous fp32 of one shape")
+        fctx.save_for_backward(eps_u, eps_c, x, target)
+        fctx.coef = (float(g), float(cx), float(ce))
+        return guided_step_loss_fwd(eps_u, eps_c, g, x, cx, ce, target)
+
+    @staticmethod
+    def backward(fctx, dloss):
+        eps_u, eps_c, x, target = fctx.saved_tensors
+        g, cx, ce = fctx.coef
+        d = guided_step_loss_bwd(eps_u, eps_c, g, x, cx, ce, target, dloss.to(torch.float32).contiguous())
+        return d, None, None, None, None, None, None
+
+
+def guided_step_loss(eps_u, eps_c, g: float, x, cx: float, ce: float, target) -> torch.Tensor:
+    return GuidedStepLoss.apply(eps_u, eps_c, g, x, cx, ce, target)
+
+
 def groupnorm_bwd(x0, gamma, beta, groups: int, silu: bool, dy, stats_ws, *, x1=None, add=None) -> torch.Tensor:
     """Input gradient of `groupnorm` (concat layout [.., C0 + C1]); stats_ws is the forward's workspace, or its
     (mean, rstd) block as a [B, groups, 2] tensor (`gn_stats` — sliceable along the batch)."""
@@ -543,4 +646,13 @@ def adamw(table: torch.Tensor, n_tensors: int, max_numel: int, lr: float, beta1:
     lib = _begin()
     _cabi.check(lib.sb200_adamw(_ctx(table), _stream(), _p(table), n_tensors, int(max_numel), float(lr), float(beta1),
                                 float(beta2), float(eps), float(weight_decay), int(step)))
+    _count()
+
+
+def adam_f32(table: torch.Tensor, n_tensors: int, max_numel: int, lr: float, beta1: float, beta2: float, eps: float,
+             weight_decay: float, step: int) -> None:
+    """One `adam_f32_kernel` launch over a device table of fp32 (p, g, m, v, n) records (int64 [n_tensors, 5])."""
+    lib = _begin()
+    _cabi.check(lib.sb200_adam_f32(_ctx(table), _stream(), _p(table), n_tensors, int(max_numel), float(lr),
+                                   float(beta1), float(beta2), float(eps), float(weight_decay), int(step)))
     _count()

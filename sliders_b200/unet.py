@@ -688,14 +688,35 @@ class UNet2DConditionModel(nn.Module):
     # ---- public forward --------------------------------------------------------------------------------
     def forward(self, sample, timestep, encoder_hidden_states=None, added_cond_kwargs=None,
                 cross_attention_kwargs=None, return_dict: bool = True, **unused):
-        if torch.is_grad_enabled() and self._needs_grad():
+        ehs_grad = (torch.is_grad_enabled() and torch.is_tensor(encoder_hidden_states)
+                    and encoder_hidden_states.requires_grad)
+        if torch.is_grad_enabled() and (self._needs_grad() or ehs_grad):
             # training: keep activations and hand torch.autograd a node whose backward runs the sb200 backward kernels
             return self._forward_nograd(sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict,
-                                        train=True)
+                                        train=True, ehs_grad=ehs_grad)
         with torch.no_grad():
             return self._forward_nograd(sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict)
 
-    def _forward_nograd(self, sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict, train=False):
+    def _check_ehs_grad(self, sample, added_cond_kwargs):
+        """The encoder_hidden_states gradient covers the batched cross-attention K / V path with frozen or trainable
+        adaptors elsewhere; the cases below are not implemented and say so instead of returning a silent None."""
+        if sample.requires_grad:
+            raise NotImplementedError("sliders_b200: a gradient w.r.t. `sample` (the latents) is not implemented")
+        for k, v in (added_cond_kwargs or {}).items():
+            if torch.is_tensor(v) and v.requires_grad:
+                raise NotImplementedError(f"sliders_b200: a gradient w.r.t. added_cond_kwargs['{k}'] is not implemented")
+        for _, _, mods in self._kv_plan().values():
+            for a in mods:
+                for leaf in (a.to_k, a.to_v):
+                    ad = _adaptor_of(leaf)
+                    if ad is not None and float(ad.multiplier) * float(ad.scale) != 0.0:
+                        raise NotImplementedError(
+                            "sliders_b200: a gradient w.r.t. encoder_hidden_states while adaptors on the cross-attention "
+                            "attn2.to_k / to_v are active (train methods xattn / full with multiplier != 0) is not "
+                            "implemented")
+
+    def _forward_nograd(self, sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict, train=False,
+                        ehs_grad=False):
         if not sample.is_cuda:
             raise RuntimeError("sliders_b200.UNet2DConditionModel runs only on a CUDA (sm_90) device; "
                                "there is no CPU path (the CPU oracle lives under oracle/ for tests)")
@@ -711,14 +732,19 @@ class UNet2DConditionModel(nn.Module):
         out_dtype = sample.dtype if sample.dtype in (torch.float32, BF16) else BF16
         x = sample if sample.dtype in (torch.float32, BF16) else sample.to(BF16)
         x = x.contiguous()
-        ehs = encoder_hidden_states.to(device=dev, dtype=BF16).contiguous()
         if train:
             from . import autograd as sb_autograd
 
-            out = sb_autograd.apply(self, x.detach(), t, ehs.detach(), added_cond_kwargs, out_dtype)
+            if ehs_grad:
+                self._check_ehs_grad(sample, added_cond_kwargs)
+            # the autograd node converts encoder_hidden_states to bf16 itself, so that its gradient can come back in
+            # the caller's dtype (fp32 for an optimised embedding)
+            out = sb_autograd.apply(self, x.detach(), t, encoder_hidden_states, added_cond_kwargs, out_dtype, ehs_grad)
         elif self.use_cuda_graph:
+            ehs = encoder_hidden_states.to(device=dev, dtype=BF16).contiguous()
             out = self._graphed(x, t, ehs, added_cond_kwargs, out_dtype)
         else:
+            ehs = encoder_hidden_states.to(device=dev, dtype=BF16).contiguous()
             out = self._forward_impl(x, t, ehs, added_cond_kwargs, out_dtype)
         if not return_dict:
             return (out,)
