@@ -8,9 +8,11 @@ The frozen weights need no gradient, so the pass is
   * per adapted leaf  y = W x + s up (down x):  d_up = s dY^T (x down^T),  d_down = s (dY up)^T x,  dX += s (dY up) down
     as rank-r reductions (csrc/backward.cu).
 `UNet2DConditionModel.forward` routes here (through `_UNetFunction`) whenever autograd is enabled and an active
-adaptor requires grad or `encoder_hidden_states` requires grad; otherwise the inference forward runs.  The training
-forward keeps the activations the backward needs (about 7 GB for an SDXL CFG pair at 1024 px) and applies GEGLU unfused
-so its pre-activation can be kept.
+adaptor requires grad or `encoder_hidden_states` requires grad; otherwise the inference forward runs.  Both run the one
+forward walk `UNet2DConditionModel._walk`: given a tape it also keeps the activations the backward needs (about 7 GB for
+an SDXL CFG pair at 1024 px), so the backward mirrors exactly the function inference computes, and it applies GEGLU
+unfused so its pre-activation can be kept.  Every Linear / conv leaf the walk runs carries its adaptor, if active, in
+both modes.
 The gradient w.r.t. `encoder_hidden_states` (null-text inversion optimises the unconditional text embedding through the
 UNet) is the transpose of the batched cross-attention K / V projection of the forward (`unet._kv_plan`): every
 cross-attention block's dK | dV lands in its columns of one [B * 77, sum 2C] matrix, and one fp32 split-K GEMM against
@@ -29,6 +31,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from . import ops
+from .unet import _GraphInputs
 
 BF16 = torch.bfloat16
 
@@ -98,13 +101,14 @@ class _Grads:
         return g, True
 
 
-def _snapshot_scales(unet) -> Dict[int, tuple]:
-    out = {}
+def _new_tape(unet) -> list:
+    """A tape for `unet._walk`, opened with the snapshot of the active adaptors that `_Grads` reads."""
+    scales = {}
     for leaf, a in unet._adapted_leaves():
         s = float(a.multiplier) * float(a.scale)
         if s != 0.0:
-            out[id(leaf)] = (a, s, bool(a.lora_down.weight.requires_grad))
-    return out
+            scales[id(leaf)] = (a, s, bool(a.lora_down.weight.requires_grad))
+    return [("scales", scales)]
 
 
 def _lora_linear_bwd(unet, grads: _Grads, leaf, xs: List[torch.Tensor], dY: torch.Tensor,
@@ -162,30 +166,8 @@ def _lora_conv_bwd(unet, grads: _Grads, conv, x: torch.Tensor, dY: torch.Tensor,
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# training forward (keeps what the backward needs) and the mirrored backward, block by block
+# the backward, block by block, of the records `UNet2DConditionModel._walk` leaves on the tape
 # ----------------------------------------------------------------------------------------------------------------
-def _resnet_fwd(unet, blk, x0, x1, emb_act):
-    B, H, W, _ = x0.shape
-    n1, n2 = blk.norm1, blk.norm2
-    ws1 = ops.gn_ws(B, n1.num_groups, x0.device)
-    h1 = ops.groupnorm(x0, *unet._w_norm(n1), n1.num_groups, n1.eps, True, x1=x1, stats_ws=ws1)
-    temb = ops.small_linear(emb_act, unet._w(blk.time_emb_proj), unet._b(blk.time_emb_proj),
-                            lora=unet._lora([blk.time_emb_proj]))
-    h2 = ops.conv3x3(h1, unet._w(blk.conv1), bias=unet._b(blk.conv1), rowbias=temb, lora=unet._lora([blk.conv1]))
-    ws2 = ops.gn_ws(B, n2.num_groups, x0.device)
-    h3 = ops.groupnorm(h2, *unet._w_norm(n2), n2.num_groups, n2.eps, True, stats_ws=ws2)
-    if blk.conv_shortcut is not None:
-        sc = blk.conv_shortcut
-        res = ops.gemm(x0.view(-1, x0.shape[-1]), unet._w(sc), bias=unet._b(sc),
-                       x1=x1.view(-1, x1.shape[-1]) if x1 is not None else None,
-                       lora=unet._lora([sc])).view(B, H, W, sc.weight.shape[0])
-    else:
-        assert x1 is None
-        res = x0
-    out = ops.conv3x3(h3, unet._w(blk.conv2), bias=unet._b(blk.conv2), resid=res, lora=unet._lora([blk.conv2]))
-    return out, (blk, x0, x1, emb_act, ops.gn_stats(ws1, B, n1.num_groups), h1, h2, ops.gn_stats(ws2, B, n2.num_groups), h3)
-
-
 def _resnet_bwd(unet, grads, rec, d_out, need_dx=True):
     """Returns (dx0, dx1): gradients w.r.t. the block input and the skip source (views of one concat buffer)."""
     blk, x0, x1, emb_act, ws1, h1, h2, ws2, h3 = rec
@@ -222,33 +204,6 @@ def _resnet_bwd(unet, grads, rec, d_out, need_dx=True):
     if x1 is None:
         return dx, None
     return dx[..., :C0], dx[..., C0:]
-
-
-def _attn_fwd(unet, attn, x_norm, resid, B, S, ctx=None, Sctx=0, kv_all=None):
-    """Training twin of UNet2DConditionModel._attn: also returns what the backward needs."""
-    C_ = attn.to_q.weight.shape[0]
-    scale = attn.dim_head ** -0.5
-    lse = torch.empty((B, attn.heads, S), device=x_norm.device, dtype=torch.float32)
-    if ctx is None:
-        leaves = [attn.to_q, attn.to_k, attn.to_v]
-        qkv = ops.gemm(x_norm, unet._fused_w(leaves), lora=unet._lora(leaves))
-        q, k, v = qkv[:, :C_], qkv[:, C_:2 * C_], qkv[:, 2 * C_:]
-        Skv = S
-    else:
-        q = ops.gemm(x_norm, unet._w(attn.to_q), lora=unet._lora([attn.to_q]))
-        if kv_all is not None:
-            kv, offs = kv_all[C_]
-            off = offs[id(attn)]
-            k, v = kv[:, off:off + C_], kv[:, off + C_:off + 2 * C_]
-        else:
-            kvl = [attn.to_k, attn.to_v]
-            kv = ops.gemm(ctx, unet._fused_w(kvl), lora=unet._lora(kvl))
-            k, v = kv[:, :C_], kv[:, C_:]
-        Skv = Sctx
-    o = ops.attention(q, k, v, B, attn.heads, S, Skv, scale, attn.dim_head, lse=lse)
-    out = attn.to_out[0]
-    h = ops.gemm(o, unet._w(out), bias=unet._b(out), resid=resid, lora=unet._lora([out]))
-    return h, (q, k, v, o, lse, Skv, ctx)
 
 
 def _attn_bwd(unet, grads, attn, rec, x_norm, d_h, B, S):
@@ -289,33 +244,6 @@ def _attn_bwd(unet, grads, attn, rec, x_norm, d_h, B, S):
     return d_n
 
 
-def _transformer_fwd(unet, tr, x, ctx, Sctx, kv_all):
-    B, H, W, C_ = x.shape
-    S = H * W
-    res = x.view(B * S, C_)
-    gn = tr.norm
-    ws = ops.gn_ws(B, gn.num_groups, x.device)
-    hn = ops.groupnorm(x, *unet._w_norm(gn), gn.num_groups, gn.eps, False, stats_ws=ws).view(B * S, C_)
-    h = ops.gemm(hn, unet._w(tr.proj_in), bias=unet._b(tr.proj_in), lora=unet._lora([tr.proj_in]))
-    blocks = []
-    for blk in tr.transformer_blocks:
-        h1 = h
-        n = ops.layernorm(h1, *unet._w_norm(blk.norm1), eps=blk.norm1.eps)
-        h, a1 = _attn_fwd(unet, blk.attn1, n, h1, B, S)
-        h2 = h
-        n = ops.layernorm(h2, *unet._w_norm(blk.norm2), eps=blk.norm2.eps)
-        h, a2 = _attn_fwd(unet, blk.attn2, n, h2, B, S, ctx=ctx, Sctx=Sctx, kv_all=kv_all)
-        h3 = h
-        n = ops.layernorm(h3, *unet._w_norm(blk.norm3), eps=blk.norm3.eps)
-        ffp, ffo = blk.ff.net[0].proj, blk.ff.net[2]
-        pre = ops.gemm(n, unet._w(ffp), bias=unet._b(ffp), lora=unet._lora([ffp]))
-        f = ops.geglu(pre)
-        h = ops.gemm(f, unet._w(ffo), bias=unet._b(ffo), resid=h3, lora=unet._lora([ffo]))
-        blocks.append((blk, h1, a1, h2, a2, h3, pre))
-    out = ops.gemm(h, unet._w(tr.proj_out), bias=unet._b(tr.proj_out), resid=res, lora=unet._lora([tr.proj_out]))
-    return out.view(B, H, W, C_), (tr, x, ops.gn_stats(ws, B, gn.num_groups), hn, blocks, h)
-
-
 def _transformer_bwd(unet, grads, rec, d_out):
     tr, x, ws, hn, blocks, h_last = rec
     B, H, W, C_ = x.shape
@@ -347,61 +275,6 @@ def _transformer_bwd(unet, grads, rec, d_out):
     _lora_linear_bwd(unet, grads, tr.proj_in, [hn], d_h, d_hn)
     gn = tr.norm
     return ops.groupnorm_bwd(x, *unet._w_norm(gn), gn.num_groups, False, d_hn.view(B, H, W, C_), ws, add=d_out)
-
-
-def forward_train(unet, sample, timesteps_f32, ehs, added_cond_kwargs, out_dtype):
-    """Same arithmetic as UNet2DConditionModel._forward_impl (GEGLU unfused); returns (eps, tape)."""
-    B = sample.shape[0]
-    Sctx = ehs.shape[1]
-    ctx = ehs.reshape(B * Sctx, ehs.shape[-1])
-    kv_all = unet._cross_kv(ctx)
-    emb = unet._embeddings(timesteps_f32, B, added_cond_kwargs)
-    h = ops.conv_in(sample, unet._w(unet.conv_in), unet._b(unet.conv_in))
-    tape = [("scales", _snapshot_scales(unet)), ("ctx", Sctx)]
-    skips = [h]
-    for blk in unet.down_blocks:
-        attns = getattr(blk, "attentions", None)
-        for i, rn in enumerate(blk.resnets):
-            h, rec = _resnet_fwd(unet, rn, h, None, emb)
-            tape.append(("res", rec))
-            if attns is not None:
-                h, rec = _transformer_fwd(unet, attns[i], h, ctx, Sctx, kv_all)
-                tape.append(("tr", rec))
-            skips.append(h)
-            tape.append(("skip", None))
-        if blk.downsamplers is not None:
-            conv = blk.downsamplers[0].conv
-            x_in = h
-            h = ops.conv3x3(h, unet._w(conv), stride=2, bias=unet._b(conv), lora=unet._lora([conv]))
-            tape.append(("down", (conv, x_in)))
-            skips.append(h)
-            tape.append(("skip", None))
-    mid = unet.mid_block
-    h, rec = _resnet_fwd(unet, mid.resnets[0], h, None, emb)
-    tape.append(("res", rec))
-    h, rec = _transformer_fwd(unet, mid.attentions[0], h, ctx, Sctx, kv_all)
-    tape.append(("tr", rec))
-    h, rec = _resnet_fwd(unet, mid.resnets[1], h, None, emb)
-    tape.append(("res", rec))
-    for blk in unet.up_blocks:
-        attns = getattr(blk, "attentions", None)
-        for i, rn in enumerate(blk.resnets):
-            h, rec = _resnet_fwd(unet, rn, h, skips.pop(), emb)
-            tape.append(("res", rec))
-            if attns is not None:
-                h, rec = _transformer_fwd(unet, attns[i], h, ctx, Sctx, kv_all)
-                tape.append(("tr", rec))
-        if blk.upsamplers is not None:
-            conv = blk.upsamplers[0].conv
-            x_in = h
-            h = ops.conv3x3(ops.upsample2x(h), unet._w(conv), bias=unet._b(conv), lora=unet._lora([conv]))
-            tape.append(("up", (conv, x_in)))
-    gn = unet.conv_norm_out
-    ws = ops.gn_ws(B, gn.num_groups, h.device)
-    hn = ops.groupnorm(h, *unet._w_norm(gn), gn.num_groups, gn.eps, True, stats_ws=ws)
-    out = ops.conv_out(hn, unet._w(unet.conv_out), unet._b(unet.conv_out), out_dtype=out_dtype)
-    tape.append(("out", (h, ops.gn_stats(ws, B, gn.num_groups))))
-    return out, tape
 
 
 def slice_tape(obj, lo: int, hi: int, B: int):
@@ -504,7 +377,7 @@ def _param_grad(shape, dtype, g: torch.Tensor) -> torch.Tensor:
     return g.reshape(shape).to(dtype)
 
 
-class _TrainCapture:
+class _TrainCapture(_GraphInputs):
     """Training forward + backward of one call signature as two CUDA graphs sharing a memory pool: the eager path is
     host-bound (~5 000 launches per CFG pair, 124 ms against ~75 ms of device time at SDXL size).  The activations
     of the tape live in the graph pool between the two replays; inputs, the incoming gradient and the flat gradient
@@ -512,12 +385,8 @@ class _TrainCapture:
     inference graphs use; the backward bakes it in, so the factor is part of the cache key."""
 
     def __init__(self, unet, sample, t, ehs, added, out_dtype, params, keys, need_ehs=False):
-        self.x, self.t, self.ehs = sample.clone(), t.clone(), ehs.clone()
+        super().__init__(sample, t, ehs, added)
         self.need_ehs = need_ehs
-        self.added = None
-        if added is not None:
-            self.added = {"text_embeds": added["text_embeds"].to(device=sample.device, dtype=BF16).clone(),
-                          "time_ids": added["time_ids"].to(device=sample.device, dtype=torch.float32).clone()}
         self.keys = keys
         self.meta = [(tuple(p.shape), p.dtype) for p in params]
         self.pending = False
@@ -525,16 +394,18 @@ class _TrainCapture:
         stream = torch.cuda.Stream(device=sample.device)
         stream.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(stream):  # warm-up: weight / LoRA packing caches, transposed weights, TMA descriptors
-            out, tape = forward_train(unet, self.x, self.t, self.ehs, self.added, out_dtype)
+            tape = _new_tape(unet)
+            out = unet._walk(self.x, self.t, self.ehs, self.added, out_dtype, tape)
             backward(unet, tape, torch.zeros_like(out), need_ehs)
             del tape
         torch.cuda.current_stream().wait_stream(stream)
         torch.cuda.synchronize()
         self.gf = torch.cuda.CUDAGraph()
+        self.tape = _new_tape(unet)
         unet._capturing = True
         try:
             with torch.cuda.graph(self.gf):
-                self.out, self.tape = forward_train(unet, self.x, self.t, self.ehs, self.added, out_dtype)
+                self.out = unet._walk(self.x, self.t, self.ehs, self.added, out_dtype, self.tape)
         finally:
             unet._capturing = False
         self.d_out = torch.zeros_like(self.out)
@@ -564,16 +435,7 @@ class _TrainCapture:
         self.bwd[dead] = (graph, flat, by_param.get("ehs"))
 
     def run_forward(self, unet, x, t, ehs, added):
-        self.x.copy_(x)
-        self.t.copy_(t)
-        self.ehs.copy_(ehs)
-        if added is not None:
-            self.added["text_embeds"].copy_(added["text_embeds"])
-            self.added["time_ids"].copy_(added["time_ids"])
-        _, common = unet._lora_signature()
-        if unet._slider_scale_dev is not None:
-            unet._slider_scale_dev.fill_(1.0 if common is None else common)
-        unet._refresh_lora_packs()
+        self.load(unet, x, t, ehs, added)
         self.gf.replay()
         self.pending = True
         return self.out.clone()
@@ -611,11 +473,8 @@ def _capture_for(unet, sample, t, ehs, added, out_dtype, params, keys, need_ehs=
     sig, common = unet._lora_signature()
     if common is None and any(sig[0]):
         return None
-    addk = None
-    if added is not None:
-        addk = (tuple(added["text_embeds"].shape), tuple(added["time_ids"].shape))
-    key = ("train", tuple(sample.shape), sample.dtype, tuple(ehs.shape), addk, out_dtype, sig,
-           round(common, 9) if common is not None else None, tuple(keys), bool(need_ehs))
+    key = (("train",) + _GraphInputs.key(sample, ehs, added, out_dtype)
+           + (sig, round(common, 9) if common is not None else None, tuple(keys), bool(need_ehs)))
     cache = unet.__dict__.setdefault("_train_graphs", {})
     cap = cache.get(key)
     if cap is None:
@@ -660,8 +519,8 @@ class _UNetFunction(torch.autograd.Function):
             fctx.token = _Token()
             fctx.cap.pending_token = weakref.ref(fctx.token)
             return fctx.cap.run_forward(unet, sample, t, ehs, added)
-        out, fctx.tape = forward_train(unet, sample, t, ehs, added, out_dtype)
-        return out
+        fctx.tape = _new_tape(unet)
+        return unet._walk(sample, t, ehs, added, out_dtype, fctx.tape)
 
     @staticmethod
     def backward(fctx, d_out):

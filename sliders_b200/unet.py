@@ -479,16 +479,21 @@ class UNet2DConditionModel(nn.Module):
     _bake_scales = False
 
     # ---- forward pieces ------------------------------------------------------------------------------
-    def _resnet(self, blk: ResnetBlock2D, x0, x1, emb_act) -> torch.Tensor:
+    # One walk serves inference and training.  `tape` is None for inference; for training it is a list to which every
+    # block appends what its backward reads (sliders_b200/autograd.py): the GroupNorm statistics, the attention
+    # log-sum-exp and the GEGLU pre-activation are kept, so GEGLU runs as GEMM + `ops.geglu` instead of in the epilogue.
+    def _resnet(self, blk: ResnetBlock2D, x0, x1, emb_act, tape=None) -> torch.Tensor:
         """x0 (and optional skip x1): [B,H,W,C*] NHWC.  emb_act: SiLU(emb) [B, 1280]."""
         B, H, W, _ = x0.shape
-        n1 = blk.norm1
-        h = ops.groupnorm(x0, self._w_norm(n1)[0], self._w_norm(n1)[1], n1.num_groups, n1.eps, True, x1=x1)
+        n1, n2 = blk.norm1, blk.norm2
+        ws1 = ws2 = None
+        if tape is not None:
+            ws1, ws2 = ops.gn_ws(B, n1.num_groups, x0.device), ops.gn_ws(B, n2.num_groups, x0.device)
+        h1 = ops.groupnorm(x0, *self._w_norm(n1), n1.num_groups, n1.eps, True, x1=x1, stats_ws=ws1)
         temb = ops.small_linear(emb_act, self._w(blk.time_emb_proj), self._b(blk.time_emb_proj),
                                 lora=self._lora([blk.time_emb_proj]))
-        h = ops.conv3x3(h, self._w(blk.conv1), bias=self._b(blk.conv1), rowbias=temb, lora=self._lora([blk.conv1]))
-        n2 = blk.norm2
-        h = ops.groupnorm(h, self._w_norm(n2)[0], self._w_norm(n2)[1], n2.num_groups, n2.eps, True)
+        h2 = ops.conv3x3(h1, self._w(blk.conv1), bias=self._b(blk.conv1), rowbias=temb, lora=self._lora([blk.conv1]))
+        h3 = ops.groupnorm(h2, *self._w_norm(n2), n2.num_groups, n2.eps, True, stats_ws=ws2)
         if blk.conv_shortcut is not None:
             sc = blk.conv_shortcut
             cout = sc.weight.shape[0]
@@ -498,7 +503,11 @@ class UNet2DConditionModel(nn.Module):
         else:
             assert x1 is None
             res = x0
-        return ops.conv3x3(h, self._w(blk.conv2), bias=self._b(blk.conv2), resid=res, lora=self._lora([blk.conv2]))
+        out = ops.conv3x3(h3, self._w(blk.conv2), bias=self._b(blk.conv2), resid=res, lora=self._lora([blk.conv2]))
+        if tape is not None:
+            tape.append(("res", (blk, x0, x1, emb_act, ops.gn_stats(ws1, B, n1.num_groups), h1, h2,
+                                 ops.gn_stats(ws2, B, n2.num_groups), h3)))
+        return out
 
     def _w_norm(self, norm: nn.Module):
         key = ("n", id(norm))
@@ -526,60 +535,90 @@ class UNet2DConditionModel(nn.Module):
             self._packed["kvplan"] = plan
         return plan
 
-    def _cross_kv(self, ctx):
-        """{C: (kv_all [B*77, n_blocks*2C], offsets)} or None when an active adaptor sits on a to_k / to_v of attn2
-        (train methods xattn / full: those keep the per-block fused path with its own LoRA stack)."""
-        plan = self._kv_plan()
-        for _, _, mods in plan.values():
+    def _cross_kv_adapted(self) -> bool:
+        """True when an active adaptor sits on a to_k / to_v of attn2 (train methods xattn / full)."""
+        for _, _, mods in self._kv_plan().values():
             for a in mods:
                 for leaf in (a.to_k, a.to_v):
                     ad = _adaptor_of(leaf)
                     if ad is not None and float(ad.multiplier) * float(ad.scale) != 0.0:
-                        return None
-        return {C_: (ops.gemm(ctx, w), offs) for C_, (w, offs, _) in plan.items()}
+                        return True
+        return False
 
-    def _attn(self, attn: Attention, x_norm, resid, B, S, ctx=None, Sctx=0, kv_all=None):
-        """x_norm: [B*S, C] normalised input; returns resid + to_out(attention)."""
+    def _cross_kv(self, ctx):
+        """{C: (kv_all [B*77, n_blocks*2C], offsets)} or None when attn2's to_k / to_v carry active adaptors: those
+        blocks keep the per-block fused path with its own LoRA stack."""
+        if self._cross_kv_adapted():
+            return None
+        return {C_: (ops.gemm(ctx, w), offs) for C_, (w, offs, _) in self._kv_plan().items()}
+
+    def _kv(self, attn: Attention, ctx, kv_all):
+        """K, V of a cross-attention block: its columns of the batched projection `kv_all`, or its own fused
+        to_k|to_v GEMM when there is none."""
+        C_ = attn.to_k.weight.shape[0]
+        if kv_all is not None:
+            kv, offs = kv_all[C_]
+            off = offs[id(attn)]
+            return kv[:, off:off + C_], kv[:, off + C_:off + 2 * C_]
+        kvl = [attn.to_k, attn.to_v]
+        kv = ops.gemm(ctx, self._fused_w(kvl), lora=self._lora(kvl))
+        return kv[:, :C_], kv[:, C_:]
+
+    def _attn(self, attn: Attention, x_norm, resid, B, S, ctx=None, Sctx=0, kv_all=None, keep=False):
+        """x_norm: [B*S, C] normalised input; returns (resid + to_out(attention), the backward's record or None)."""
         C_ = attn.to_q.weight.shape[0]
         scale = attn.dim_head ** -0.5
         if ctx is None:
             leaves = [attn.to_q, attn.to_k, attn.to_v]
             qkv = ops.gemm(x_norm, self._fused_w(leaves), lora=self._lora(leaves))
-            o = ops.attention(qkv[:, :C_], qkv[:, C_:2 * C_], qkv[:, 2 * C_:], B, attn.heads, S, S, scale, attn.dim_head)
+            q, k, v = qkv[:, :C_], qkv[:, C_:2 * C_], qkv[:, 2 * C_:]
+            Skv = S
         else:
             q = ops.gemm(x_norm, self._w(attn.to_q), lora=self._lora([attn.to_q]))
-            if kv_all is not None:
-                kv, offs = kv_all[C_]
-                off = offs[id(attn)]
-                k, v = kv[:, off:off + C_], kv[:, off + C_:off + 2 * C_]
-            else:
-                kvl = [attn.to_k, attn.to_v]
-                kv = ops.gemm(ctx, self._fused_w(kvl), lora=self._lora(kvl))
-                k, v = kv[:, :C_], kv[:, C_:]
-            o = ops.attention(q, k, v, B, attn.heads, S, Sctx, scale, attn.dim_head)
+            k, v = self._kv(attn, ctx, kv_all)
+            Skv = Sctx
+        lse = torch.empty((B, attn.heads, S), device=x_norm.device, dtype=torch.float32) if keep else None
+        o = ops.attention(q, k, v, B, attn.heads, S, Skv, scale, attn.dim_head, lse=lse)
         out = attn.to_out[0]
-        return ops.gemm(o, self._w(out), bias=self._b(out), resid=resid, lora=self._lora([out]))
+        h = ops.gemm(o, self._w(out), bias=self._b(out), resid=resid, lora=self._lora([out]))
+        return h, ((q, k, v, o, lse, Skv, ctx) if keep else None)
 
-    def _transformer(self, tr: Transformer2DModel, x, ctx, Sctx, kv_all=None) -> torch.Tensor:
+    def _transformer(self, tr: Transformer2DModel, x, ctx, Sctx, kv_all=None, tape=None) -> torch.Tensor:
         B, H, W, C_ = x.shape
         S = H * W
         res = x.view(B * S, C_)
         gn = tr.norm
-        h = ops.groupnorm(x, self._w_norm(gn)[0], self._w_norm(gn)[1], gn.num_groups, gn.eps, False).view(B * S, C_)
-        if self.fuse_layernorm and C_ >= self.fuse_layernorm_min_c:
-            return self._transformer_lnfold(tr, h, res, ctx, Sctx, kv_all, B, S).view(B, H, W, C_)
-        h = ops.gemm(h, self._w(tr.proj_in), bias=self._b(tr.proj_in))
+        keep = tape is not None
+        ws = ops.gn_ws(B, gn.num_groups, x.device) if keep else None
+        hn = ops.groupnorm(x, *self._w_norm(gn), gn.num_groups, gn.eps, False, stats_ws=ws).view(B * S, C_)
+        if not keep and self.fuse_layernorm and C_ >= self.fuse_layernorm_min_c:
+            return self._transformer_lnfold(tr, hn, res, ctx, Sctx, kv_all, B, S).view(B, H, W, C_)
+        h = ops.gemm(hn, self._w(tr.proj_in), bias=self._b(tr.proj_in), lora=self._lora([tr.proj_in]))
+        blocks = []
         for blk in tr.transformer_blocks:
-            n = ops.layernorm(h, *self._w_norm(blk.norm1), eps=blk.norm1.eps)
-            h = self._attn(blk.attn1, n, h, B, S)
-            n = ops.layernorm(h, *self._w_norm(blk.norm2), eps=blk.norm2.eps)
-            h = self._attn(blk.attn2, n, h, B, S, ctx=ctx, Sctx=Sctx, kv_all=kv_all)
-            n = ops.layernorm(h, *self._w_norm(blk.norm3), eps=blk.norm3.eps)
+            h1 = h
+            n = ops.layernorm(h1, *self._w_norm(blk.norm1), eps=blk.norm1.eps)
+            h, a1 = self._attn(blk.attn1, n, h1, B, S, keep=keep)
+            h2 = h
+            n = ops.layernorm(h2, *self._w_norm(blk.norm2), eps=blk.norm2.eps)
+            h, a2 = self._attn(blk.attn2, n, h2, B, S, ctx=ctx, Sctx=Sctx, kv_all=kv_all, keep=keep)
+            h3 = h
+            n = ops.layernorm(h3, *self._w_norm(blk.norm3), eps=blk.norm3.eps)
             ffp, ffo = blk.ff.net[0].proj, blk.ff.net[2]
-            f = ops.gemm(n, self._w(ffp), bias=self._b(ffp), geglu=True)
-            h = ops.gemm(f, self._w(ffo), bias=self._b(ffo), resid=h)
-        h = ops.gemm(h, self._w(tr.proj_out), bias=self._b(tr.proj_out), resid=res)
-        return h.view(B, H, W, C_)
+            la = self._lora([ffp])
+            pre = None
+            if keep or la is not None:  # the GEGLU epilogue carries no LoRA, and the backward needs `pre`
+                pre = ops.gemm(n, self._w(ffp), bias=self._b(ffp), lora=la)
+                f = ops.geglu(pre)
+            else:
+                f = ops.gemm(n, self._w(ffp), bias=self._b(ffp), geglu=True)
+            h = ops.gemm(f, self._w(ffo), bias=self._b(ffo), resid=h3, lora=self._lora([ffo]))
+            if keep:
+                blocks.append((blk, h1, a1, h2, a2, h3, pre))
+        out = ops.gemm(h, self._w(tr.proj_out), bias=self._b(tr.proj_out), resid=res, lora=self._lora([tr.proj_out]))
+        if keep:
+            tape.append(("tr", (tr, x, ops.gn_stats(ws, B, gn.num_groups), hn, blocks, h)))
+        return out.view(B, H, W, C_)
 
     def _transformer_lnfold(self, tr: Transformer2DModel, h, res, ctx, Sctx, kv_all, B, S) -> torch.Tensor:
         """The same block sequence without LayerNorm launches: every GEMM that writes the residual stream (proj_in, the
@@ -603,9 +642,11 @@ class UNet2DConditionModel(nn.Module):
             wp, c, d = self._ln_pack(norm, leaves)
             la, cl, dl = self._ln_lora(norm, leaves)
             fold = ops.LnFold(stats[0], stats[1], C_, norm.eps, c, d, cl, dl)
+            if geglu and la is not None:  # the GEGLU epilogue carries no LoRA
+                return ops.geglu(ops.gemm(x, wp, lora=la, ln=fold))
             return ops.gemm(x, wp, geglu=geglu, lora=la, ln=fold)
 
-        h, st = produce(h, tr.proj_in, None)
+        h, st = produce(h, tr.proj_in, None, self._lora([tr.proj_in]))
         for blk in tr.transformer_blocks:
             a1, a2 = blk.attn1, blk.attn2
             qkv = consume(h, st, blk.norm1, [a1.to_q, a1.to_k, a1.to_v])
@@ -613,20 +654,13 @@ class UNet2DConditionModel(nn.Module):
                               a1.dim_head)
             h, st = produce(o, a1.to_out[0], h, self._lora([a1.to_out[0]]))
             q = consume(h, st, blk.norm2, [a2.to_q])
-            if kv_all is not None:
-                kv, offs = kv_all[C_]
-                off = offs[id(a2)]
-                k, v = kv[:, off:off + C_], kv[:, off + C_:off + 2 * C_]
-            else:
-                kvl = [a2.to_k, a2.to_v]
-                kv = ops.gemm(ctx, self._fused_w(kvl), lora=self._lora(kvl))
-                k, v = kv[:, :C_], kv[:, C_:]
+            k, v = self._kv(a2, ctx, kv_all)
             o = ops.attention(q, k, v, B, a2.heads, S, Sctx, a2.dim_head ** -0.5, a2.dim_head)
             h, st = produce(o, a2.to_out[0], h, self._lora([a2.to_out[0]]))
             ffp, ffo = blk.ff.net[0].proj, blk.ff.net[2]
             f = consume(h, st, blk.norm3, [ffp], geglu=True)
-            h, st = produce(f, ffo, h)
-        return ops.gemm(h, self._w(tr.proj_out), bias=self._b(tr.proj_out), resid=res)
+            h, st = produce(f, ffo, h, self._lora([ffo]))
+        return ops.gemm(h, self._w(tr.proj_out), bias=self._b(tr.proj_out), resid=res, lora=self._lora([tr.proj_out]))
 
     def _embeddings(self, timesteps_f32, B, added_cond_kwargs):
         """Returns SiLU(emb) [B, temb].  In diffusers `emb` has exactly one kind of consumer — every
@@ -648,42 +682,55 @@ class UNet2DConditionModel(nn.Module):
             emb = ops.small_linear(a, self._w(ae.linear_2), self._b(ae.linear_2), resid=emb, act_out=2)
         return emb
 
-    def _forward_impl(self, sample, timesteps_f32, ehs, added_cond_kwargs, out_dtype):
+    def _walk(self, sample, timesteps_f32, ehs, added_cond_kwargs, out_dtype, tape=None):
+        """The UNet forward.  With a `tape` (a list) it also records, in order, what the backward reads: ("ctx", tokens
+        of encoder_hidden_states), then one ("res" | "tr" | "skip" | "down" | "up" | "out", record) per block."""
+        def record(kind, rec):
+            if tape is not None:
+                tape.append((kind, rec))
+
         B = sample.shape[0]
         Sctx = ehs.shape[1]
         ctx = ehs.reshape(B * Sctx, ehs.shape[-1])
         kv_all = self._cross_kv(ctx)
         emb = self._embeddings(timesteps_f32, B, added_cond_kwargs)
         h = ops.conv_in(sample, self._w(self.conv_in), self._b(self.conv_in))
+        record("ctx", Sctx)
         skips = [h]
         for blk in self.down_blocks:
             attns = getattr(blk, "attentions", None)
             for i, rn in enumerate(blk.resnets):
-                h = self._resnet(rn, h, None, emb)
+                h = self._resnet(rn, h, None, emb, tape)
                 if attns is not None:
-                    h = self._transformer(attns[i], h, ctx, Sctx, kv_all)
+                    h = self._transformer(attns[i], h, ctx, Sctx, kv_all, tape)
                 skips.append(h)
+                record("skip", None)
             if blk.downsamplers is not None:
                 conv = blk.downsamplers[0].conv
+                record("down", (conv, h))
                 h = ops.conv3x3(h, self._w(conv), stride=2, bias=self._b(conv), lora=self._lora([conv]))
                 skips.append(h)
+                record("skip", None)
         mid = self.mid_block
-        h = self._resnet(mid.resnets[0], h, None, emb)
-        h = self._transformer(mid.attentions[0], h, ctx, Sctx, kv_all)
-        h = self._resnet(mid.resnets[1], h, None, emb)
+        h = self._resnet(mid.resnets[0], h, None, emb, tape)
+        h = self._transformer(mid.attentions[0], h, ctx, Sctx, kv_all, tape)
+        h = self._resnet(mid.resnets[1], h, None, emb, tape)
         for blk in self.up_blocks:
             attns = getattr(blk, "attentions", None)
             for i, rn in enumerate(blk.resnets):
-                h = self._resnet(rn, h, skips.pop(), emb)
+                h = self._resnet(rn, h, skips.pop(), emb, tape)
                 if attns is not None:
-                    h = self._transformer(attns[i], h, ctx, Sctx, kv_all)
+                    h = self._transformer(attns[i], h, ctx, Sctx, kv_all, tape)
             if blk.upsamplers is not None:
                 conv = blk.upsamplers[0].conv
-                h = ops.upsample2x(h)
-                h = ops.conv3x3(h, self._w(conv), bias=self._b(conv), lora=self._lora([conv]))
+                record("up", (conv, h))
+                h = ops.conv3x3(ops.upsample2x(h), self._w(conv), bias=self._b(conv), lora=self._lora([conv]))
         gn = self.conv_norm_out
-        h = ops.groupnorm(h, self._w_norm(gn)[0], self._w_norm(gn)[1], gn.num_groups, gn.eps, True)
-        return ops.conv_out(h, self._w(self.conv_out), self._b(self.conv_out), out_dtype=out_dtype)
+        ws = ops.gn_ws(B, gn.num_groups, h.device) if tape is not None else None
+        hn = ops.groupnorm(h, *self._w_norm(gn), gn.num_groups, gn.eps, True, stats_ws=ws)
+        if tape is not None:
+            tape.append(("out", (h, ops.gn_stats(ws, B, gn.num_groups))))
+        return ops.conv_out(hn, self._w(self.conv_out), self._b(self.conv_out), out_dtype=out_dtype)
 
     # ---- public forward --------------------------------------------------------------------------------
     def forward(self, sample, timestep, encoder_hidden_states=None, added_cond_kwargs=None,
@@ -705,15 +752,10 @@ class UNet2DConditionModel(nn.Module):
         for k, v in (added_cond_kwargs or {}).items():
             if torch.is_tensor(v) and v.requires_grad:
                 raise NotImplementedError(f"sliders_b200: a gradient w.r.t. added_cond_kwargs['{k}'] is not implemented")
-        for _, _, mods in self._kv_plan().values():
-            for a in mods:
-                for leaf in (a.to_k, a.to_v):
-                    ad = _adaptor_of(leaf)
-                    if ad is not None and float(ad.multiplier) * float(ad.scale) != 0.0:
-                        raise NotImplementedError(
-                            "sliders_b200: a gradient w.r.t. encoder_hidden_states while adaptors on the cross-attention "
-                            "attn2.to_k / to_v are active (train methods xattn / full with multiplier != 0) is not "
-                            "implemented")
+        if self._cross_kv_adapted():
+            raise NotImplementedError(
+                "sliders_b200: a gradient w.r.t. encoder_hidden_states while adaptors on the cross-attention "
+                "attn2.to_k / to_v are active (train methods xattn / full with multiplier != 0) is not implemented")
 
     def _forward_nograd(self, sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict, train=False,
                         ehs_grad=False):
@@ -745,7 +787,7 @@ class UNet2DConditionModel(nn.Module):
             out = self._graphed(x, t, ehs, added_cond_kwargs, out_dtype)
         else:
             ehs = encoder_hidden_states.to(device=dev, dtype=BF16).contiguous()
-            out = self._forward_impl(x, t, ehs, added_cond_kwargs, out_dtype)
+            out = self._walk(x, t, ehs, added_cond_kwargs, out_dtype)
         if not return_dict:
             return (out,)
         return UNet2DConditionOutput(sample=out)
@@ -780,10 +822,7 @@ class UNet2DConditionModel(nn.Module):
 
     def _graphed(self, x, t, ehs, added, out_dtype):
         sig, _ = self._lora_signature()
-        addk = None
-        if added is not None:
-            addk = (tuple(added["text_embeds"].shape), tuple(added["time_ids"].shape))
-        key = (tuple(x.shape), x.dtype, tuple(ehs.shape), addk, out_dtype, sig)
+        key = _GraphInputs.key(x, ehs, added, out_dtype) + (sig,)
         cap = self._graphs.get(key)
         if cap is None:
             cap = _CapturedForward(self, x, t, ehs, added, out_dtype)
@@ -791,39 +830,29 @@ class UNet2DConditionModel(nn.Module):
         return cap.replay(self, x, t, ehs, added)
 
 
-class _CapturedForward:
-    """One captured CUDA graph of the whole UNet forward for fixed shapes (inputs are copied into static
-    buffers; the LoRA slider factor and the timestep are device-side values, so one graph serves every
-    denoise step and every slider scale)."""
+class _GraphInputs:
+    """Static input buffers of a captured UNet graph (sample, timesteps, encoder_hidden_states, added_cond_kwargs) and
+    what every replay does before the graph runs.  Shared by the inference graph below and the training graphs of
+    sliders_b200/autograd.py."""
 
-    def __init__(self, unet: UNet2DConditionModel, x, t, ehs, added, out_dtype):
+    def __init__(self, x, t, ehs, added):
         self.x, self.t, self.ehs = x.clone(), t.clone(), ehs.clone()
         self.added = None
         if added is not None:
             self.added = {"text_embeds": added["text_embeds"].to(device=x.device, dtype=BF16).clone(),
                           "time_ids": added["time_ids"].to(device=x.device, dtype=torch.float32).clone()}
-        # one decision for the whole graph: a factor common to ALL active adaptors is a device-side scalar (one graph
-        # serves every slider scale); otherwise the factors are baked into the packed weights (and are part of the key)
-        self.bake = unet._lora_signature()[1] is None
-        unet._bake_scales = self.bake
-        stream = torch.cuda.Stream(device=x.device)
-        stream.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(stream):
-            for _ in range(2):  # warm-up: fills weight / LoRA packing caches and the TMA descriptor cache
-                unet._forward_impl(self.x, self.t, self.ehs, self.added, out_dtype)
-        torch.cuda.current_stream().wait_stream(stream)
-        torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        unet._capturing = True
-        try:
-            with torch.cuda.graph(self.graph):
-                self.out = unet._forward_impl(self.x, self.t, self.ehs, self.added, out_dtype)
-        finally:
-            unet._capturing = False
-            unet._bake_scales = False
-        self.launches = None
 
-    def replay(self, unet: UNet2DConditionModel, x, t, ehs, added):
+    @staticmethod
+    def key(x, ehs, added, out_dtype) -> tuple:
+        """The shape part of a graph cache key."""
+        addk = None
+        if added is not None:
+            addk = (tuple(added["text_embeds"].shape), tuple(added["time_ids"].shape))
+        return (tuple(x.shape), x.dtype, tuple(ehs.shape), addk, out_dtype)
+
+    def load(self, unet: UNet2DConditionModel, x, t, ehs, added, bake: bool = False) -> None:
+        """Copies the call's inputs in, sets the device-side slider factor and refreshes the packed LoRA weights if the
+        optimiser changed them (same storage, so the graph sees them)."""
         self.x.copy_(x)
         self.t.copy_(t)
         self.ehs.copy_(ehs)
@@ -833,12 +862,42 @@ class _CapturedForward:
         _, common = unet._lora_signature()
         if unet._slider_scale_dev is not None:
             unet._slider_scale_dev.fill_(1.0 if common is None else common)
-        # refresh packed LoRA weights if the optimiser changed them (same storage, so the graph sees them)
-        unet._bake_scales = self.bake
+        unet._bake_scales = bake
         try:
             unet._refresh_lora_packs()
         finally:
             unet._bake_scales = False
+
+
+class _CapturedForward(_GraphInputs):
+    """One captured CUDA graph of the whole UNet forward for fixed shapes (inputs are copied into static
+    buffers; the LoRA slider factor and the timestep are device-side values, so one graph serves every
+    denoise step and every slider scale)."""
+
+    def __init__(self, unet: UNet2DConditionModel, x, t, ehs, added, out_dtype):
+        super().__init__(x, t, ehs, added)
+        # one decision for the whole graph: a factor common to ALL active adaptors is a device-side scalar (one graph
+        # serves every slider scale); otherwise the factors are baked into the packed weights (and are part of the key)
+        self.bake = unet._lora_signature()[1] is None
+        unet._bake_scales = self.bake
+        stream = torch.cuda.Stream(device=x.device)
+        stream.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(stream):
+            for _ in range(2):  # warm-up: fills weight / LoRA packing caches and the TMA descriptor cache
+                unet._walk(self.x, self.t, self.ehs, self.added, out_dtype)
+        torch.cuda.current_stream().wait_stream(stream)
+        torch.cuda.synchronize()
+        self.graph = torch.cuda.CUDAGraph()
+        unet._capturing = True
+        try:
+            with torch.cuda.graph(self.graph):
+                self.out = unet._walk(self.x, self.t, self.ehs, self.added, out_dtype)
+        finally:
+            unet._capturing = False
+            unet._bake_scales = False
+
+    def replay(self, unet: UNet2DConditionModel, x, t, ehs, added):
+        self.load(unet, x, t, ehs, added, self.bake)
         self.graph.replay()
         return self.out.clone()
 

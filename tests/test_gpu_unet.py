@@ -556,6 +556,73 @@ def test_tiny_xl_gradients_other_train_methods(dev, method, n_expected):
         assert any("attn2_to_k" in l.lora_name for l in net.unet_loras)
 
 
+@pytest.mark.parametrize("config", ["tiny_xl", "tiny_sd"])
+def test_tiny_transformer_leaf_adaptors_inference_and_gradients(dev, config):
+    """c3lier plus "Transformer2DModel" in the target list (the reference keeps it as a commented-out target): adaptors
+    also sit on proj_in / proj_out (1x1 convs in SD1.x), the feed-forward and attn2.  The no_grad forward (plain and
+    LayerNorm-folded) and the grad-mode forward must all compute the fp32 oracle with the LoRA folded in, and the
+    gradients of every adaptor must match the oracle's."""
+    from oracle import unet as ounet
+    from sliders_b200 import lora as plora, synthetic
+    from sliders_b200.unet import UNet2DConditionModel, UNetConfig
+
+    ocfg = getattr(ounet.UNetConfig, config)()
+    pm = UNet2DConditionModel(UNetConfig.from_dict(ocfg.__dict__))
+    synthetic.init_synthetic_(pm, seed=41)
+    pm = pm.to(dev, BF).eval().requires_grad_(False)
+    om = ounet.UNet2DConditionModel(ocfg)
+    om.load_state_dict({k: v.float() for k, v in pm.state_dict().items()})  # the bf16-rounded weights
+    om = om.to(dev).eval().requires_grad_(False)
+    with c3lier(plora):
+        plora.DEFAULT_TARGET_REPLACE.append("Transformer2DModel")
+        net = plora.LoRANetwork(pm, rank=4, multiplier=1.0, alpha=2.0, train_method="noxattn").to(dev, BF)
+    names = [l.lora_name for l in net.unet_loras]
+    for leaf in ("proj_in", "proj_out", "ff_net_0_proj", "ff_net_2"):
+        assert any(n.endswith(leaf) for n in names), leaf
+    synthetic.init_lora_nonzero_(net, seed=42, up_std=0.05, reseed_down=True)
+    g = torch.Generator().manual_seed(43)
+    x = torch.randn(2, 4, 32, 32, generator=g).to(dev, BF)
+    ehs = torch.randn(2, 77, ocfg.cross_attention_dim, generator=g).to(dev, BF)
+    added = None
+    if ocfg.addition_embed_type == "text_time":
+        added = {"text_embeds": torch.randn(2, 128, generator=g).to(dev, BF),
+                 "time_ids": torch.tensor([[256., 256., 0., 0., 256., 256.]] * 2, device=dev)}
+    goal = torch.randn(2, 4, 32, 32, generator=g).to(dev)
+    net.set_lora_slider(0.5)
+    eps = {}
+    for fold in (False, True):
+        pm.fuse_layernorm = fold
+        with torch.no_grad(), net:
+            eps[f"no_grad fold={fold}"] = pm(x, 321, encoder_hidden_states=ehs, added_cond_kwargs=added).sample
+    pm.fuse_layernorm = False
+    net.requires_grad_(True)
+    with net:
+        pred = pm(x, 321, encoder_hidden_states=ehs, added_cond_kwargs=added).sample
+    assert pred.requires_grad
+    eps["grad"] = pred.detach()
+    torch.nn.functional.mse_loss(pred.float(), goal).backward()
+    torch.cuda.synchronize()
+    ref = {}
+
+    def call(fp):
+        kw = {"added_cond_kwargs": {k: v.float() for k, v in added.items()}} if added is not None else {}
+        out = torch.func.functional_call(om, fp, (x.float(), 321, ehs.float()), kw).sample
+        ref["eps"] = out.detach()
+        return torch.nn.functional.mse_loss(out, goal)
+
+    leaves = _oracle_lora_grads(om, net, 0.5, call)
+    for what, got in eps.items():
+        assert rel_rms(got, ref["eps"]) < 2.5e-2, (config, what, rel_rms(got, ref["eps"]))
+    num = den = 0.0
+    for l in net.unet_loras:
+        for got, want in ((l.lora_down.weight.grad, leaves[l.lora_name][0].grad),
+                          (l.lora_up.weight.grad, leaves[l.lora_name][1].grad)):
+            assert got is not None and torch.isfinite(got).all(), l.lora_name
+            num += (got.float() - want).pow(2).sum().item()
+            den += want.pow(2).sum().item()
+    assert (num / den) ** 0.5 < 5e-2, (config, (num / den) ** 0.5)
+
+
 @pytest.mark.parametrize("h,w", [(72, 88), (40, 104), (24, 36)])
 def test_tiny_xl_bucket_resolutions_forward_and_gradients(dev, h, w):
     """`dynamic_resolution` draws latent sizes that are multiples of 8 but neither square nor powers of two

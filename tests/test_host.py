@@ -269,6 +269,55 @@ def test_launch_plan_dry_run_counts_and_flops():
     assert abs(per_pass - 6.761e12) / 6.761e12 < 0.01, per_pass
 
 
+def _lora_calls(plan):
+    """Indices of the GEMM / conv / small-linear launches that carry a LoRA adaptor (tag letter L)."""
+    return [i for i, (_, d, _) in enumerate(plan) if "L" in d.split(" (")[0].split()[-1]]
+
+
+def _unfuse_geglu(plan):
+    """The inference plan in training form: a GEMM with the GEGLU epilogue becomes the plain GEMM + `geglu`."""
+    out = []
+    for k, d, f in plan:
+        head, tag = d.rsplit(" ", 1)
+        if k == "gemm_kernel" and d.startswith("gemm") and "G" in tag:
+            out.append((k, head + " " + tag.replace("G", ""), f))
+            M, N = (int(w[1:]) for w in head.split()[1:3])
+            out.append(("geglu_kernel", f"geglu M{M} N{N // 2}", 0.0))
+        else:
+            out.append((k, d, f))
+    return out
+
+
+def test_training_walk_matches_inference_walk_dry_run():
+    """The training forward is the inference walk with a tape: on the meta device both walks of SDXL put LoRA on the same
+    GEMM / conv calls, and the training plan equals the inference plan except that each GEGLU fused into a GEMM runs as
+    GEMM + `geglu` and attention keeps its log-sum-exp.  Also with adaptors on every Transformer2DModel leaf
+    (proj_in / proj_out, the feed-forward, attn2), which the inference walk must apply like the training walk."""
+    import json
+    import subprocess
+    import sys as _sys
+
+    code = (
+        "import sys, json; sys.path.insert(0, %r); sys.path.insert(0, %r + '/tools');"
+        "import shape_trace as st;"
+        "print(json.dumps({str(i): [st.trace(2, train=t, extra_targets=e) for t in (False, True)]"
+        " for i, e in enumerate([(), ('Transformer2DModel',)])}))" % (ROOT, ROOT))
+    out = subprocess.run([_sys.executable, "-c", code], capture_output=True, text=True, timeout=300)
+    assert out.returncode == 0, out.stderr[-2000:]
+    plans = json.loads(out.stdout.strip().splitlines()[-1])
+    for net, (inf, train) in plans.items():
+        inf = [tuple(c) for c in inf]
+        train = [tuple(c) for c in train]
+        assert _lora_calls(inf) and len(_lora_calls(inf)) == len(_lora_calls(train)), net
+        assert all("lse" in d for k, d, _ in train if k == "attention_kernel")
+        assert not any("lse" in d for k, d, _ in inf if k == "attention_kernel")
+        assert _unfuse_geglu(inf) == [(k, d.replace(" lse", ""), f) for k, d, f in train], net
+    c3lier_inf, c3lier_train = plans["0"]
+    assert len(c3lier_inf) == 1008 and len(c3lier_train) == 1078
+    # every Transformer2DModel leaf adapted: 70 x (attn2 q / kv / out, ff in / out) + 11 x (proj_in, proj_out) more
+    assert len(_lora_calls(plans["1"][0])) == len(_lora_calls(c3lier_inf)) + 70 * 5 + 11 * 2
+
+
 # ---------------------------------------------------------------------------------------- trainer host logic
 def test_prompt_pair_loss_and_optimizer_factory():
     from sliders_b200 import trainer, train_util

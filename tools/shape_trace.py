@@ -1,5 +1,6 @@
 """Dry-run the UNet forward on the meta device to list every kernel call with its shape, then (optionally)
 join it with an ncu launch list (gpu__time_duration per launch, same order) to get a per-shape time table.
+`trace(batch, train=True)` lists the training walk instead (tape kept: GEGLU unfused, attention keeps its lse).
 
     python tools/shape_trace.py 8 gpurun_out/launches_b8.csv
 """
@@ -45,9 +46,16 @@ def conv3x3(x0, w, *, x1=None, stride=1, bias=None, rowbias=None, resid=None, lo
     return _meta(B, H // stride, W // stride, Cout)
 
 
-def attention(q, k, v, B, heads, Sq, Skv, scale, head_dim=64):
-    calls.append(("attention_kernel", f"attn B{B} h{heads} Sq{Sq} Skv{Skv}", 4.0 * B * heads * Sq * Skv * 64))
+def attention(q, k, v, B, heads, Sq, Skv, scale, head_dim=64, lse=None):
+    keep = " lse" if lse is not None else ""
+    calls.append(("attention_kernel", f"attn B{B} h{heads} Sq{Sq} Skv{Skv}{keep}", 4.0 * B * heads * Sq * Skv * 64))
     return _meta(B * Sq, heads * 64)
+
+
+def geglu(pre):
+    M, F2 = pre.shape
+    calls.append(("geglu_kernel", f"geglu M{M} N{F2 // 2}", 0.0))
+    return _meta(M, F2 // 2)
 
 
 def groupnorm(x0, gamma, beta, groups, eps, silu, *, x1=None, stats_ws=None):
@@ -64,7 +72,8 @@ def layernorm(x, gamma, beta, eps=1e-5):
 
 
 def small_linear(x, w, bias=None, *, act_in=False, act_out=0, lora=None, resid=None):
-    calls.append(("small_linear_kernel", f"small_linear M{x.shape[0]} N{w.shape[0]} K{x.shape[1]}", 0.0))
+    tag = " L" if lora is not None else ""
+    calls.append(("small_linear_kernel", f"small_linear M{x.shape[0]} N{w.shape[0]} K{x.shape[1]}{tag}", 0.0))
     return _meta(x.shape[0], w.shape[0])
 
 
@@ -91,16 +100,19 @@ def upsample2x(x):
     return _meta(B, 2 * H, 2 * W, C)
 
 
-def trace(batch, with_lora=True):
-    for name in ("gemm", "conv3x3", "attention", "groupnorm", "layernorm", "small_linear", "sinusoid", "conv_in",
-                 "conv_out", "upsample2x"):
+def trace(batch, with_lora=True, train=False, extra_targets=()):
+    """The launch plan of one SDXL forward: the inference walk, or with `train` the training walk (tape kept).  The
+    LoRA network is `noxattn` on the default targets plus the conv targets (c3lier) plus `extra_targets`."""
+    calls.clear()
+    for name in ("gemm", "conv3x3", "attention", "geglu", "groupnorm", "layernorm", "small_linear", "sinusoid",
+                 "conv_in", "conv_out", "upsample2x"):
         setattr(ops, name, globals()[name])
     with torch.device("meta"):
         unet = UNet2DConditionModel(UNetConfig.sdxl()).to(torch.bfloat16)
         net = None
         if with_lora:
             saved = list(plora.DEFAULT_TARGET_REPLACE)
-            plora.DEFAULT_TARGET_REPLACE += plora.UNET_TARGET_REPLACE_MODULE_CONV
+            plora.DEFAULT_TARGET_REPLACE += plora.UNET_TARGET_REPLACE_MODULE_CONV + list(extra_targets)
             net = plora.LoRANetwork(unet, rank=4, multiplier=1.0, alpha=1.0, train_method="noxattn")
             del plora.DEFAULT_TARGET_REPLACE[len(saved):]
         unet._ln_pack = lambda norm, leaves: (_meta(sum(l.weight.shape[0] for l in leaves), leaves[0].weight.shape[1]), None, None)
@@ -113,8 +125,8 @@ def trace(batch, with_lora=True):
         ehs = torch.empty(batch, 77, 2048, dtype=torch.bfloat16)
         added = {"text_embeds": torch.empty(batch, 1280, dtype=torch.bfloat16),
                  "time_ids": torch.empty(batch, 6, dtype=torch.float32)}
-        unet._forward_impl(x, t, ehs, added, torch.float32)
-    return calls
+        unet._walk(x, t, ehs, added, torch.float32, [] if train else None)
+    return list(calls)
 
 
 def main():
