@@ -97,6 +97,9 @@ int sb200_create(int device, void** handle) {
   Ctx* ctx = new Ctx();
   ctx->device = device;
   ctx->num_sms = prop.multiProcessorCount;
+  ctx->smem_per_sm = static_cast<int>(prop.sharedMemPerMultiprocessor);
+  ctx->smem_optin = static_cast<int>(prop.sharedMemPerBlockOptin);
+  ctx->smem_reserved = static_cast<int>(prop.reservedSharedMemPerBlock);
   ctx->encode = reinterpret_cast<EncodeTiledFn>(fn);
   *handle = ctx;
   return 0;

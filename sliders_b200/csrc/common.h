@@ -60,6 +60,9 @@ struct TmapKeyHash {
 struct Ctx {
   int device = 0;
   int num_sms = 0;
+  int smem_per_sm = 0;     // shared memory of one SM (bytes)
+  int smem_optin = 0;      // largest dynamic shared memory one CTA may opt in to
+  int smem_reserved = 0;   // shared memory the system reserves per resident CTA
   EncodeTiledFn encode = nullptr;
   std::mutex mu;
   std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> tmaps;

@@ -11,7 +11,11 @@
 // Epilogue: both warpgroups park their accumulators in shared memory as an fp32 [128 x (BN + rt)] tile (over the stage
 // ring, which is free once the main loop has ended).  Each thread then owns one row: rank-r LoRA up-projection,
 // LayerNorm fold, bias / time-embedding row bias / GEGLU / residual; residual tiles come in by cp.async and results
-// leave through a swizzled smem staging tile so that global accesses are coalesced.
+// leave through a swizzled smem staging tile (also in the ring, behind the accumulator tile) so that global accesses
+// are coalesced.
+// Residency: two CTAs per SM wherever 96 registers per thread hold the accumulators without spills (BN = 64, or no
+// LoRA), so one CTA's prologue and epilogue run while the other's wgmmas keep the tensor cores busy; BN = 128 with LoRA
+// needs ~160 registers and runs one CTA per SM.  Each CTA's ring is sized from its share of the SM's shared memory.
 // CTA pairs (kCtas = 2): a cluster of two CTAs on consecutive 128-row tiles of the same N tile.  Each CTA loads half
 // of the W (and LoRA-down) rows of a stage and multicasts them to both, which halves the weight traffic from L2.
 //
@@ -26,6 +30,8 @@
 // trainscripts/textsliders/train_util.py:242-247 together with the LoRA hook trainscripts/textsliders/lora.py:108-112.
 #include <stdlib.h>
 
+#include <algorithm>
+
 #include "common.h"
 #include "ptx.cuh"
 
@@ -38,18 +44,22 @@ constexpr int kEpiPerQuarter = kEpiWarps / 4;  // epilogue warps sharing one 32-
 constexpr int kProducerWarp = kEpiWarps;
 constexpr int kGemmThreads = 32 * (kEpiWarps + 1);
 constexpr int kMaxStages = 8;
-constexpr int kSmemBudget = 227 * 1024;
 constexpr int kBarRegion = 1024;
-constexpr int kLoraCols = 32;         // accumulator columns kept for t = A . down^T (rt <= 32)
+constexpr int kAlignSlack = 1024;     // the dynamic smem base is rounded up to 1024 B
 constexpr int kSlab = 32;             // output columns staged per epilogue-warp iteration
 constexpr int kEpiBufBytes = 32 * 64; // [32 rows x 32 cols] bf16
 constexpr int kEpiBytes = kEpiWarps * kEpiBufBytes;  // + kEpiWarps x [32 cols][r] fp32 of lora_up rows with LoRA
 constexpr int kConsumerBar = 5;       // named barrier of the 256 consumer threads (1..4: row-statistics reduction)
 
-// fp32 accumulator tile in shared memory: row stride BN + kLoraCols + 4 floats, so that the 32 rows a warp reads at
-// one column fall into distinct 16-byte bank groups
-__host__ __device__ constexpr int acc_stride(int bn) { return bn + kLoraCols + 4; }
-__host__ __device__ constexpr int acc_tile_bytes(int bn) { return kBM * acc_stride(bn) * 4; }
+// CTAs per SM an instantiation is compiled for (its launch bounds): under two, ptxas caps a thread at 96 registers,
+// which holds BN = 64 with LoRA and BN = 128 without it; BN = 128 with LoRA would spill and serialise its wgmmas
+__host__ __device__ constexpr int gemm_slots(int bn, int rt) { return (bn == 64 || rt == 0) ? 2 : 1; }
+
+// fp32 accumulator tile in shared memory: row stride BN + rt + 4 floats (an odd multiple of 16 bytes), so that the 32
+// rows a warp reads at one column fall into distinct 16-byte bank groups.  The 4 padding floats also absorb the
+// 8-float read of the last rank-4 adaptor's t columns.
+__host__ __device__ constexpr int acc_stride(int bn, int rt) { return bn + rt + 4; }
+__host__ __device__ constexpr int acc_tile_bytes(int bn, int rt) { return kBM * acc_stride(bn, rt) * 4; }
 
 struct GemmParams {
   CUtensorMap tmA[4];
@@ -64,7 +74,7 @@ struct GemmParams {
   int kblocks;      // K / 64 (conv: 9 * cb_total)
   int stages;
   int stage_bytes;  // bytes of one smem stage
-  int ring_bytes;   // stage ring, also holds the fp32 accumulator tile after the main loop
+  int ring_bytes;   // stage ring; after the main loop: fp32 accumulator tile, then the epilogue staging buffers
   int a_tx;         // bytes one A load deposits (box bytes; < 16 KB for conv patches smaller than 128 pixels)
   int b_rows;       // W rows one CTA loads per k-block (bn / kCtas)
   int l_rows;       // LoRA-down rows one CTA loads per k-block (rt / kCtas)
@@ -178,7 +188,7 @@ __device__ __forceinline__ void conv_origin(const GemmParams& p, int st, int& b0
 }
 
 template <int BN, int kCtas, int RT>
-__global__ void __launch_bounds__(kGemmThreads, 1) gemm_kernel(const __grid_constant__ GemmParams p) {
+__global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(const __grid_constant__ GemmParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -338,7 +348,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_kernel(const __grid_cons
 
     // ------------------------------------------------------------------ epilogue
     const uint32_t accs = tiles;  // fp32 accumulator tile, over the stage ring
-    constexpr int kStride = acc_stride(BN);
+    constexpr int kStride = acc_stride(BN, RT);
     asm volatile("bar.sync %0, %1;" ::"n"(kConsumerBar), "n"(32 * kEpiWarps) : "memory");  // both warpgroups done reading
     store_frag<BN>(acc, accs, wg * 64, 0, kStride);
     if constexpr (rt == 16)
@@ -367,9 +377,11 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_kernel(const __grid_cons
     const bool has_resid = (p.flags & SB200_EPI_RESID) != 0;
     // per-warp staging buffer ([32 rows x 32 cols] bf16, 64 B rows, 16-byte chunks XOR-swizzled by (row >> 1) & 3):
     // residual tiles arrive here by cp.async with coalesced global reads, results leave from here with coalesced global
-    // writes; in between every thread touches only its own row.
-    const uint32_t ebuf = tiles + static_cast<uint32_t>(p.ring_bytes) +
-                          static_cast<uint32_t>(warp) * (kEpiBufBytes + p.up_buf_bytes);
+    // writes; in between every thread touches only its own row.  The buffers sit in the ring behind the accumulator
+    // tile: every k-block's loads have landed (this CTA waited on each full barrier, whose byte count includes the
+    // peer's multicast) and both warpgroups have passed kConsumerBar, so nothing else writes or reads there.
+    const uint32_t epi = tiles + static_cast<uint32_t>(acc_tile_bytes(BN, RT));
+    const uint32_t ebuf = epi + static_cast<uint32_t>(warp) * (kEpiBufBytes + p.up_buf_bytes);
     const uint32_t ubuf = ebuf + kEpiBufBytes;  // p.up_buf_bytes of lora_up rows
     const uint32_t arow = accs + static_cast<uint32_t>((q * 32 + lane) * kStride) * 4u;
     // output row of this thread's accumulator row (q * 32 + lane), or -1 (padding row of the tile)
@@ -558,8 +570,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_kernel(const __grid_cons
       // The kEpiPerQuarter warps of a quarter hold partial sums of the SAME 32 rows (different slabs): combine them
       // through the quarter's first warp's staging buffer (free after its last copy-out), so that a row has one slot
       // per N tile.  Named barrier 1 + q, 32 * kEpiPerQuarter threads.
-      const uint32_t red = tiles + static_cast<uint32_t>(p.ring_bytes) +
-                           static_cast<uint32_t>(q) * (kEpiBufBytes + p.up_buf_bytes);
+      const uint32_t red = epi + static_cast<uint32_t>(q) * (kEpiBufBytes + p.up_buf_bytes);
       asm volatile("bar.sync %0, %1;" ::"r"(1 + q), "r"(32 * kEpiPerQuarter) : "memory");  // first warp done with its buffer
       if (hsel != 0)
         asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(red + ((hsel - 1) * 32 + lane) * 8), "f"(rs1), "f"(rs2)
@@ -610,20 +621,29 @@ static bool pairs_always() {
 static bool bn_supported(int bn) { return bn == 64 || bn == 128; }
 
 // Tile width from a cost model in SM cycles.  A 128 x bn tile's 64-deep k-block takes 4 bn cycles of tensor work (m64
-// wgmmas of two warpgroups at 4096 bf16 FLOP / clk / SM) plus the LoRA columns; a tile pays ~2000 cycles of prologue
-// and pipeline fill and an epilogue of ~14 cycles per output column (more with a residual / LoRA / GEGLU).  One CTA per
-// SM: work is dealt in waves of num_sms tiles.
+// wgmmas of two warpgroups at 4096 bf16 FLOP / clk / SM) plus the LoRA columns and ~208 cycles of per-k-block
+// overhead; a tile pays ~1500 cycles of prologue and pipeline fill and an epilogue of ~21 cycles per output column
+// (more with a residual / LoRA / GEGLU).  The busiest SM runs ceil(tiles / num_sms) tiles; their tensor work adds up,
+// but where two CTAs share the SM (gemm_slots) one's prologue and epilogue run under the other's wgmmas, so the fixed
+// cost is paid once per pair.  The constants are a least-squares fit (7 % rms) to the times of the B = 8 SDXL shapes
+// with BN forced (no CTA pairs, each instantiation at its own residency) on an H100 80GB HBM3 SXM at 400 W, in us
+// (BN 64 / 128): 8192 x 10240 x 1280 GEGLU 683 / 551,
+// 8192 x 1280 x 5120 + residual 293 / 245, 8192 x 3840 x 1280 LoRA 299 / 241, 32768 x 5120 x 640 GEGLU 833 / 625,
+// 32768 x 1920 x 640 LoRA 361 / 315, 32768 x 640 x 640 LoRA + residual 137 / 131, 616 x 153600 x 2048 1225 / 949,
+// LoRA convs 32x32 1280 -> 1280 850 / 620, 64x64 640 -> 640 831 / 630, 128x128 320 -> 320 881 / 832 (B = 8).
 static TileChoice pick_tile(int ncols, int num_sms, int kblocks, int lora_rt, int force_ctas, int sub_tiles, int flags) {
   double best = -1;
   TileChoice bc{1, 64};
   const int ctas = force_ctas ? force_ctas : (pairs_always() ? 2 : 1);
   const bool geglu = (flags & SB200_EPI_GEGLU) != 0;
-  const double epi_per_col = 14.0 + ((flags & SB200_EPI_RESID) ? 5.0 : 0.0) + (lora_rt ? 6.0 : 0.0) + (geglu ? 10.0 : 0.0);
+  const double epi_per_col = 21.0 + ((flags & SB200_EPI_RESID) ? 7.5 : 0.0) + (lora_rt ? 9.0 : 0.0) + (geglu ? 15.0 : 0.0);
   for (int bn = 64; bn <= 128; bn *= 2) {
     const long tiles = static_cast<long>(sub_tiles) * ((ncols + bn - 1) / bn);
-    const long waves = (tiles + num_sms - 1) / num_sms;
-    const double perkb = 4.0 * (bn + lora_rt) + 64.0;
-    const double cost = waves * (kblocks * perkb + 2000.0 + epi_per_col * (geglu ? bn / 2 : bn));
+    const long load = (tiles + num_sms - 1) / num_sms;
+    const int slots = gemm_slots(bn, lora_rt);
+    const double perkb = 4.0 * (bn + lora_rt) + 208.0;
+    const double cost = load * kblocks * perkb +
+                        ((load + slots - 1) / slots) * (1500.0 + epi_per_col * (geglu ? bn / 2 : bn));
     if (best < 0 || cost < best - 1e-9 || (cost < best + 1e-9 && bn > bc.bn)) {
       best = cost;
       bc = TileChoice{ctas, bn};
@@ -640,12 +660,26 @@ static bool n_fast_default() {
   return v;
 }
 
+// Dynamic shared memory one CTA may use when `slots` CTAs are to share an SM.
+static int smem_budget(const Ctx* ctx, int slots) {
+  return std::min(ctx->smem_optin, ctx->smem_per_sm / slots - ctx->smem_reserved);
+}
+
 template <int BN, int kCtas, int RT>
 static int launch_gemm_bn(Ctx* ctx, cudaStream_t stream, const GemmParams& p, int smem) {
   static bool attr_set = false;  // one flag per instantiation
   if (!attr_set) {
+    const auto kernel = gemm_kernel<BN, kCtas, RT>;
+    constexpr int slots = gemm_slots(BN, RT);
+    SB200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin));
     SB200_CUDA_CHECK(
-        cudaFuncSetAttribute(gemm_kernel<BN, kCtas, RT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
+        cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    int resident = 0;
+    SB200_CUDA_CHECK(
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kernel, kGemmThreads, smem_budget(ctx, slots)));
+    if (resident < slots)
+      return set_error(SB200_ERR_CUDA, "gemm_kernel<%d, %d, %d>: %d CTA(s) per SM fit, built for %d", BN, kCtas, RT,
+                       resident, slots);
     attr_set = true;
   }
   const int total = p.num_m_tiles * p.num_n_tiles;
@@ -682,17 +716,18 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
   p.l_rows = has_lora ? p.lora_rt / ctas : 0;
   p.stage_bytes = kBM * 128 + p.bn * 128 + (has_lora ? p.lora_rt * 128 : 0);
   p.up_buf_bytes = has_lora ? kSlab * p.lora_r * 4 : 0;
-  const int epi_bytes = kEpiBytes + kEpiWarps * p.up_buf_bytes;
-  int stages = (kSmemBudget - kBarRegion - 1024 - epi_bytes) / p.stage_bytes;
+  const int rt = has_lora ? p.lora_rt : 0;
+  const int grid_ctas = p.num_m_tiles * p.num_n_tiles * ctas * (p.sk_ws ? p.sk_splits : 1);
+  // A grid that gives each SM at most one CTA lets that CTA have the whole SM's shared memory (a deeper ring).
+  const int budget = smem_budget(ctx, grid_ctas > ctx->num_sms ? gemm_slots(p.bn, rt) : 1);
+  int stages = (budget - kBarRegion - kAlignSlack) / p.stage_bytes;
   if (stages > kMaxStages) stages = kMaxStages;
   if (stages < 2) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
   p.stages = stages;
-  p.ring_bytes = stages * p.stage_bytes;
-  if (p.ring_bytes < acc_tile_bytes(p.bn)) p.ring_bytes = acc_tile_bytes(p.bn);
-  const int smem = kBarRegion + 1024 + p.ring_bytes + epi_bytes;
-  if (smem > kSmemBudget) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
-  pdl_hint() = p.num_m_tiles * p.num_n_tiles * ctas * (p.sk_ws ? p.sk_splits : 1) <= 2 * ctx->num_sms;
-  const int rt = has_lora ? p.lora_rt : 0;
+  p.ring_bytes = std::max(stages * p.stage_bytes, acc_tile_bytes(p.bn, rt) + kEpiBytes + kEpiWarps * p.up_buf_bytes);
+  const int smem = kBarRegion + kAlignSlack + p.ring_bytes;
+  if (smem > budget) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
+  pdl_hint() = grid_ctas <= 2 * ctx->num_sms;
   const int variant = (ctas == 2 ? 6 : 0) + (p.bn == 128 ? 3 : 0) + (rt == 16 ? 1 : (rt == 32 ? 2 : 0));
   cudaStream_t s = stream;
   int st;
