@@ -173,8 +173,11 @@ def gemm(x: torch.Tensor, w: torch.Tensor, *, bias=None, rowbias=None, rows_per_
 
 
 def conv3x3(x0: torch.Tensor, w_packed: torch.Tensor, *, x1: Optional[torch.Tensor] = None, stride: int = 1,
-            bias=None, rowbias=None, resid=None, lora: Optional[Lora] = None, bn: int = 0) -> torch.Tensor:
-    """3x3 / pad 1 conv on NHWC bf16 ([B,H,W,C] tensors); w_packed is [Cout,3,3,Cin].  One `gemm_kernel`."""
+            bias=None, rowbias=None, resid=None, lora: Optional[Lora] = None, out: Optional[torch.Tensor] = None,
+            bn: int = 0) -> torch.Tensor:
+    """3x3 / pad 1 conv on NHWC bf16 ([B,H,W,C] tensors); w_packed is [Cout,3,3,Cin].  One `gemm_kernel`.
+    `out`: [B, Ho, Wo, Cout] whose pixels are rows of one 2-D matrix with row stride out.stride(2) (e.g. a column
+    slice of a wider NHWC buffer)."""
     B, H, W, C0 = x0.shape
     C1 = x1.shape[-1] if x1 is not None else 0
     Cout = w_packed.shape[0]
@@ -187,11 +190,17 @@ def conv3x3(x0: torch.Tensor, w_packed: torch.Tensor, *, x1: Optional[torch.Tens
         flags |= EPI_RESID
     if lora is not None:
         flags |= EPI_LORA
-    out = torch.empty((B, H // stride, W // stride, Cout), device=x0.device, dtype=BF16)
+    Ho, Wo = H // stride, W // stride
+    if out is None:
+        out = torch.empty((B, Ho, Wo, Cout), device=x0.device, dtype=BF16)
+    elif (tuple(out.shape) != (B, Ho, Wo, Cout) or out.stride(3) != 1 or out.stride(1) != Wo * out.stride(2)
+          or out.stride(0) != Ho * out.stride(1)):
+        raise ValueError(f"conv3x3: out {tuple(out.shape)} / strides {out.stride()} is not a [B*Ho*Wo, ldo] matrix "
+                         f"of [{B}, {Ho}, {Wo}, {Cout}]")
     lib = _begin()
     _cabi.check(lib.sb200_conv3x3(
         _ctx(x0), _stream(), _p(x0), x0.stride(2), _p(x1), x1.stride(2) if x1 is not None else 0, C0, C1,
-        _p(w_packed), _p(out), Cout, B, H, W, Cout, stride, flags, _p(bias), _p(rowbias), _p(resid),
+        _p(w_packed), _p(out), out.stride(2), B, H, W, Cout, stride, flags, _p(bias), _p(rowbias), _p(resid),
         resid.stride(2) if resid is not None else 0, lora.ref() if lora is not None else None, bn))
     _count("conv3x3", 2.0 * B * (H // stride) * (W // stride) * Cout * 9 * (C0 + C1))
     return out
