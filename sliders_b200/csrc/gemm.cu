@@ -187,6 +187,45 @@ __device__ __forceinline__ void conv_origin(const GemmParams& p, int st, int& b0
   b0 = (r / p.tiles_h) * p.bb;
 }
 
+// Where the A operand of 128-row sub-tile st starts: its first row (plain) or its first output pixel (conv)
+struct AOrigin {
+  int m0, b0, h0, w0;
+};
+__device__ __forceinline__ AOrigin a_origin(const GemmParams& p, int st) {
+  AOrigin o{st * kBM, 0, 0, 0};
+  if (p.a_mode != 0) {
+    if (st < p.num_sub)
+      conv_origin(p, st, o.b0, o.h0, o.w0);
+    else
+      o.b0 = p.B;  // phantom sub-tile of an odd pair: every box is out of bounds -> zero fill
+  }
+  return o;
+}
+
+// TMA load of k-block kb of the A tile at `o` into sA (128 rows x 64 k, or the conv patch), completing on `bar`
+__device__ __forceinline__ void load_a(const GemmParams& p, const AOrigin& o, int kb, uint32_t sA, uint32_t bar) {
+  const int a_mode = p.a_mode, kb_split = p.kb_split, cb_total = p.cb_total;
+  if (a_mode == 0) {
+    const int src = kb < kb_split ? 0 : 1;
+    tma_load_2d(sA, &p.tmA[src], bar, (src ? kb - kb_split : kb) * kBK, o.m0);
+  } else {
+    const int tap = kb / cb_total;  // filter tap and channel block of this k-block
+    const int cb = kb - tap * cb_total;
+    const int kh = tap / 3;
+    const int kw = tap - kh * 3;
+    if (a_mode == 1) {
+      const int src = cb < kb_split ? 0 : 1;
+      tma_load_4d(sA, &p.tmA[src], bar, (src ? cb - kb_split : cb) * kBK, o.w0 + kw - 1, o.h0 + kh - 1, o.b0);
+    } else {
+      // input row 2*ho + kh - 1: kh=0 -> odd plane, row ho-1; kh=1 -> even plane, row ho; kh=2 -> odd plane, row ho
+      const int ph = (kh == 1) ? 0 : 1;
+      const int pwl = (kw == 1) ? 0 : 1;
+      tma_load_4d(sA, &p.tmA[ph * 2 + pwl], bar, cb * kBK, o.w0 + ((kw == 0) ? -1 : 0), o.h0 + ((kh == 0) ? -1 : 0),
+                  o.b0);
+    }
+  }
+}
+
 template <int BN, int kCtas, int RT>
 __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(const __grid_constant__ GemmParams p) {
   pdl_trigger();
@@ -237,16 +276,8 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
 
   if (warp == kProducerWarp) {
     // ------------------------------------------------------------------ TMA producer, converged warp
-    const int a_mode = p.a_mode, kb_split = p.kb_split, cb_total = p.cb_total;
     const uint32_t tx = static_cast<uint32_t>(p.a_tx) + b_bytes + static_cast<uint32_t>(rt) * 128u;
-    const int m0 = st * kBM;
-    int b0 = 0, h0 = 0, w0 = 0;
-    if (a_mode != 0) {
-      if (st < p.num_sub)
-        conv_origin(p, st, b0, h0, w0);
-      else
-        b0 = p.B;  // phantom sub-tile of an odd pair: every box is out of bounds -> zero fill
-    }
+    const AOrigin ao = a_origin(p, st);
     // W rows this CTA loads (a pair: half each, multicast to both)
     int brow;
     if (geglu) {
@@ -264,25 +295,7 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
         mbar_expect_tx(full_bar, tx);
         const uint32_t sA = tiles + static_cast<uint32_t>(stage) * stage_bytes;
         const uint32_t sB = sA + a_bytes;
-        if (a_mode == 0) {
-          const int src = kb < kb_split ? 0 : 1;
-          tma_load_2d(sA, &p.tmA[src], full_bar, (src ? kb - kb_split : kb) * kBK, m0);
-        } else {
-          const int tap = kb / cb_total;  // filter tap and channel block of this k-block
-          const int cb = kb - tap * cb_total;
-          const int kh = tap / 3;
-          const int kw = tap - kh * 3;
-          if (a_mode == 1) {
-            const int src = cb < kb_split ? 0 : 1;
-            tma_load_4d(sA, &p.tmA[src], full_bar, (src ? cb - kb_split : cb) * kBK, w0 + kw - 1, h0 + kh - 1, b0);
-          } else {
-            // input row 2*ho + kh - 1: kh=0 -> odd plane, row ho-1; kh=1 -> even plane, row ho; kh=2 -> odd plane, row ho
-            const int ph = (kh == 1) ? 0 : 1;
-            const int pwl = (kw == 1) ? 0 : 1;
-            tma_load_4d(sA, &p.tmA[ph * 2 + pwl], full_bar, cb * kBK, w0 + ((kw == 0) ? -1 : 0),
-                        h0 + ((kh == 0) ? -1 : 0), b0);
-          }
-        }
+        load_a(p, ao, kb, sA, full_bar);
         if constexpr (kCtas == 2) {
           const uint32_t boff = cta_rank * static_cast<uint32_t>(p.b_rows) * 128u;
           tma_load_2d_mc(sB + boff, &p.tmB, full_bar, kb * kBK, brow, 3);
@@ -596,6 +609,327 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
 }
 
 // -------------------------------------------------------------------------------------------------
+// Wide tiles: a persistent kernel for layers whose W has a multiple of 256 rows
+// -------------------------------------------------------------------------------------------------
+// gemm_wide_kernel<RT>: 128 x 256 tiles (GEGLU: 256 W rows, 128 output columns), 384 threads, one CTA per SM, each CTA
+// walking the tiles blockIdx.x, blockIdx.x + gridDim.x, ... in launch_gemm's order:
+//   warpgroup 2    producer: gives its registers to the consumers (setmaxnreg 40); one elected thread of warp 8 issues
+//                  the TMA loads, running ahead into the next tile while the consumers finish the current epilogue
+//   warpgroups 0/1 consumers (setmaxnreg 232): rows 0..63 / 64..127, an m64 x 256 accumulator of 128 registers
+// The k-loop, its barrier protocol and the LoRA-down rows behind the W rows are those of gemm_kernel; the ring's phases
+// run on across tiles.  The epilogue works on the accumulator registers: per element it applies, in gemm_kernel's
+// order and with its expressions, the LoRA update, bias, row bias and GEGLU, rounds to bf16, adds the residual in bf16,
+// and leaves through a swizzled staging buffer (two per warpgroup, 64 rows x 64 columns each) with coalesced stores.
+// Only t = A.down^T and the tile's lora_up rows are staged in shared memory.  No LayerNorm fold, row statistics,
+// split-K or CTA pairs: those stay on gemm_kernel.
+constexpr int kWideBN = 256;
+constexpr int kWideThreads = 384;
+constexpr int kWideChunk = 64;                        // output columns per staging buffer
+constexpr int kWideStgBytes = 64 * kWideChunk * 2;    // [64 rows x 64 cols] bf16, 128 B rows
+constexpr int kWideBarBase = 1;                       // named barriers 1, 2: one per consumer warpgroup
+
+// Shared memory of one consumer warpgroup's epilogue: two staging buffers, then with LoRA its 64 rows of t
+// (row stride rt + 4 floats) and the tile's 256 lora_up rows.
+__host__ __device__ constexpr int wide_t_bytes(int rt) { return rt ? 64 * (rt + 4) * 4 : 0; }
+__host__ __device__ constexpr int wide_epi_bytes(int rt, int r) {
+  return 2 * kWideStgBytes + wide_t_bytes(rt) + (rt ? kWideBN * r * 4 : 0);
+}
+
+// Output row of row r of 128-row sub-tile st (the conv patch mapping of conv_origin), or -1 for a padding row
+__device__ __forceinline__ int tile_out_row(const GemmParams& p, int st, int r) {
+  if (p.a_mode == 0) {
+    const int m = st * kBM + r;
+    return m < p.M ? m : -1;
+  }
+  int b0, h0, w0;
+  conv_origin(p, st, b0, h0, w0);
+  const int iw = r % p.bw;
+  const int t2 = r / p.bw;
+  const int ih = t2 % p.bh;
+  const int ib = t2 / p.bh;
+  const int b = b0 + ib, h = h0 + ih, w = w0 + iw;
+  return (ib < p.bb && b < p.B && h < p.H && w < p.W) ? (b * p.H + h) * p.W + w : -1;
+}
+
+template <int RT>
+__global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid_constant__ GemmParams p) {
+  pdl_trigger();
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024 B alignment
+  const int warp = threadIdx.x >> 5;
+  const int S = p.stages;
+  const uint32_t bar_full = base;            // S barriers
+  const uint32_t bar_empty = base + 8u * S;  // S barriers
+  const uint32_t tiles = base + kBarRegion;
+  const uint32_t stage_bytes = static_cast<uint32_t>(p.stage_bytes);
+  constexpr uint32_t a_bytes = kBM * 128;
+  constexpr uint32_t b_bytes = kWideBN * 128;
+  const bool geglu = (p.flags & SB200_EPI_GEGLU) != 0;
+  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&p.tmA[0]);
+    tma_prefetch_desc(&p.tmB);
+    if (RT) tma_prefetch_desc(&p.tmL);
+  }
+  if (threadIdx.x == 32) {
+    for (int i = 0; i < S; ++i) {
+      mbar_init(bar_full + 8u * i, 1);
+      mbar_init(bar_empty + 8u * i, 2);  // one arrival per consumer warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();  // everything above overlapped the previous kernel's tail; global memory is touched only below
+
+  if (warp >= 8) {
+    // ------------------------------------------------------------------ TMA producer
+    setmaxnreg_dec<40>();
+    if (warp != 8) return;
+    const uint32_t tx = static_cast<uint32_t>(p.a_tx) + b_bytes + static_cast<uint32_t>(RT) * 128u;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+      const int mt = p.n_fast ? t / p.num_n_tiles : t % p.num_m_tiles;
+      const int nt = p.n_fast ? t % p.num_n_tiles : t / p.num_m_tiles;
+      const AOrigin ao = a_origin(p, mt);
+      // GEGLU: the tile's 128 value rows of W, then the 128 matching gate rows
+      const int brow = geglu ? nt * (kWideBN / 2) : nt * kWideBN;
+      for (int kb = 0; kb < p.kblocks; ++kb) {
+        const uint32_t full_bar = bar_full + 8u * stage, empty_bar = bar_empty + 8u * stage;
+        mbar_wait(empty_bar, phase ^ 1u);
+        if (elect_one()) {
+          mbar_expect_tx(full_bar, tx);
+          const uint32_t sA = tiles + static_cast<uint32_t>(stage) * stage_bytes;
+          const uint32_t sB = sA + a_bytes;
+          load_a(p, ao, kb, sA, full_bar);
+          tma_load_2d(sB, &p.tmB, full_bar, kb * kBK, brow);
+          if (geglu) tma_load_2d(sB + (b_bytes >> 1), &p.tmB, full_bar, kb * kBK, (p.N >> 1) + brow);
+          if (RT) tma_load_2d(sB + b_bytes, &p.tmL, full_bar, kb * kBK, 0);
+        }
+        __syncwarp();
+        if (++stage == S) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      }
+    }
+    return;
+  }
+
+  // ------------------------------------------------------------------ consumers
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2;
+  const int tid = threadIdx.x & 127;
+  const int lane = threadIdx.x & 31;
+  const int q = lane & 3;
+  const int fr0 = (warp & 3) * 16 + (lane >> 2);  // accumulator rows of this thread: fr0 and fr0 + 8 (of 64)
+  const bool signal = tid == 0;
+  const bool has_lora = RT != 0;
+  const bool has_resid = (p.flags & SB200_EPI_RESID) != 0;
+  const bool has_bias = (p.flags & SB200_EPI_BIAS) != 0;
+  const bool has_rb = (p.flags & SB200_EPI_ROWBIAS) != 0;
+  const int r = has_lora ? p.lora_r : 0;
+  const float lscale = has_lora ? (p.lora_scale_dev ? p.lora_scale * __ldg(p.lora_scale_dev) : p.lora_scale) : 0.f;
+  const int nchunks = p.ncols_out / kWideChunk;  // 4, or 2 with GEGLU
+  const uint32_t epi = tiles + static_cast<uint32_t>(S) * stage_bytes +
+                       static_cast<uint32_t>(wg) * static_cast<uint32_t>(wide_epi_bytes(RT, r));
+  const uint32_t tbuf = epi + 2 * kWideStgBytes;  // [64][RT + 4] fp32: t of this warpgroup's rows
+  const uint32_t ubuf = tbuf + wide_t_bytes(RT);  // [256][r] fp32: the tile's lora_up rows
+  constexpr int kTStride = RT + 4;
+  // rows / 16-byte chunk this thread moves between a staging buffer and global memory: rows crow + 16 i, chunk cch
+  const int crow = tid >> 3, cch = tid & 7;
+  const uint32_t bar_id = kWideBarBase + wg;
+  auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); };
+
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+    const int mt = p.n_fast ? t / p.num_n_tiles : t % p.num_m_tiles;
+    const int nt = p.n_fast ? t % p.num_n_tiles : t / p.num_m_tiles;
+    float acc[kWideBN / 2];
+    float accl[RT ? RT / 2 : 1];
+#pragma unroll
+    for (int i = 0; i < kWideBN / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (RT ? RT / 2 : 1); ++i) accl[i] = 0.f;
+    int prev = 0;
+    for (int kb = 0; kb < p.kblocks; ++kb) {
+      mbar_wait(bar_full + 8u * stage, phase);
+      const uint32_t sA = tiles + static_cast<uint32_t>(stage) * stage_bytes + static_cast<uint32_t>(wg) * 64u * 128u;
+      const uint32_t sB = tiles + static_cast<uint32_t>(stage) * stage_bytes + a_bytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBK / 16; ++k) {
+        const uint64_t adesc = gmma_desc_sw128(sA + 32u * k);
+        wgmma_ss_n256(acc, adesc, gmma_desc_sw128(sB + 32u * k), 1u);
+        if constexpr (RT == 16)
+          wgmma_ss_n16(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
+        else if constexpr (RT == 32)
+          wgmma_ss_n32(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block's products have read their stage: hand it back to the producer
+      if (kb > 0 && signal) mbar_arrive(bar_empty + 8u * prev);
+      prev = stage;
+      if (++stage == S) {
+        stage = 0;
+        phase ^= 1u;
+      }
+    }
+    wgmma_wait<0>();
+    if (signal) mbar_arrive(bar_empty + 8u * prev);  // the last stage of the tile, for the producer's next tile
+#pragma unroll
+    for (int i = 0; i < kWideBN / 2; ++i) reg_fence(acc[i]);
+#pragma unroll
+    for (int i = 0; i < (RT ? RT / 2 : 1); ++i) reg_fence(accl[i]);
+
+    // ------------------------------------------------------------------ epilogue
+    const int st = mt;
+    const int n_base = nt * p.ncols_out;
+    int orow[4];  // output rows this thread copies
+#pragma unroll
+    for (int i = 0; i < 4; ++i) orow[i] = tile_out_row(p, st, wg * 64 + crow + 16 * i);
+    auto prefetch_resid = [&](int c, uint32_t buf) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int row = crow + 16 * i;
+        if (orow[i] >= 0)
+          cp_async_16(buf + row * 128 + ((cch ^ (row & 7)) << 4),
+                      p.resid + static_cast<size_t>(orow[i]) * p.ldr + n_base + c * kWideChunk + cch * 8);
+      }
+      cp_async_commit();
+    };
+    wg_sync();  // every thread of the warpgroup is done with the previous tile's staging, t and lora_up buffers
+    if constexpr (RT != 0) {
+      // t = A.down^T of this warpgroup's rows (fragment layout as in wgmma.cuh), and the tile's lora_up rows
+#pragma unroll
+      for (int i = 0; i < RT / 2; i += 2) {
+        const int row = fr0 + 8 * ((i >> 1) & 1);
+        const int col = 8 * (i >> 2) + 2 * q;
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(tbuf + (row * kTStride + col) * 4), "f"(accl[i]),
+                     "f"(accl[i + 1])
+                     : "memory");
+      }
+      const float* up_src = p.lora_up + static_cast<size_t>(n_base) * r;
+      for (int i = tid; i < kWideBN * r / 4; i += 128) cp_async_16(ubuf + i * 16, up_src + i * 4);
+      cp_async_commit();
+    }
+    if (has_resid) prefetch_resid(0, epi);
+    if (has_resid || has_lora) {
+      cp_async_wait<0>();
+      wg_sync();
+    }
+    const __nv_bfloat16* rb[2] = {nullptr, nullptr};
+    if (has_rb) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int orw = tile_out_row(p, st, wg * 64 + fr0 + 8 * h);
+        rb[h] = p.rowbias + static_cast<size_t>(orw >= 0 ? orw / p.rows_per_batch : 0) * p.Nout;
+      }
+    }
+    float tl[2][8];  // lscale * t of the current adaptor, rows fr0 and fr0 + 8
+    int cur_grp = -1;
+    // A runtime loop over the chunks keeps one copy of the epilogue code (unrolled four times it outgrows the
+    // instruction cache); each pass first selects its chunk's 32 accumulator registers (and 32 gate registers).
+#pragma unroll 1
+    for (int c = 0; c < nchunks; ++c) {
+      {
+        constexpr int kChunkRegs = kWideChunk / 2;  // accumulator registers per thread and chunk
+        float v[kChunkRegs], gv[kChunkRegs];
+#pragma unroll
+        for (int k = 0; k < kChunkRegs; ++k) {
+          v[k] = c == 0 ? acc[k] : c == 1 ? acc[kChunkRegs + k] : c == 2 ? acc[2 * kChunkRegs + k] : acc[3 * kChunkRegs + k];
+          gv[k] = c == 0 ? acc[2 * kChunkRegs + k] : acc[3 * kChunkRegs + k];  // GEGLU: column + 128, the gate half
+        }
+        const uint32_t buf = epi + static_cast<uint32_t>(c & 1) * kWideStgBytes;
+        uint32_t o[8][2];
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j = c * 8 + jj;  // 8-column block of the accumulator
+          const int n = n_base + 8 * j + 2 * q;
+          float up[2][8];
+          if constexpr (RT != 0) {
+            const int grp = n / p.lora_group_n;
+            if (grp != cur_grp) {
+              cur_grp = grp;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const uint32_t ta = tbuf + ((fr0 + 8 * h) * kTStride + grp * r) * 4;
+                const uint4 a = ld_shared_v4(ta);
+                const uint4 b = r == 8 ? ld_shared_v4(ta + 16) : make_uint4(0, 0, 0, 0);
+                const uint32_t tv[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+                for (int jt = 0; jt < 8; ++jt) tl[h][jt] = __uint_as_float(tv[jt]) * lscale;
+              }
+            }
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const uint32_t ua = ubuf + (8 * j + 2 * q + e) * r * 4;
+              const uint4 a = ld_shared_v4(ua);
+              const uint4 b = r == 8 ? ld_shared_v4(ua + 16) : make_uint4(0, 0, 0, 0);
+              const uint32_t uv[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+              for (int ju = 0; ju < 8; ++ju) up[e][ju] = __uint_as_float(uv[ju]);
+            }
+          }
+          const uint32_t bw = has_bias ? __ldg(reinterpret_cast<const uint32_t*>(p.bias + n)) : 0u;
+          const uint32_t gbw = (has_bias && geglu) ? __ldg(reinterpret_cast<const uint32_t*>(p.bias + p.Nout + n)) : 0u;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t rbw = has_rb ? __ldg(reinterpret_cast<const uint32_t*>(rb[h] + n)) : 0u;
+            float f[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int i = 4 * jj + 2 * h + e;
+              f[e] = v[i];
+              if constexpr (RT != 0) {
+                // gemm_kernel's lora_apply, term for term
+                f[e] += tl[h][0] * up[e][0] + tl[h][1] * up[e][1] + tl[h][2] * up[e][2] + tl[h][3] * up[e][3];
+                if (r == 8)
+                  f[e] += tl[h][4] * up[e][4] + tl[h][5] * up[e][5] + tl[h][6] * up[e][6] + tl[h][7] * up[e][7];
+              }
+              if (has_bias) f[e] += e ? bf16_hi(bw) : bf16_lo(bw);
+              if (has_rb) f[e] += e ? bf16_hi(rbw) : bf16_lo(rbw);
+              if (geglu) {
+                float gb = gv[i];
+                if (has_bias) gb += e ? bf16_hi(gbw) : bf16_lo(gbw);
+                f[e] *= gelu_erf_f(gb);
+              }
+            }
+            o[jj][h] = pack_bf16x2(f[0], f[1]);
+          }
+        }
+        if (has_resid && c > 0) {
+          cp_async_wait<0>();
+          wg_sync();  // chunk c's residual has landed; chunk c - 1's copy-out from the other buffer is done
+        }
+        if (has_resid && c + 1 < nchunks) prefetch_resid(c + 1, epi + static_cast<uint32_t>((c + 1) & 1) * kWideStgBytes);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = fr0 + 8 * h;
+            const uint32_t a = buf + row * 128 + ((jj ^ (row & 7)) << 4) + q * 4;
+            // the residual is added to the ROUNDED projection, in bf16, as in gemm_kernel
+            st_shared_u32(a, has_resid ? add_bf16x2(o[jj][h], ld_shared_u32(a)) : o[jj][h]);
+          }
+        }
+        wg_sync();
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int row = crow + 16 * i;
+          const uint4 v = ld_shared_v4(buf + row * 128 + ((cch ^ (row & 7)) << 4));
+          if (orow[i] >= 0)
+            *reinterpret_cast<uint4*>(p.out + static_cast<size_t>(orow[i]) * p.ldo + n_base + c * kWideChunk +
+                                      cch * 8) = v;
+        }
+      }
+    }
+  }
+}
+
+// -------------------------------------------------------------------------------------------------
 // host side
 // -------------------------------------------------------------------------------------------------
 struct TileChoice {
@@ -617,8 +951,15 @@ static bool pairs_always() {
   return v;
 }
 
-// Tile widths the kernel is instantiated for (a 256-wide accumulator does not fit the registers of 288 threads).
-static bool bn_supported(int bn) { return bn == 64 || bn == 128; }
+// Tile widths: 64 and 128 run gemm_kernel, 256 runs gemm_wide_kernel (a 256-wide accumulator needs the registers a
+// producer warpgroup gives up, which 288 threads do not have).
+static bool bn_supported(int bn) { return bn == 64 || bn == 128 || bn == kWideBN; }
+
+// gemm_wide_kernel takes W with a multiple of 256 rows (with GEGLU: 128 rows per half, so a tile writes 128 output
+// columns), single CTAs, and none of LayerNorm fold and row statistics.
+static bool wide_eligible(int N, int ctas, bool lnfold, bool rowstats) {
+  return N % kWideBN == 0 && ctas == 1 && !lnfold && !rowstats;
+}
 
 // Tile width from a cost model in SM cycles.  A 128 x bn tile's 64-deep k-block takes 4 bn cycles of tensor work (m64
 // wgmmas of two warpgroups at 4096 bf16 FLOP / clk / SM) plus the LoRA columns and ~208 cycles of per-k-block
@@ -631,19 +972,43 @@ static bool bn_supported(int bn) { return bn == 64 || bn == 128; }
 // 8192 x 1280 x 5120 + residual 293 / 245, 8192 x 3840 x 1280 LoRA 299 / 241, 32768 x 5120 x 640 GEGLU 833 / 625,
 // 32768 x 1920 x 640 LoRA 361 / 315, 32768 x 640 x 640 LoRA + residual 137 / 131, 616 x 153600 x 2048 1225 / 949,
 // LoRA convs 32x32 1280 -> 1280 850 / 620, 64x64 640 -> 640 831 / 630, 128x128 320 -> 320 881 / 832 (B = 8).
-static TileChoice pick_tile(int ncols, int num_sms, int kblocks, int lora_rt, int force_ctas, int sub_tiles, int flags) {
+// gemm_wide_kernel in the same units: 4 (256 + rt) + kWidePerKb cycles per k-block, kWideTile per tile (epilogue and
+// pipeline refill; the wide epilogue does not overlap the tensor cores), kWideLoraTile more per tile with LoRA, and
+// the fixed cost once per CTA.  Fitted to the same shapes timed with each width forced on an H100 80GB HBM3 SXM at
+// 700 W (us, BN 64 / 128 / 256): 8192 x 10240 x 1280 GEGLU 616 / 459 / 429, 8192 x 1280 x 5120 + residual
+// 268 / 215 / 179, 32768 x 5120 x 640 GEGLU 812 / 557 / 552, 616 x 153600 x 2048 1099 / 749 / 653,
+// 8192 x 1280 x 1280 bias 70 / 64 / 65, 8192 x 3840 x 1280 LoRA 240 / 209 / 245, 8192 x 1280 x 1280 LoRA + residual
+// 93 / 85 / 101, LoRA convs 32x32 1280 -> 1280 676 / 462 / 480, 2560 -> 1280 1502 / 933 / 1175 (B = 8); SD-1.5 at
+// B = 1 (CFG pair): 512 x 1280 x 1280 + residual 9.8 / 13.7 / 22.2, 512 x 3840 x 1280 LoRA 19.7 / 15.3 / 32.0,
+// 512 x 10240 x 1280 GEGLU 47.3 / 44.1 / 43.2, 2048 x 5120 x 640 GEGLU 54.4 / 42.7 / 45.1, convs 16x16 and 8x8
+// 1280 -> 1280 + residual 72 / 84 / 117 and 71 / 84 / 116.  The wide tile wins on the GEGLU, deep-K and many-tile
+// shapes and loses with LoRA and on grids of few tiles; the fit reproduces every choice but the 512 x 10240 GEGLU tie.
+constexpr double kWidePerKb = 136.0;
+constexpr double kWideTile = 6500.0;
+constexpr double kWideLoraTile = 40000.0;
+constexpr double kWideFixed = 1500.0;
+static TileChoice pick_tile(int ncols, int num_sms, int kblocks, int lora_rt, int force_ctas, int sub_tiles, int flags,
+                            bool lnfold, bool rowstats) {
   double best = -1;
   TileChoice bc{1, 64};
   const int ctas = force_ctas ? force_ctas : (pairs_always() ? 2 : 1);
   const bool geglu = (flags & SB200_EPI_GEGLU) != 0;
   const double epi_per_col = 21.0 + ((flags & SB200_EPI_RESID) ? 7.5 : 0.0) + (lora_rt ? 9.0 : 0.0) + (geglu ? 15.0 : 0.0);
-  for (int bn = 64; bn <= 128; bn *= 2) {
+  const int max_bn = wide_eligible(ncols, ctas, lnfold, rowstats) ? kWideBN : 128;
+  for (int bn = 64; bn <= max_bn; bn *= 2) {
     const long tiles = static_cast<long>(sub_tiles) * ((ncols + bn - 1) / bn);
     const long load = (tiles + num_sms - 1) / num_sms;
-    const int slots = gemm_slots(bn, lora_rt);
-    const double perkb = 4.0 * (bn + lora_rt) + 208.0;
-    const double cost = load * kblocks * perkb +
-                        ((load + slots - 1) / slots) * (1500.0 + epi_per_col * (geglu ? bn / 2 : bn));
+    const int cols_out = geglu ? bn / 2 : bn;
+    double cost;
+    if (bn == kWideBN) {
+      // persistent, one CTA per SM: the fixed cost once per CTA
+      cost = load * (kblocks * (4.0 * (bn + lora_rt) + kWidePerKb) + kWideTile + (lora_rt ? kWideLoraTile : 0.0)) +
+             kWideFixed;
+    } else {
+      const int slots = gemm_slots(bn, lora_rt);
+      const double perkb = 4.0 * (bn + lora_rt) + 208.0;
+      cost = load * kblocks * perkb + ((load + slots - 1) / slots) * (1500.0 + epi_per_col * cols_out);
+    }
     if (best < 0 || cost < best - 1e-9 || (cost < best + 1e-9 && bn > bc.bn)) {
       best = cost;
       bc = TileChoice{ctas, bn};
@@ -702,6 +1067,33 @@ static int launch_gemm_bn(Ctx* ctx, cudaStream_t stream, const GemmParams& p, in
   return 0;
 }
 
+template <int RT>
+static int launch_gemm_wide(Ctx* ctx, cudaStream_t stream, const GemmParams& p, int smem) {
+  static bool attr_set = false;  // one flag per instantiation
+  const auto kernel = gemm_wide_kernel<RT>;
+  if (!attr_set) {
+    SB200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin));
+    SB200_CUDA_CHECK(
+        cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    int resident = 0;
+    SB200_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kernel, kWideThreads, smem));
+    if (resident < 1) return set_error(SB200_ERR_CUDA, "gemm_wide_kernel<%d>: no CTA fits an SM", RT);
+    attr_set = true;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(std::min(p.num_m_tiles * p.num_n_tiles, ctx->num_sms));
+  cfg.blockDim = dim3(kWideThreads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = (pdl_mode() == 2 || (pdl_mode() == 1 && pdl_hint())) ? 1 : 0;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  SB200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, p));
+  return 0;
+}
+
 static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
   // Tile order: N fastest reads each A row-tile from DRAM once and re-reads W once per row-tile, which is free while W
   // stays in L2.  When W is the big operand and does not fit (the batched cross-attention K/V projection: 616 x 2048
@@ -717,6 +1109,26 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
   p.stage_bytes = kBM * 128 + p.bn * 128 + (has_lora ? p.lora_rt * 128 : 0);
   p.up_buf_bytes = has_lora ? kSlab * p.lora_r * 4 : 0;
   const int rt = has_lora ? p.lora_rt : 0;
+  if (p.bn == kWideBN) {
+    // one CTA per SM: the ring gets what the two warpgroups' epilogue buffers leave of the SM's shared memory
+    const int budget = smem_budget(ctx, 1);
+    const int epi = 2 * wide_epi_bytes(rt, has_lora ? p.lora_r : 0);
+    const int stages = std::min(kMaxStages, (budget - kBarRegion - kAlignSlack - epi) / p.stage_bytes);
+    if (stages < 2) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
+    p.stages = stages;
+    p.ring_bytes = stages * p.stage_bytes + epi;
+    const int smem = kBarRegion + kAlignSlack + p.ring_bytes;
+    pdl_hint() = p.num_m_tiles * p.num_n_tiles <= 2 * ctx->num_sms;
+    int st;
+    switch (rt) {
+      case 0: st = launch_gemm_wide<0>(ctx, stream, p, smem); break;
+      case 16: st = launch_gemm_wide<16>(ctx, stream, p, smem); break;
+      default: st = launch_gemm_wide<32>(ctx, stream, p, smem); break;
+    }
+    if (st) return st;
+    SB200_CUDA_CHECK(cudaGetLastError());
+    return 0;
+  }
   const int grid_ctas = p.num_m_tiles * p.num_n_tiles * ctas * (p.sk_ws ? p.sk_splits : 1);
   // A grid that gives each SM at most one CTA lets that CTA have the whole SM's shared memory (a deeper ring).
   const int budget = smem_budget(ctx, grid_ctas > ctx->num_sms ? gemm_slots(p.bn, rt) : 1);
@@ -901,10 +1313,13 @@ extern "C" int sb200_gemm_ln(void* handle, void* stream, const void* x0, int ldx
   }
   int bn, force_ctas;
   decode_bn(bn_arg, &bn, &force_ctas);
-  TileChoice tc = pick_tile(N, ctx->num_sms, p.kblocks, has_lora ? lora->rt : 0, force_ctas, p.num_sub, flags);
+  TileChoice tc = pick_tile(N, ctx->num_sms, p.kblocks, has_lora ? lora->rt : 0, force_ctas, p.num_sub, flags,
+                            ln != nullptr, rowstats != nullptr);
   if (bn > 0) tc.bn = bn;
   if (force_ctas) tc.ctas = force_ctas;
-  SB200_REQUIRE(bn_supported(tc.bn), "gemm: bn=%d invalid (64 or 128)", tc.bn);
+  SB200_REQUIRE(bn_supported(tc.bn), "gemm: bn=%d invalid (64, 128 or 256)", tc.bn);
+  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(N, tc.ctas, ln != nullptr, rowstats != nullptr),
+                "gemm: bn=256 needs N %% 256 == 0 and single CTAs, without lnfold or rowstats (N=%d)", N);
   p.bn = tc.bn;
   p.ncols_out = geglu ? tc.bn / 2 : tc.bn;
   p.num_m_tiles = (p.num_sub + tc.ctas - 1) / tc.ctas;
@@ -1045,10 +1460,13 @@ extern "C" int sb200_conv3x3(void* handle, void* stream, const void* x0, int ldx
   }
   int bn, force_ctas;
   decode_bn(bn_arg, &bn, &force_ctas);
-  TileChoice tc = pick_tile(Cout, ctx->num_sms, p.kblocks, has_lora ? lora->rt : 0, force_ctas, p.num_sub, flags);
+  TileChoice tc = pick_tile(Cout, ctx->num_sms, p.kblocks, has_lora ? lora->rt : 0, force_ctas, p.num_sub, flags,
+                            false, false);
   if (bn > 0) tc.bn = bn;
   if (force_ctas) tc.ctas = force_ctas;
-  SB200_REQUIRE(bn_supported(tc.bn), "conv3x3: bn=%d invalid (64 or 128)", tc.bn);
+  SB200_REQUIRE(bn_supported(tc.bn), "conv3x3: bn=%d invalid (64, 128 or 256)", tc.bn);
+  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(Cout, tc.ctas, false, false),
+                "conv3x3: bn=256 needs Cout %% 256 == 0 and single CTAs (Cout=%d)", Cout);
   p.bn = tc.bn;
   p.ncols_out = tc.bn;
   p.num_m_tiles = (p.num_sub + tc.ctas - 1) / tc.ctas;

@@ -132,6 +132,13 @@ __device__ __forceinline__ void wgmma_wait() {
 // Keeps the compiler from moving accumulator accesses across a wgmma wait.
 __device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
+// Warpgroup register reallocation: every thread of the warpgroup lowers (dec) or raises (inc) its register count to N;
+// registers a producer warpgroup gives back become available to the consumer warpgroups' inc.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // Descriptor of a 128-byte-swizzled tile whose rows are 128 B (64 bf16), as TMA writes it with SWIZZLE_128B:
 //   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4 (unused by these layouts: 1)
 //   bits [32,46) stride byte offset >> 4   bits [62,64) layout type (1 = SWIZZLE_128B)
@@ -194,6 +201,14 @@ __device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint4& v) {
   asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
                : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------
