@@ -395,6 +395,10 @@ static int attention_bwd_impl(void* handle, void* stream, const void* q, int ldq
   SB200_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && lddo % 8 == 0 && lddq % 8 == 0 &&
                     (!dk || (lddk % 8 == 0 && lddv % 8 == 0)),
                 "attention_bwd: leading dims must be multiples of 8");
+  const int width = heads * head_dim;
+  SB200_REQUIRE(ldq >= width && ldk >= width && ldv >= width && ldo >= width && lddo >= width && lddq >= width &&
+                    (!dk || (lddk >= width && lddv >= width)),
+                "attention_bwd: heads=%d x head_dim=%d exceeds a row", heads, head_dim);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   {
     const size_t total = static_cast<size_t>(B) * Sq * heads;

@@ -870,7 +870,9 @@ extern "C" int sb200_groupnorm_bwd(void* handle, void* stream, const void* x0, i
   SB200_REQUIRE(ldx0 % 8 == 0 && lddy % 8 == 0 && lddx % 8 == 0 && (C1 == 0 || ldx1 % 8 == 0) &&
                     (!add || ldadd % 8 == 0),
                 "groupnorm_bwd: leading dims");
-  SB200_REQUIRE(C / 8 <= 1024 && fwd_stats && ws && gamma && beta && dy && dx, "groupnorm_bwd: arguments");
+  SB200_REQUIRE(fwd_stats && ws && gamma && beta && dy && dx, "groupnorm_bwd: arguments");
+  // the stats kernel keeps [rows_par][C][2] fp32 partials in dynamic shared memory without opting in above 48 KB
+  SB200_REQUIRE(gn_stats_smem_ok(C), "groupnorm_bwd: C=%d too large", C);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   GnBwdArgs a;
   a.x0 = static_cast<const bf*>(x0);
@@ -890,6 +892,15 @@ extern "C" int sb200_groupnorm_bwd(void* handle, void* stream, const void* x0, i
   int rows_par = 512 / nvec;
   if (rows_par < 1) rows_par = 1;
   const int threads = nvec * rows_par;
+  // above C = 4096 a block has C/8 > 512 threads; the stats / apply kernels' register use caps the block size
+  int max_threads = 1024;
+  for (const void* fn : {reinterpret_cast<const void*>(gn_bwd_stats_kernel), reinterpret_cast<const void*>(gn_bwd_apply_kernel)}) {
+    cudaFuncAttributes attr;
+    SB200_CUDA_CHECK(cudaFuncGetAttributes(&attr, fn));
+    if (attr.maxThreadsPerBlock < max_threads) max_threads = attr.maxThreadsPerBlock;
+  }
+  SB200_REQUIRE(threads <= max_threads, "groupnorm_bwd: C=%d too large (%d threads per block, at most %d)", C, threads,
+                max_threads);
   int chunks = (ctx->num_sms * 4 + B - 1) / B;
   if (chunks > kGnBwdMaxChunks) chunks = kGnBwdMaxChunks;
   int rows_per_block = (HW + chunks - 1) / chunks;

@@ -112,4 +112,15 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 
 inline Ctx* as_ctx(void* h) { return reinterpret_cast<Ctx*>(h); }
 
+// GroupNorm forward / backward stats kernels: block = (C/8) x rows_par threads, rows_par = max(1, 512 / (C/8)), with
+// [rows_par][C][2] fp32 partials in dynamic shared memory.  They launch without opting in above the default 48 KB,
+// so C may not exceed 6144 (rows_par = 1 for C > 4096).
+inline int gn_rows_par(int C) {
+  const int rp = 512 / (C / 8);
+  return rp < 1 ? 1 : rp;
+}
+inline bool gn_stats_smem_ok(int C) {
+  return C > 0 && sizeof(float) * 2 * static_cast<size_t>(C) * gn_rows_par(C) <= 48 * 1024;
+}
+
 }  // namespace sb200

@@ -279,7 +279,8 @@ extern "C" int sb200_groupnorm(void* handle, void* stream, const void* x0, int l
   SB200_REQUIRE(B > 0 && HW > 0 && C0 > 0 && C0 % 8 == 0 && C1 % 8 == 0, "groupnorm: dims (C0=%d C1=%d)", C0, C1);
   SB200_REQUIRE(groups > 0 && C % groups == 0, "groupnorm: C=%d not divisible by groups=%d", C, groups);
   SB200_REQUIRE(ldx0 % 8 == 0 && ldo % 8 == 0 && (C1 == 0 || ldx1 % 8 == 0), "groupnorm: leading dims");
-  SB200_REQUIRE(C / 8 <= 1024, "groupnorm: C=%d too large", C);
+  // the stats kernel keeps [rows_par][C][2] fp32 partials in dynamic shared memory without opting in above 48 KB
+  SB200_REQUIRE(gn_stats_smem_ok(C), "groupnorm: C=%d too large", C);
   SB200_REQUIRE(stats_ws && gamma && beta, "groupnorm: NULL argument");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   pdl_hint() = static_cast<long long>(B) * HW * C <= (16LL << 20);

@@ -465,53 +465,81 @@ def guided_step_loss(eps_u, eps_c, g: float, x, cx: float, ce: float, target) ->
     return GuidedStepLoss.apply(eps_u, eps_c, g, x, cx, ce, target)
 
 
-def groupnorm_bwd(x0, gamma, beta, groups: int, silu: bool, dy, stats_ws, *, x1=None, add=None) -> torch.Tensor:
+def _row_matrix_out(out: Optional[torch.Tensor], shape, what: str, dtype=BF16) -> torch.Tensor:
+    """`out` if its elements are the rows of one 2-D matrix (unit column stride, every leading dimension packed
+    over the next; e.g. a column slice of a wider buffer) of the given shape and dtype, else ValueError.  None stays
+    None (the caller allocates)."""
+    shape = tuple(shape)
+    if out is None:
+        return None
+    st = out.stride()
+    if (tuple(out.shape) != shape or out.dtype != dtype or st[-1] != 1
+            or any(st[i] != shape[i + 1] * st[i + 1] for i in range(len(shape) - 2))):
+        raise ValueError(f"{what}: out {tuple(out.shape)} {out.dtype} / strides {st} is not a row-strided "
+                         f"{shape} {dtype} matrix")
+    return out
+
+
+def groupnorm_bwd(x0, gamma, beta, groups: int, silu: bool, dy, stats_ws, *, x1=None, add=None,
+                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Input gradient of `groupnorm` (concat layout [.., C0 + C1]); stats_ws is the forward's workspace, or its
-    (mean, rstd) block as a [B, groups, 2] tensor (`gn_stats` — sliceable along the batch)."""
+    (mean, rstd) block as a [B, groups, 2] tensor (`gn_stats` — sliceable along the batch).  `out`: a [.., C0 + C1]
+    tensor whose pixels are rows of one 2-D matrix with row stride out.stride(-2) (e.g. a column slice)."""
     shp = x0.shape
     B, C0 = shp[0], shp[-1]
     HW = x0.numel() // (B * C0)
     C1 = x1.shape[-1] if x1 is not None else 0
     Cc = C0 + C1
-    dx = torch.empty(shp[:-1] + (Cc,), device=x0.device, dtype=BF16)
+    dx = _row_matrix_out(out, shp[:-1] + (Cc,), "groupnorm_bwd")
+    if dx is None:
+        dx = torch.empty(shp[:-1] + (Cc,), device=x0.device, dtype=BF16)
     ws = gn_ws(B, groups, x0.device)
     fwd = stats_ws if stats_ws.dim() == 3 else stats_ws[B * groups * 2 * GN_STATS_OFFSET:]
     assert fwd.is_contiguous()
     lib = _begin()
     _cabi.check(lib.sb200_groupnorm_bwd(
         _ctx(x0), _stream(), _p(x0), x0.stride(-2), C0, _p(x1), x1.stride(-2) if x1 is not None else 0, C1,
-        _p(gamma), _p(beta), _p(dy), dy.stride(-2), _p(add), add.stride(-2) if add is not None else 0, _p(dx), Cc,
-        B, HW, groups, int(silu), _p(fwd), _p(ws)))
+        _p(gamma), _p(beta), _p(dy), dy.stride(-2), _p(add), add.stride(-2) if add is not None else 0, _p(dx),
+        dx.stride(-2), B, HW, groups, int(silu), _p(fwd), _p(ws)))
     _count("groupnorm_bwd")
     return dx
 
 
-def layernorm_bwd(x, gamma, dy, eps: float = 1e-5, add=None) -> torch.Tensor:
+def layernorm_bwd(x, gamma, dy, eps: float = 1e-5, add=None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """`out`: an [M, C] row-strided matrix (e.g. a column slice of a wider buffer) to write dx into."""
     M, Cc = x.shape
-    dx = torch.empty((M, Cc), device=x.device, dtype=BF16)
+    dx = _row_matrix_out(out, (M, Cc), "layernorm_bwd")
+    if dx is None:
+        dx = torch.empty((M, Cc), device=x.device, dtype=BF16)
     lib = _begin()
     _cabi.check(lib.sb200_layernorm_bwd(_ctx(x), _stream(), _p(x), x.stride(0), _p(gamma), _p(dy), dy.stride(0),
-                                        _p(add), add.stride(0) if add is not None else 0, _p(dx), Cc, M, Cc,
-                                        float(eps)))
+                                        _p(add), add.stride(0) if add is not None else 0, _p(dx), dx.stride(0), M,
+                                        Cc, float(eps)))
     _count()
     return dx
 
 
-def geglu(pre: torch.Tensor) -> torch.Tensor:
+def geglu(pre: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """`out`: an [M, F] row-strided matrix to write a * gelu(g) into."""
     M, F2 = pre.shape
-    out = torch.empty((M, F2 // 2), device=pre.device, dtype=BF16)
+    o = _row_matrix_out(out, (M, F2 // 2), "geglu")
+    if o is None:
+        o = torch.empty((M, F2 // 2), device=pre.device, dtype=BF16)
     lib = _begin()
-    _cabi.check(lib.sb200_geglu(_ctx(pre), _stream(), _p(pre), pre.stride(0), _p(out), F2 // 2, M, F2 // 2))
+    _cabi.check(lib.sb200_geglu(_ctx(pre), _stream(), _p(pre), pre.stride(0), _p(o), o.stride(0), M, F2 // 2))
     _count()
-    return out
+    return o
 
 
-def geglu_bwd(pre: torch.Tensor, dout: torch.Tensor) -> torch.Tensor:
+def geglu_bwd(pre: torch.Tensor, dout: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """`out`: an [M, 2F] row-strided matrix to write [da | dg] into."""
     M, F2 = pre.shape
-    dpre = torch.empty((M, F2), device=pre.device, dtype=BF16)
+    dpre = _row_matrix_out(out, (M, F2), "geglu_bwd")
+    if dpre is None:
+        dpre = torch.empty((M, F2), device=pre.device, dtype=BF16)
     lib = _begin()
     _cabi.check(lib.sb200_geglu_bwd(_ctx(pre), _stream(), _p(pre), pre.stride(0), _p(dout), dout.stride(0),
-                                    _p(dpre), F2, M, F2 // 2))
+                                    _p(dpre), dpre.stride(0), M, F2 // 2))
     _count()
     return dpre
 

@@ -668,6 +668,31 @@ def test_bad_arguments_return_errors_not_crashes(dev):
         ops.conv3x3(torch.zeros(1, 9, 9, 64, device=dev, dtype=BF), torch.zeros(64, 3, 3, 64, device=dev, dtype=BF), stride=2)
     with pytest.raises(_cabi.Sb200Error, match="CUDA tensors"):
         ops.layernorm(torch.zeros(4, 64, dtype=BF), torch.zeros(64, dtype=BF), torch.zeros(64, dtype=BF))
+    # GroupNorm: the stats kernels' shared memory (8 C bytes once C > 4096) stays within the default 48 KB
+    for C, ok in ((6144, True), (6152, False)):
+        x = torch.randn(1, 4, 4, C, device=dev).to(BF)
+        gm, bt = torch.ones(C, device=dev, dtype=BF), torch.zeros(C, device=dev, dtype=BF)
+        ws = ops.gn_ws(1, 8, dev)
+        if ok:
+            y = ops.groupnorm(x, gm, bt, 8, 1e-5, False, stats_ws=ws)
+            torch.cuda.synchronize()
+            assert torch.isfinite(y.float()).all()
+            # the backward's 768-thread blocks exceed what its kernels' registers allow (at most 640 on sm_90a):
+            # refused before any launch
+            with pytest.raises(_cabi.Sb200Error, match="too large"):
+                ops.groupnorm_bwd(x, gm, bt, 8, False, x, ws)
+            continue
+        with pytest.raises(_cabi.Sb200Error, match="too large"):
+            ops.groupnorm(x, gm, bt, 8, 1e-5, False, stats_ws=ws)
+        with pytest.raises(_cabi.Sb200Error, match="too large"):
+            ops.groupnorm_bwd(x, gm, bt, 8, False, x, ws)
+    # attention backward: every operand row must hold heads x head_dim columns
+    q = torch.zeros(64, 128, device=dev, dtype=BF)
+    lse = torch.zeros(1, 2, 64, device=dev)
+    with pytest.raises(_cabi.Sb200Error, match="exceeds a row"):
+        ops.attention_bwd(q, q, q, q, q, lse, 1, 2, 64, 64, 0.125, 64, torch.zeros(128, 64, device=dev, dtype=BF))
+    with pytest.raises(ValueError, match="row-strided"):
+        ops.layernorm_bwd(q, q[0], q, out=q.t())
 
 
 @pytest.mark.parametrize("B,heads,Sq,Skv,d", [
