@@ -5,6 +5,7 @@ CUDA graph.  There is deliberately no PyTorch fallback: a missing extension or a
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Optional
 
 import torch
@@ -209,7 +210,16 @@ def conv3x3(x0: torch.Tensor, w_packed: torch.Tensor, *, x1: Optional[torch.Tens
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, B: int, heads: int, Sq: int, Skv: int,
               scale: float, head_dim: int = 64, lse: Optional[torch.Tensor] = None) -> torch.Tensor:
     """q/k/v: 2-D (possibly column-sliced) token matrices; head h = columns [h*head_dim, (h+1)*head_dim).
-    One `attention_kernel`.  lse: optional fp32 [B, heads, Sq] output kept for `attention_bwd`."""
+    One `attention_kernel`.  lse: optional fp32 [B, heads, Sq] output kept for `attention_bwd`.
+    The kernel's TMA descriptors cover exactly B * Sq query and B * Skv key rows of at least heads * head_dim
+    columns, so other layouts raise ValueError."""
+    for name, t, rows in (("q", q, B * Sq), ("k", k, B * Skv), ("v", v, B * Skv)):
+        if t.dim() != 2 or t.shape[0] != rows or t.shape[1] < heads * head_dim:
+            raise ValueError(f"attention: {name} {tuple(t.shape)} is not a [{rows}, >= {heads * head_dim}] matrix")
+        _row_matrix(t, t.shape, "attention", name)
+    if lse is not None and (tuple(lse.shape) != (B, heads, Sq) or lse.dtype != torch.float32
+                            or not lse.is_contiguous()):
+        raise ValueError(f"attention: lse {tuple(lse.shape)} {lse.dtype} is not a contiguous fp32 [{B}, {heads}, {Sq}]")
     out = torch.empty((B * Sq, heads * head_dim), device=q.device, dtype=BF16)
     lib = _begin()
     _cabi.check(lib.sb200_attention(_ctx(q), _stream(), _p(q), q.stride(0), _p(k), k.stride(0), _p(v),
@@ -226,6 +236,11 @@ def groupnorm(x0: torch.Tensor, gamma, beta, groups: int, eps: float, silu: bool
     B, C0 = shp[0], shp[-1]
     HW = x0.numel() // (B * C0)
     C1 = x1.shape[-1] if x1 is not None else 0
+    _row_matrix(x0, shp, "groupnorm", "x0")
+    if x1 is not None:
+        if tuple(x1.shape[:-1]) != tuple(shp[:-1]):
+            raise ValueError(f"groupnorm: x1 {tuple(x1.shape)} has other batch / pixel dims than x0 {tuple(shp)}")
+        _row_matrix(x1, x1.shape, "groupnorm", "x1")
     out = torch.empty(shp[:-1] + (C0 + C1,), device=x0.device, dtype=BF16)
     if stats_ws is None:
         stats_ws = torch.empty(B * groups * 2 * 129, device=x0.device, dtype=torch.float32)  # SB200_GN_WS_FLOATS
@@ -239,6 +254,7 @@ def groupnorm(x0: torch.Tensor, gamma, beta, groups: int, eps: float, silu: bool
 
 def layernorm(x: torch.Tensor, gamma, beta, eps: float = 1e-5) -> torch.Tensor:
     M, Cc = x.shape
+    _row_matrix(x, (M, Cc), "layernorm", "x")
     out = torch.empty((M, Cc), device=x.device, dtype=BF16)
     lib = _begin()
     _cabi.check(lib.sb200_layernorm(_ctx(x), _stream(), _p(x), x.stride(0), _p(gamma), _p(beta), _p(out), Cc, M,
@@ -249,9 +265,15 @@ def layernorm(x: torch.Tensor, gamma, beta, eps: float = 1e-5) -> torch.Tensor:
 
 def small_linear(x: torch.Tensor, w: torch.Tensor, bias=None, *, act_in: bool = False, act_out: int = 0,
                  lora: Optional[Lora] = None, resid: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """act_out: 0 none, 1 SiLU(y) + resid, 2 SiLU(bf16(y + resid)) — see sb200_small_linear."""
+    """act_out: 0 none, 1 SiLU(y) + resid, 2 SiLU(bf16(y + resid)) — see sb200_small_linear.  The kernel reads
+    resid[m * N + n], so resid must be a contiguous [M, N]."""
     M, K = x.shape
     N = w.shape[0]
+    _row_matrix(x, (M, K), "small_linear", "x")
+    _row_matrix(w, (N, K), "small_linear", "w")
+    if resid is not None and (tuple(resid.shape) != (M, N) or resid.dtype != BF16 or not resid.is_contiguous()):
+        raise ValueError(f"small_linear: resid {tuple(resid.shape)} {resid.dtype} / strides {resid.stride()} is not a "
+                         f"contiguous [{M}, {N}] bf16 matrix")
     out = torch.empty((M, N), device=x.device, dtype=BF16)
     lib = _begin()
     _cabi.check(lib.sb200_small_linear(_ctx(x), _stream(), _p(x), x.stride(0), _p(w), w.stride(0), _p(bias),
@@ -285,7 +307,10 @@ def conv_in(latent: torch.Tensor, w_packed: torch.Tensor, bias) -> torch.Tensor:
 
 
 def conv_out(x: torch.Tensor, w_packed: torch.Tensor, bias, out_dtype=BF16) -> torch.Tensor:
+    """x: contiguous NHWC bf16 [B, H, W, Cin] -> NCHW [B, 4, H, W]."""
     B, H, W, Cin = x.shape
+    if x.dtype != BF16 or not x.is_contiguous():
+        raise ValueError(f"conv_out: x {tuple(x.shape)} {x.dtype} / strides {x.stride()} is not contiguous NHWC bf16")
     out = torch.empty((B, 4, H, W), device=x.device, dtype=out_dtype)
     lib = _begin()
     _cabi.check(lib.sb200_conv_out(_ctx(x), _stream(), _p(x), _p(w_packed), _p(bias), _p(out),
@@ -295,7 +320,10 @@ def conv_out(x: torch.Tensor, w_packed: torch.Tensor, bias, out_dtype=BF16) -> t
 
 
 def upsample2x(x: torch.Tensor) -> torch.Tensor:
+    """x: contiguous NHWC bf16 [B, H, W, C] -> [B, 2H, 2W, C] (nearest)."""
     B, H, W, Cc = x.shape
+    if x.dtype != BF16 or not x.is_contiguous():
+        raise ValueError(f"upsample2x: x {tuple(x.shape)} {x.dtype} / strides {x.stride()} is not contiguous NHWC bf16")
     out = torch.empty((B, 2 * H, 2 * W, Cc), device=x.device, dtype=BF16)
     lib = _begin()
     _cabi.check(lib.sb200_upsample2x(_ctx(x), _stream(), _p(x), _p(out), B, H, W, Cc))
@@ -315,6 +343,11 @@ def cfg_ddim(eps2: torch.Tensor, guidance: float, x: Optional[torch.Tensor] = No
     else:
         n = eps2.numel() // 2
         shape = (eps2.shape[0] // 2,) + tuple(eps2.shape[1:])
+    if not eps2.is_contiguous() or (not single and eps2.shape[0] % 2):
+        raise ValueError(f"cfg_ddim: eps2 {tuple(eps2.shape)} / strides {eps2.stride()} is not a contiguous "
+                         f"{'eps' if single else '[uncond ; cond]'} batch")
+    if x is not None and (not x.is_contiguous() or x.numel() != n):
+        raise ValueError(f"cfg_ddim: x {tuple(x.shape)} / strides {x.stride()} is not contiguous with {n} elements")
     if eps2.dtype not in (torch.float32, BF16):
         eps2 = eps2.to(torch.float32)
     out_dtype = out_dtype or (x.dtype if x is not None else eps2.dtype)
@@ -465,19 +498,24 @@ def guided_step_loss(eps_u, eps_c, g: float, x, cx: float, ce: float, target) ->
     return GuidedStepLoss.apply(eps_u, eps_c, g, x, cx, ce, target)
 
 
-def _row_matrix_out(out: Optional[torch.Tensor], shape, what: str, dtype=BF16) -> torch.Tensor:
-    """`out` if its elements are the rows of one 2-D matrix (unit column stride, every leading dimension packed
-    over the next; e.g. a column slice of a wider buffer) of the given shape and dtype, else ValueError.  None stays
-    None (the caller allocates)."""
+def _row_matrix(t: torch.Tensor, shape, what: str, name: str = "out", dtype=BF16) -> torch.Tensor:
+    """t if its elements are the rows of one 2-D matrix of the given shape and dtype, else ValueError.  A row-strided
+    matrix has unit column stride and every leading dimension packed over the next ones with the row stride
+    t.stride(-2) the wrappers pass as the leading dimension (e.g. a column slice of a wider buffer, or an NHWC tensor
+    whose pixels are the rows); a dimension of size 1 is never stepped, so its stride does not matter."""
     shape = tuple(shape)
-    if out is None:
-        return None
-    st = out.stride()
-    if (tuple(out.shape) != shape or out.dtype != dtype or st[-1] != 1
-            or any(st[i] != shape[i + 1] * st[i + 1] for i in range(len(shape) - 2))):
-        raise ValueError(f"{what}: out {tuple(out.shape)} {out.dtype} / strides {st} is not a row-strided "
+    st = t.stride()
+    ld = st[-2] if len(shape) > 1 else 0
+    packed = all(shape[i] == 1 or st[i] == ld * math.prod(shape[i + 1:-1]) for i in range(len(shape) - 2))
+    if tuple(t.shape) != shape or t.dtype != dtype or (shape[-1] > 1 and st[-1] != 1) or not packed:
+        raise ValueError(f"{what}: {name} {tuple(t.shape)} {t.dtype} / strides {st} is not a row-strided "
                          f"{shape} {dtype} matrix")
-    return out
+    return t
+
+
+def _row_matrix_out(out: Optional[torch.Tensor], shape, what: str, dtype=BF16) -> Optional[torch.Tensor]:
+    """`_row_matrix` for an optional output: None stays None (the caller allocates)."""
+    return None if out is None else _row_matrix(out, shape, what, "out", dtype)
 
 
 def groupnorm_bwd(x0, gamma, beta, groups: int, silu: bool, dy, stats_ws, *, x1=None, add=None,
