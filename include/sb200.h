@@ -50,8 +50,10 @@ int sb200_create(int device, void** handle);
 int sb200_destroy(void* handle);
 
 /* LoRA side inputs of a fused GEMM / conv (reference: LoRAModule.forward, trainscripts/textsliders/lora.py:108-112).
+ *   r    : the slot width of one adaptor, 4, 8 or 16.  An adaptor of lower rank is padded with zeros to the next
+ *          slot width (down rows and up columns beyond its rank are 0), which leaves every fp32 sum unchanged.
  *   down : [rt, K] bf16, row j = lora_down.weight row (conv: [r, kh, kw, Cin] flattened tap-major); rows
- *          beyond the used ranks must be zero; rt is 16 or 32.
+ *          beyond the used ranks must be zero; rt is 16, 32 or 64 and at least groups * r.
  *   up   : [N, r] FP32 (lora_up.weight, widened once at pack time so the epilogue spends no cycles on
  *          conversion); output column n uses down rows [(n / group_n) * r, +r), so one call
  *          can carry several adapted leaves that share an input (to_q|to_k|to_v fused: group_n = C).
@@ -212,7 +214,7 @@ int sb200_conv_out_bwd(void* handle, void* stream, const void* deps, int deps_f3
 /* out[b, c] = sum_hw dy[b, hw, c] (fp32): gradient reaching time_emb_proj's output. */
 int sb200_colsum(void* handle, void* stream, const void* dy, int ld, float* out, int B, int HW, int C);
 
-/* Rank-r (r = 4 or 8) LoRA gradient pieces for y = W x + s * up (down x), lora.py:108-112:
+/* Rank-r (r = 4, 8 or 16; lower ranks zero-padded to the next of these) LoRA gradient pieces for y = W x + s * up (down x), lora.py:108-112:
  *   t = x down^T, u = dY up        : sb200_lora_proj   (T[M,r] (+)= A[M,C] Bt[r,C]^T, fp32 out)
  *   d_up = s dY^T t, d_down = s u^T x : sb200_lora_wgrad  (G[c*gs_c + j*gs_r] (+)= scale * sum_m A[m,c] T[m,j])
  *   dX += s u down                 : sb200_lora_rank_update

@@ -79,6 +79,7 @@ class _Grads:
 
     def __init__(self, scales: Dict[int, tuple]):
         self.by_param: Dict[int, torch.Tensor] = {}
+        self.slots: Dict[int, torch.Tensor] = {}
         self.scales = scales
         self.dkv: Optional[torch.Tensor] = None
         self.kv_off: Dict[int, int] = {}
@@ -92,13 +93,29 @@ class _Grads:
     def any_trainable(self) -> bool:
         return any(v[2] for v in self.scales.values())
 
-    def buf(self, param: torch.Tensor, shape) -> Tuple[torch.Tensor, bool]:
-        g = self.by_param.get(id(param))
+    def buf(self, param: torch.Tensor, shape, r: int, rank_dim: int) -> Tuple[torch.Tensor, bool]:
+        """(fp32 gradient buffer of `param` in the kernels' layout `shape`, whose axis `rank_dim` has the slot width;
+        whether it already holds a gradient).  by_param files its first r entries along that axis: the gradient in
+        the parameter's own rank, without the padding."""
+        g = self.slots.get(id(param))
         if g is None:
             g = torch.empty(shape, device=param.device, dtype=torch.float32)
-            self.by_param[id(param)] = g
+            self.slots[id(param)] = g
+            self.by_param[id(param)] = g.narrow(rank_dim, 0, r)
             return g, False
         return g, True
+
+
+def _pad_rank(t: torch.Tensor, dim: int, rp: int) -> torch.Tensor:
+    """t zero-padded along its rank axis `dim` to the slot width rp (t itself when it has that size already)."""
+    r = t.shape[dim]
+    if r == rp:
+        return t
+    shape = list(t.shape)
+    shape[dim] = rp
+    out = t.new_zeros(shape)
+    out.narrow(dim, 0, r).copy_(t)
+    return out
 
 
 def _new_tape(unet) -> list:
@@ -121,6 +138,8 @@ def _lora_linear_bwd(unet, grads: _Grads, leaf, xs: List[torch.Tensor], dY: torc
     down = a.lora_down.weight.detach().reshape(a.lora_down.weight.shape[0], -1).to(BF16)   # [r, K]
     up = a.lora_up.weight.detach().reshape(a.lora_up.weight.shape[0], -1).to(BF16)         # [N, r]
     r, K = down.shape
+    rp, _ = ops.lora_slots(r)  # the kernels take rank rp: zero rows / columns beyond r
+    down, up = _pad_rank(down, 0, rp), _pad_rank(up, 1, rp)
     if not train:  # frozen adaptor: its share of the input gradient only
         ops.lora_rank_update(dX, ops.lora_proj(dY, up.t().contiguous()), down, s)
         return
@@ -130,9 +149,9 @@ def _lora_linear_bwd(unet, grads: _Grads, leaf, xs: List[torch.Tensor], dY: torc
         t = ops.lora_proj(x, down[:, k0:k0 + x.shape[1]], out=t)
         k0 += x.shape[1]
     u = ops.lora_proj(dY, up.t().contiguous())
-    g_up, acc = grads.buf(a.lora_up.weight, (up.shape[0], r))
+    g_up, acc = grads.buf(a.lora_up.weight, (up.shape[0], rp), r, 1)
     ops.lora_wgrad(dY, t, g_up, False, s, accumulate=acc)
-    g_down, acc = grads.buf(a.lora_down.weight, (r, K))
+    g_down, acc = grads.buf(a.lora_down.weight, (rp, K), r, 0)
     k0 = 0
     for x in xs:
         ops.lora_wgrad(x, u, g_down[:, k0:k0 + x.shape[1]], True, s, accumulate=acc)
@@ -151,15 +170,17 @@ def _lora_conv_bwd(unet, grads: _Grads, conv, x: torch.Tensor, dY: torch.Tensor,
     D = a.lora_down.weight.detach().permute(0, 2, 3, 1).to(BF16).contiguous()             # [r, 3, 3, Cin]
     up = a.lora_up.weight.detach().reshape(a.lora_up.weight.shape[0], -1).to(BF16)        # [Cout, r]
     r = D.shape[0]
+    rp, _ = ops.lora_slots(r)
+    D, up = _pad_rank(D, 0, rp), _pad_rank(up, 1, rp)
     dY2 = dY.reshape(-1, dY.shape[-1])
     if not train:  # frozen adaptor: its share of the input gradient only
         ops.lora_conv_rank_update(dX, ops.lora_proj(dY2, up.t().contiguous()), D, s, stride)
         return
     t = ops.lora_conv_proj(x, D, stride)
     u = ops.lora_proj(dY2, up.t().contiguous())
-    g_up, acc = grads.buf(a.lora_up.weight, (up.shape[0], r))
+    g_up, acc = grads.buf(a.lora_up.weight, (up.shape[0], rp), r, 1)
     ops.lora_wgrad(dY2, t, g_up, False, s, accumulate=acc)
-    g_down, acc = grads.buf(a.lora_down.weight, tuple(D.shape))
+    g_down, acc = grads.buf(a.lora_down.weight, tuple(D.shape), r, 0)
     ops.lora_conv_wgrad(x, u, g_down, s, stride, accumulate=acc)
     if dX is not None:
         ops.lora_conv_rank_update(dX, u, D, s, stride)

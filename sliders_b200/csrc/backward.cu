@@ -492,9 +492,9 @@ __global__ void colsum_kernel(const __nv_bfloat16* __restrict__ dy, int ld, floa
 }
 
 // ------------------------------------------------------------------------------------------------
-// LoRA rank-r helpers (r <= 8).  Matrices: A [M, C] bf16 activations or gradients (row stride lda).
+// LoRA rank-r helpers (r = 4, 8 or 16).  Matrices: A [M, C] bf16 activations or gradients (row stride lda).
 // ------------------------------------------------------------------------------------------------
-constexpr int kMaxR = 8;
+constexpr int kMaxR = 16;
 constexpr int kVB = 32;  // 8-channel vectors per block in the wgrad / rank-update kernels (block = kVB x 4 row lanes)
 
 // T[m, j] = sum_c A[m, c] * Bt[j, c]     (Bt: [r][C] bf16, row stride ldb)  -> T fp32 [M, r]
@@ -522,8 +522,10 @@ __global__ void lora_proj_kernel(const __nv_bfloat16* __restrict__ A, int lda, c
     }
 #pragma unroll
     for (int j = 0; j < kMaxR; ++j) {
+      if (j < r) {
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], o);
+        for (int o = 16; o > 0; o >>= 1) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], o);
+      }
     }
     if (lane == 0) {
       for (int j = 0; j < r; ++j) {
@@ -534,7 +536,9 @@ __global__ void lora_proj_kernel(const __nv_bfloat16* __restrict__ A, int lda, c
   }
 }
 
-// partial[chunk][c][j] = sum_{m in chunk} A[m, c] * T[m, j];   grid (chunks, ceil(C/8/kVB)), block (kVB vectors, 4 row lanes)
+// partial[chunk][c][j] = sum_{m in chunk} A[m, c] * T[m, j];   grid (chunks, ceil(C/8/kVB), halves), block (kVB vectors,
+// 4 row lanes).  Each z slice owns R consecutive columns j of T and partial, whose rows are halves * R wide: rank 16
+// runs as two R = 8 slices (R = 16 would need 64 KB of static shared memory and 128 accumulators per thread).
 template <int R>
 __global__ void lora_wgrad_kernel(const __nv_bfloat16* __restrict__ A, int lda, const float* __restrict__ T,
                                   float* __restrict__ partial, int M, int C, int rows_per_block) {
@@ -543,6 +547,7 @@ __global__ void lora_wgrad_kernel(const __nv_bfloat16* __restrict__ A, int lda, 
   __shared__ float sh[4][kVB][8 * R];
   const int cv = blockIdx.y * kVB + threadIdx.x;
   const int nvec = C >> 3;
+  const int ldt = gridDim.z * R, j0 = blockIdx.z * R;  // row stride of T and partial, first column of this slice
   float acc[8][R];
 #pragma unroll
   for (int k = 0; k < 8; ++k)
@@ -556,7 +561,7 @@ __global__ void lora_wgrad_kernel(const __nv_bfloat16* __restrict__ A, int lda, 
       unpack8(__ldg(reinterpret_cast<const uint4*>(A + static_cast<size_t>(m) * lda + cv * 8)), a);
 #pragma unroll
       for (int j = 0; j < R; j += 4) {
-        const float4 t4 = __ldg(reinterpret_cast<const float4*>(T + static_cast<size_t>(m) * R + j));
+        const float4 t4 = __ldg(reinterpret_cast<const float4*>(T + static_cast<size_t>(m) * ldt + j0 + j));
         t[j] = t4.x, t[j + 1] = t4.y, t[j + 2] = t4.z, t[j + 3] = t4.w;
       }
 #pragma unroll
@@ -571,10 +576,11 @@ __global__ void lora_wgrad_kernel(const __nv_bfloat16* __restrict__ A, int lda, 
     for (int j = 0; j < R; ++j) sh[threadIdx.y][threadIdx.x][k * R + j] = acc[k][j];
   __syncthreads();
   if (threadIdx.y == 0 && cv < nvec) {
-    float* out = partial + (static_cast<size_t>(blockIdx.x) * C + cv * 8) * R;
+    float* out = partial + (static_cast<size_t>(blockIdx.x) * C + cv * 8) * ldt + j0;
 #pragma unroll
     for (int e = 0; e < 8 * R; ++e)
-      out[e] = sh[0][threadIdx.x][e] + sh[1][threadIdx.x][e] + sh[2][threadIdx.x][e] + sh[3][threadIdx.x][e];
+      out[(e / R) * ldt + e % R] =
+          sh[0][threadIdx.x][e] + sh[1][threadIdx.x][e] + sh[2][threadIdx.x][e] + sh[3][threadIdx.x][e];
   }
 }
 
@@ -672,22 +678,26 @@ __global__ void lora_conv_proj_kernel(ConvGeom g, const __nv_bfloat16* __restric
     }
 #pragma unroll
     for (int j = 0; j < kMaxR; ++j) {
+      if (j < r) {
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], o);
+        for (int o = 16; o > 0; o >>= 1) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], o);
+      }
     }
     if (lane == 0)
       for (int j = 0; j < r; ++j) T[static_cast<size_t>(p) * r + j] = acc[j];
   }
 }
 
-// partial[chunk][tap][c][j] = sum_{p in chunk} U[p, j] * x[p*stride + tap - 1, c];  grid (chunks, ceil(C/8/kVB), 9)
+// partial[chunk][tap][c][j] = sum_{p in chunk} U[p, j] * x[p*stride + tap - 1, c];  grid (chunks, ceil(C/8/kVB),
+// 9 * halves): z = half * 9 + tap, the column slices as in lora_wgrad_kernel
 template <int R>
 __global__ void lora_conv_wgrad_kernel(ConvGeom g, const float* __restrict__ U, float* __restrict__ partial,
                                        int rows_per_block) {
   pdl_trigger();
   pdl_wait();
   __shared__ float sh[4][kVB][8 * R];
-  const int cv = blockIdx.y * kVB + threadIdx.x, nvec = g.C >> 3, tap = blockIdx.z;
+  const int cv = blockIdx.y * kVB + threadIdx.x, nvec = g.C >> 3, tap = blockIdx.z % 9;
+  const int ldt = (gridDim.z / 9) * R, j0 = (blockIdx.z / 9) * R;  // row stride of U and partial, first column
   const int P = g.B * g.Ho * g.Wo;
   float acc[8][R];
 #pragma unroll
@@ -706,7 +716,7 @@ __global__ void lora_conv_wgrad_kernel(ConvGeom g, const float* __restrict__ U, 
       unpack8(__ldg(reinterpret_cast<const uint4*>(conv_src(g, pix, cv * 8))), a);
 #pragma unroll
       for (int j = 0; j < R; j += 4) {
-        const float4 t4 = __ldg(reinterpret_cast<const float4*>(U + static_cast<size_t>(p) * R + j));
+        const float4 t4 = __ldg(reinterpret_cast<const float4*>(U + static_cast<size_t>(p) * ldt + j0 + j));
         t[j] = t4.x, t[j + 1] = t4.y, t[j + 2] = t4.z, t[j + 3] = t4.w;
       }
 #pragma unroll
@@ -722,10 +732,11 @@ __global__ void lora_conv_wgrad_kernel(ConvGeom g, const float* __restrict__ U, 
   __syncthreads();
   if (threadIdx.y == 0 && cv < nvec) {
     // partial layout: [chunk][tap*C + c][j]  (= lora_wgrad_reduce_kernel's layout with "C" = 9*C)
-    float* out = partial + ((static_cast<size_t>(blockIdx.x) * 9 + tap) * g.C + cv * 8) * R;
+    float* out = partial + ((static_cast<size_t>(blockIdx.x) * 9 + tap) * g.C + cv * 8) * ldt + j0;
 #pragma unroll
     for (int e = 0; e < 8 * R; ++e)
-      out[e] = sh[0][threadIdx.x][e] + sh[1][threadIdx.x][e] + sh[2][threadIdx.x][e] + sh[3][threadIdx.x][e];
+      out[(e / R) * ldt + e % R] =
+          sh[0][threadIdx.x][e] + sh[1][threadIdx.x][e] + sh[2][threadIdx.x][e] + sh[3][threadIdx.x][e];
   }
 }
 
@@ -1023,7 +1034,8 @@ extern "C" int sb200_lora_proj(void* handle, void* stream, const void* A, int ld
                                int M, int C, int r, int accumulate) {
   pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
-  SB200_REQUIRE(ctx && A && Bt && T && M > 0 && C % 8 == 0 && lda % 8 == 0 && ldb % 8 == 0 && (r == 4 || r == 8),
+  SB200_REQUIRE(ctx && A && Bt && T && M > 0 && C % 8 == 0 && lda % 8 == 0 && ldb % 8 == 0 &&
+                    (r == 4 || r == 8 || r == 16),
                 "lora_proj: arguments (r=%d)", r);
   int blocks = (M + 7) / 8;
   if (blocks > ctx->num_sms * 16) blocks = ctx->num_sms * 16;
@@ -1047,13 +1059,13 @@ extern "C" int sb200_lora_wgrad(void* handle, void* stream, const void* A, int l
                                 int gs_c, int gs_r, float scale, int accumulate, int M, int C, int r, float* ws) {
   pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
-  SB200_REQUIRE(ctx && A && T && G && ws && M > 0 && C % 8 == 0 && lda % 8 == 0 && (r == 4 || r == 8),
+  SB200_REQUIRE(ctx && A && T && G && ws && M > 0 && C % 8 == 0 && lda % 8 == 0 && (r == 4 || r == 8 || r == 16),
                 "lora_wgrad: arguments (r=%d)", r);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int cblocks = (C / 8 + kVB - 1) / kVB;
   int rpb;
   const int chunks = wgrad_chunks(ctx, M, cblocks, &rpb);
-  dim3 grid(chunks, cblocks), block(kVB, 4);
+  dim3 grid(chunks, cblocks, r == 16 ? 2 : 1), block(kVB, 4);
   if (r == 4)
     SB200_CUDA_CHECK(launch_pdl(lora_wgrad_kernel<4>, dim3(grid), dim3(block), 0, s, static_cast<const bf*>(A), lda, T, ws, M, C, rpb));
   else
@@ -1066,7 +1078,8 @@ extern "C" int sb200_lora_rank_update(void* handle, void* stream, void* dX, int 
                                       int ldd, float scale, int M, int C, int r) {
   pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
-  SB200_REQUIRE(ctx && dX && U && D && M > 0 && C % 8 == 0 && ldx % 8 == 0 && ldd % 8 == 0 && (r == 4 || r == 8),
+  SB200_REQUIRE(ctx && dX && U && D && M > 0 && C % 8 == 0 && ldx % 8 == 0 && ldd % 8 == 0 &&
+                    (r == 4 || r == 8 || r == 16),
                 "lora_rank_update: arguments (r=%d)", r);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int cblocks = (C / 8 + kVB - 1) / kVB;
@@ -1076,8 +1089,11 @@ extern "C" int sb200_lora_rank_update(void* handle, void* stream, void* dX, int 
   if (r == 4)
     SB200_CUDA_CHECK(launch_pdl(lora_rank_update_kernel<4>, dim3(grid), dim3(block), 0, s, static_cast<bf*>(dX), ldx, U, static_cast<const bf*>(D), ldd,
                                                      scale, M, C, rpb));
-  else
+  else if (r == 8)
     SB200_CUDA_CHECK(launch_pdl(lora_rank_update_kernel<8>, dim3(grid), dim3(block), 0, s, static_cast<bf*>(dX), ldx, U, static_cast<const bf*>(D), ldd,
+                                                     scale, M, C, rpb));
+  else
+    SB200_CUDA_CHECK(launch_pdl(lora_rank_update_kernel<16>, dim3(grid), dim3(block), 0, s, static_cast<bf*>(dX), ldx, U, static_cast<const bf*>(D), ldd,
                                                      scale, M, C, rpb));
   return 0;
 }
@@ -1096,7 +1112,7 @@ extern "C" int sb200_lora_conv_proj(void* handle, void* stream, const void* x0, 
   pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && x0 && D && T && C0 % 8 == 0 && (!x1 || C1 % 8 == 0) && (stride == 1 || stride == 2) &&
-                    (r == 4 || r == 8),
+                    (r == 4 || r == 8 || r == 16),
                 "lora_conv_proj: arguments");
   ConvGeom g;
   fill_geom(&g, x0, ldx0, C0, x1, ldx1, C1, B, H, W, stride);
@@ -1114,7 +1130,7 @@ extern "C" int sb200_lora_conv_wgrad(void* handle, void* stream, const void* x0,
   pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && x0 && U && G && ws && C0 % 8 == 0 && (!x1 || C1 % 8 == 0) && (stride == 1 || stride == 2) &&
-                    (r == 4 || r == 8),
+                    (r == 4 || r == 8 || r == 16),
                 "lora_conv_wgrad: arguments");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   ConvGeom g;
@@ -1123,7 +1139,7 @@ extern "C" int sb200_lora_conv_wgrad(void* handle, void* stream, const void* x0,
   const int cblocks = (g.C / 8 + kVB - 1) / kVB;
   int rpb;
   const int chunks = wgrad_chunks(ctx, P, cblocks * 9, &rpb);
-  dim3 grid(chunks, cblocks, 9), block(kVB, 4);
+  dim3 grid(chunks, cblocks, r == 16 ? 18 : 9), block(kVB, 4);
   if (r == 4)
     SB200_CUDA_CHECK(launch_pdl(lora_conv_wgrad_kernel<4>, dim3(grid), dim3(block), 0, s, g, U, ws, rpb));
   else
@@ -1138,15 +1154,19 @@ extern "C" int sb200_lora_conv_rank_update(void* handle, void* stream, void* dX,
                                            float scale, int B, int H, int W, int C, int stride, int r) {
   pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
-  SB200_REQUIRE(ctx && dX && U && D && C % 8 == 0 && (stride == 1 || stride == 2) && (r == 4 || r == 8),
+  SB200_REQUIRE(ctx && dX && U && D && C % 8 == 0 && (stride == 1 || stride == 2) &&
+                    (r == 4 || r == 8 || r == 16),
                 "lora_conv_rank_update: arguments");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int blocks = grid_for(static_cast<size_t>(B) * H * W * C / 8, 256, ctx->num_sms);
   if (r == 4)
     SB200_CUDA_CHECK(launch_pdl(lora_conv_rank_update_kernel<4>, dim3(blocks), dim3(256), 0, s, static_cast<bf*>(dX), B, H, W, C, H / stride, W / stride,
                                                           stride, U, static_cast<const bf*>(D), scale));
-  else
+  else if (r == 8)
     SB200_CUDA_CHECK(launch_pdl(lora_conv_rank_update_kernel<8>, dim3(blocks), dim3(256), 0, s, static_cast<bf*>(dX), B, H, W, C, H / stride, W / stride,
+                                                          stride, U, static_cast<const bf*>(D), scale));
+  else
+    SB200_CUDA_CHECK(launch_pdl(lora_conv_rank_update_kernel<16>, dim3(blocks), dim3(256), 0, s, static_cast<bf*>(dX), B, H, W, C, H / stride, W / stride,
                                                           stride, U, static_cast<const bf*>(D), scale));
   return 0;
 }

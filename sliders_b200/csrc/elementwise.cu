@@ -30,7 +30,7 @@ __global__ void sinusoid_kernel(const float* __restrict__ values, int n, int dim
 constexpr int kSlWarps = 8;
 constexpr int kSlColsPerWarp = 1;  // more, smaller blocks: M <= 64 rows, the kernel is latency-bound (53 -> ~15 us at N = 1280)
 constexpr int kSlMaxM = 64;
-constexpr int kSlMaxR = 8;
+constexpr int kSlMaxR = 16;
 
 struct SmallLinearArgs {
   const __nv_bfloat16* x;
@@ -70,7 +70,9 @@ __device__ __forceinline__ float dot8(const uint4& a, const uint4& b, bool silu_
 __global__ void __launch_bounds__(kSlWarps * 32) small_linear_kernel(SmallLinearArgs a) {
   pdl_trigger();
   pdl_wait();
-  __shared__ float t_sh[kSlMaxM][kSlMaxR * 4];  // LoRA down-projection of every row: [M][groups*r]
+  // LoRA down-projection of every row, [M][groups * r]: a block's kSlWarps * kSlColsPerWarp columns touch at most two
+  // adaptors because group_n >= that many columns (sb200_small_linear checks it), so 2 * kSlMaxR columns (8 KB)
+  __shared__ float t_sh[kSlMaxM][2 * kSlMaxR];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nvec = a.K >> 3;
   const bool silu_in = a.act_in == 1;

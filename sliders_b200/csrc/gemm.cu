@@ -13,9 +13,10 @@
 // LayerNorm fold, bias / time-embedding row bias / GEGLU / residual; residual tiles come in by cp.async and results
 // leave through a swizzled smem staging tile (also in the ring, behind the accumulator tile) so that global accesses
 // are coalesced.
-// Residency: two CTAs per SM wherever 96 registers per thread hold the accumulators without spills (BN = 64, or no
-// LoRA), so one CTA's prologue and epilogue run while the other's wgmmas keep the tensor cores busy; BN = 128 with LoRA
-// needs ~160 registers and runs one CTA per SM.  Each CTA's ring is sized from its share of the SM's shared memory.
+// Residency: two CTAs per SM wherever 96 registers per thread hold the accumulators without spills (BN = 64 with up
+// to 32 LoRA rows, or no LoRA), so one CTA's prologue and epilogue run while the other's wgmmas keep the tensor cores
+// busy; BN = 128 with LoRA needs ~160 registers and runs one CTA per SM, as do the 64 LoRA rows (rank-16 q|k|v) at
+// either width.  Each CTA's ring is sized from its share of the SM's shared memory.
 // CTA pairs (kCtas = 2): a cluster of two CTAs on consecutive 128-row tiles of the same N tile.  Each CTA loads half
 // of the W (and LoRA-down) rows of a stage and multicasts them to both, which halves the weight traffic from L2.
 //
@@ -52,8 +53,9 @@ constexpr int kEpiBytes = kEpiWarps * kEpiBufBytes;  // + kEpiWarps x [32 cols][
 constexpr int kConsumerBar = 5;       // named barrier of the 256 consumer threads (1..4: row-statistics reduction)
 
 // CTAs per SM an instantiation is compiled for (its launch bounds): under two, ptxas caps a thread at 96 registers,
-// which holds BN = 64 with LoRA and BN = 128 without it; BN = 128 with LoRA would spill and serialise its wgmmas
-__host__ __device__ constexpr int gemm_slots(int bn, int rt) { return (bn == 64 || rt == 0) ? 2 : 1; }
+// which holds BN = 64 with up to 32 LoRA rows and BN = 128 without them; BN = 128 with LoRA, and 64 LoRA rows at any
+// width, would spill and serialise their wgmmas (DESIGN §4a)
+__host__ __device__ constexpr int gemm_slots(int bn, int rt) { return rt == 64 ? 1 : (bn == 64 || rt == 0) ? 2 : 1; }
 
 // fp32 accumulator tile in shared memory: row stride BN + rt + 4 floats (an odd multiple of 16 bytes), so that the 32
 // rows a warp reads at one column fall into distinct 16-byte bank groups.  The 4 padding floats also absorb the
@@ -126,18 +128,18 @@ __device__ __forceinline__ void add_bf16x16(float* f, const __nv_bfloat16* src) 
   }
 }
 
-template <int R>
+// f[i] += t . up[i] over NQ groups of four ranks (all R of them by default), four terms at a time in rank order.
+// up_rows: shared-memory address of the first of those ranks in 16 consecutive rows of [N, R] fp32 (same address for
+// the whole warp: broadcast)
+template <int R, int NQ = R / 4>
 __device__ __forceinline__ void lora_apply(float* f, const float* t, uint32_t up_rows) {
-  // up_rows: shared-memory address of 16 consecutive rows of [N, R] fp32 (same address for the whole warp: broadcast)
 #pragma unroll
   for (int i = 0; i < 16; ++i) {
-    const uint4 a = ld_shared_v4(up_rows + i * R * 4);
-    f[i] += t[0] * __uint_as_float(a.x) + t[1] * __uint_as_float(a.y) + t[2] * __uint_as_float(a.z) +
-            t[3] * __uint_as_float(a.w);
-    if constexpr (R == 8) {
-      const uint4 b = ld_shared_v4(up_rows + i * R * 4 + 16);
-      f[i] += t[4] * __uint_as_float(b.x) + t[5] * __uint_as_float(b.y) + t[6] * __uint_as_float(b.z) +
-              t[7] * __uint_as_float(b.w);
+#pragma unroll
+    for (int q = 0; q < NQ; ++q) {
+      const uint4 a = ld_shared_v4(up_rows + i * R * 4 + 16 * q);
+      f[i] += t[4 * q] * __uint_as_float(a.x) + t[4 * q + 1] * __uint_as_float(a.y) +
+              t[4 * q + 2] * __uint_as_float(a.z) + t[4 * q + 3] * __uint_as_float(a.w);
     }
   }
 }
@@ -240,7 +242,8 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
   const uint32_t bar_full = base;            // S barriers
   const uint32_t bar_empty = base + 8u * S;  // S barriers
   const uint32_t tiles = base + kBarRegion;
-  const bool has_lora = (p.flags & SB200_EPI_LORA) != 0;
+  // launch_gemm runs every LoRA call on an RT > 0 instantiation, so the RT = 0 ones carry no LoRA code
+  const bool has_lora = RT != 0 && (p.flags & SB200_EPI_LORA) != 0;
   const bool geglu = (p.flags & SB200_EPI_GEGLU) != 0;
   constexpr int rt = RT;  // LoRA-down rows of a stage (0 without LoRA)
 
@@ -317,12 +320,13 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
   } else {
     // ------------------------------------------------------------------ consumers: main loop
     const int wg = warp >> 2;
+    constexpr int kAccl = RT > 32 ? RT / 2 : 16;  // t = A.down^T fragment registers
     float acc[BN / 2];
-    float accl[16];
+    float accl[kAccl];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
 #pragma unroll
-    for (int i = 0; i < 16; ++i) accl[i] = 0.f;
+    for (int i = 0; i < kAccl; ++i) accl[i] = 0.f;
     const bool signal = (threadIdx.x & 127) == 0;
     const uint32_t peer_empty = kCtas == 2 ? mapa_u32(bar_empty, cta_rank ^ 1u) : 0u;
     int stage = 0, prev = 0;
@@ -340,6 +344,8 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
           wgmma_ss_n16(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
         else if constexpr (rt == 32)
           wgmma_ss_n32(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
+        else if constexpr (rt == 64)
+          wgmma_ss_n64(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
       }
       wgmma_commit();
       wgmma_wait<1>();  // the previous k-block's products have read their stage: hand it back to the producer(s)
@@ -357,7 +363,7 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
 #pragma unroll
-    for (int i = 0; i < 16; ++i) reg_fence(accl[i]);
+    for (int i = 0; i < kAccl; ++i) reg_fence(accl[i]);
 
     // ------------------------------------------------------------------ epilogue
     const uint32_t accs = tiles;  // fp32 accumulator tile, over the stage ring
@@ -368,6 +374,8 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
       store_frag<16>(accl, accs, wg * 64, BN, kStride);
     else if constexpr (rt == 32)
       store_frag<32>(accl, accs, wg * 64, BN, kStride);
+    else if constexpr (rt == 64)
+      store_frag<64>(accl, accs, wg * 64, BN, kStride);
     asm volatile("bar.sync %0, %1;" ::"n"(kConsumerBar), "n"(32 * kEpiWarps) : "memory");
     if (p.sk_ws != nullptr) {
       // split-K: this split's raw fp32 tile, row-coalesced; sb200_gemm_splitk_f32's reduction sums the splits
@@ -456,7 +464,11 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
         const uint32_t ub = ubuf + lane * p.lora_r * 4;
         const float* src = p.lora_up + static_cast<size_t>(n_base + col0 + lane) * p.lora_r;
         cp_async_16(ub, src);
-        if (p.lora_r == 8) cp_async_16(ub + 16, src + 4);
+        if (p.lora_r >= 8) cp_async_16(ub + 16, src + 4);
+        if (p.lora_r == 16) {
+          cp_async_16(ub + 32, src + 8);
+          cp_async_16(ub + 48, src + 12);
+        }
       }
       cp_async_commit();
     };
@@ -466,6 +478,22 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
         (p.flags & SB200_EPI_ROWBIAS) ? p.rowbias + static_cast<size_t>(row_ok ? my_batch : 0) * p.Nout : nullptr;
     float tl[8];
     int group_lo = 0, group_hi = 0;  // output-column range of the adaptor whose t = A.down^T is held in tl
+    // tl = lscale * (LayerNorm-folded) t, from the 8 t columns of this row at column j of the adaptor's r; columns
+    // r.. of the 8 are 0 (rank 4: the row's 4 padding floats cover the last adaptor's read)
+    auto load_t8 = [&](int j, int r_left) {
+      uint32_t tv[8];
+      ld_acc<8>(arow + (BN + j) * 4, tv);
+      if (p.ln_cl != nullptr) {
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+          tl[jj] = (jj < r_left) ? fmaf(__uint_as_float(tv[jj]), ln_rstd,
+                                        fmaf(-ln_rm, __ldg(p.ln_cl + j + jj), __ldg(p.ln_dl + j + jj))) * lscale
+                                 : 0.f;
+      } else {
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) tl[jj] = __uint_as_float(tv[jj]) * lscale;
+      }
+    };
     const uint32_t swz = static_cast<uint32_t>((lane >> 1) & 3);
     for (int k = 0; k < my_slabs; ++k) {
       const int col0 = (hsel + kEpiPerQuarter * k) * kSlab;
@@ -478,23 +506,11 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
         uint32_t g[16];
         ld_acc<16>(arow + c * 4, v);
         if (geglu) ld_acc<16>(arow + ((BN >> 1) + c) * 4, g);
-        if (has_lora && (n < group_lo || n >= group_hi)) {
+        if (has_lora && p.lora_r != 16 && (n < group_lo || n >= group_hi)) {
           const int grp = n / p.lora_group_n;
           group_lo = grp * p.lora_group_n;
           group_hi = group_lo + p.lora_group_n;
-          uint32_t tv[8];
-          const int j = grp * p.lora_r;
-          ld_acc<8>(arow + (BN + j) * 4, tv);
-          if (p.ln_cl != nullptr) {
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj)
-              tl[jj] = (jj < p.lora_r) ? fmaf(__uint_as_float(tv[jj]), ln_rstd,
-                                              fmaf(-ln_rm, __ldg(p.ln_cl + j + jj), __ldg(p.ln_dl + j + jj))) * lscale
-                                       : 0.f;
-          } else {
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) tl[jj] = __uint_as_float(tv[jj]) * lscale;
-          }
+          load_t8(grp * p.lora_r, p.lora_r);
         }
         float f[16];
 #pragma unroll
@@ -517,10 +533,20 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
         }
         if (has_lora) {
           const uint32_t up = ubuf + sub * 16 * p.lora_r * 4;
-          if (p.lora_r == 4)
+          if (p.lora_r == 4) {
             lora_apply<4>(f, tl, up);
-          else
+          } else if (p.lora_r == 8) {
             lora_apply<8>(f, tl, up);
+          } else {
+            // rank 16: t is re-read for every 16 columns, ranks 0..7 then 8..15, so that the epilogue holds no more
+            // registers than at rank 8 (the 96-register instantiations would spill); each element still adds its
+            // terms in rank order
+            const int j = (n / p.lora_group_n) * 16;
+            load_t8(j, 8);
+            lora_apply<16, 2>(f, tl, up);
+            load_t8(j + 8, 8);
+            lora_apply<16, 2>(f, tl, up + 32);
+          }
         }
         if (p.flags & SB200_EPI_BIAS) add_bf16x16(f, p.bias + n);
         if (rb) add_bf16x16(f, rb + n);
@@ -956,9 +982,10 @@ static bool pairs_always() {
 static bool bn_supported(int bn) { return bn == 64 || bn == 128 || bn == kWideBN; }
 
 // gemm_wide_kernel takes W with a multiple of 256 rows (with GEGLU: 128 rows per half, so a tile writes 128 output
-// columns), single CTAs, and none of LayerNorm fold and row statistics.
-static bool wide_eligible(int N, int ctas, bool lnfold, bool rowstats) {
-  return N % kWideBN == 0 && ctas == 1 && !lnfold && !rowstats;
+// columns), single CTAs, none of LayerNorm fold and row statistics, and LoRA of rank 4 or 8 in at most 32 rows.
+static bool wide_lora_ok(int lora_r, int lora_rt) { return lora_rt == 0 || (lora_rt <= 32 && lora_r <= 8); }
+static bool wide_eligible(int N, int ctas, bool lnfold, bool rowstats, int lora_r, int lora_rt) {
+  return N % kWideBN == 0 && ctas == 1 && !lnfold && !rowstats && wide_lora_ok(lora_r, lora_rt);
 }
 
 // Tile width from a cost model in SM cycles.  A 128 x bn tile's 64-deep k-block takes 4 bn cycles of tensor work (m64
@@ -987,14 +1014,14 @@ constexpr double kWidePerKb = 136.0;
 constexpr double kWideTile = 6500.0;
 constexpr double kWideLoraTile = 40000.0;
 constexpr double kWideFixed = 1500.0;
-static TileChoice pick_tile(int ncols, int num_sms, int kblocks, int lora_rt, int force_ctas, int sub_tiles, int flags,
-                            bool lnfold, bool rowstats) {
+static TileChoice pick_tile(int ncols, int num_sms, int kblocks, int lora_r, int lora_rt, int force_ctas, int sub_tiles,
+                            int flags, bool lnfold, bool rowstats) {
   double best = -1;
   TileChoice bc{1, 64};
   const int ctas = force_ctas ? force_ctas : (pairs_always() ? 2 : 1);
   const bool geglu = (flags & SB200_EPI_GEGLU) != 0;
   const double epi_per_col = 21.0 + ((flags & SB200_EPI_RESID) ? 7.5 : 0.0) + (lora_rt ? 9.0 : 0.0) + (geglu ? 15.0 : 0.0);
-  const int max_bn = wide_eligible(ncols, ctas, lnfold, rowstats) ? kWideBN : 128;
+  const int max_bn = wide_eligible(ncols, ctas, lnfold, rowstats, lora_r, lora_rt) ? kWideBN : 128;
   for (int bn = 64; bn <= max_bn; bn *= 2) {
     const long tiles = static_cast<long>(sub_tiles) * ((ncols + bn - 1) / bn);
     const long load = (tiles + num_sms - 1) / num_sms;
@@ -1119,6 +1146,8 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
     p.ring_bytes = stages * p.stage_bytes + epi;
     const int smem = kBarRegion + kAlignSlack + p.ring_bytes;
     pdl_hint() = p.num_m_tiles * p.num_n_tiles <= 2 * ctx->num_sms;
+    SB200_REQUIRE(wide_lora_ok(p.lora_r, rt), "gemm: bn=256 takes LoRA of rank 4 or 8 in 16 or 32 rows (r=%d, rt=%d)",
+                  p.lora_r, rt);
     int st;
     switch (rt) {
       case 0: st = launch_gemm_wide<0>(ctx, stream, p, smem); break;
@@ -1140,22 +1169,26 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
   const int smem = kBarRegion + kAlignSlack + p.ring_bytes;
   if (smem > budget) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
   pdl_hint() = grid_ctas <= 2 * ctx->num_sms;
-  const int variant = (ctas == 2 ? 6 : 0) + (p.bn == 128 ? 3 : 0) + (rt == 16 ? 1 : (rt == 32 ? 2 : 0));
+  const int variant = (ctas == 2 ? 8 : 0) + (p.bn == 128 ? 4 : 0) + (rt == 16 ? 1 : rt == 32 ? 2 : rt == 64 ? 3 : 0);
   cudaStream_t s = stream;
   int st;
   switch (variant) {
     case 0: st = launch_gemm_bn<64, 1, 0>(ctx, s, p, smem); break;
     case 1: st = launch_gemm_bn<64, 1, 16>(ctx, s, p, smem); break;
     case 2: st = launch_gemm_bn<64, 1, 32>(ctx, s, p, smem); break;
-    case 3: st = launch_gemm_bn<128, 1, 0>(ctx, s, p, smem); break;
-    case 4: st = launch_gemm_bn<128, 1, 16>(ctx, s, p, smem); break;
-    case 5: st = launch_gemm_bn<128, 1, 32>(ctx, s, p, smem); break;
-    case 6: st = launch_gemm_bn<64, 2, 0>(ctx, s, p, smem); break;
-    case 7: st = launch_gemm_bn<64, 2, 16>(ctx, s, p, smem); break;
-    case 8: st = launch_gemm_bn<64, 2, 32>(ctx, s, p, smem); break;
-    case 9: st = launch_gemm_bn<128, 2, 0>(ctx, s, p, smem); break;
-    case 10: st = launch_gemm_bn<128, 2, 16>(ctx, s, p, smem); break;
-    default: st = launch_gemm_bn<128, 2, 32>(ctx, s, p, smem); break;
+    case 3: st = launch_gemm_bn<64, 1, 64>(ctx, s, p, smem); break;
+    case 4: st = launch_gemm_bn<128, 1, 0>(ctx, s, p, smem); break;
+    case 5: st = launch_gemm_bn<128, 1, 16>(ctx, s, p, smem); break;
+    case 6: st = launch_gemm_bn<128, 1, 32>(ctx, s, p, smem); break;
+    case 7: st = launch_gemm_bn<128, 1, 64>(ctx, s, p, smem); break;
+    case 8: st = launch_gemm_bn<64, 2, 0>(ctx, s, p, smem); break;
+    case 9: st = launch_gemm_bn<64, 2, 16>(ctx, s, p, smem); break;
+    case 10: st = launch_gemm_bn<64, 2, 32>(ctx, s, p, smem); break;
+    case 11: st = launch_gemm_bn<64, 2, 64>(ctx, s, p, smem); break;
+    case 12: st = launch_gemm_bn<128, 2, 0>(ctx, s, p, smem); break;
+    case 13: st = launch_gemm_bn<128, 2, 16>(ctx, s, p, smem); break;
+    case 14: st = launch_gemm_bn<128, 2, 32>(ctx, s, p, smem); break;
+    default: st = launch_gemm_bn<128, 2, 64>(ctx, s, p, smem); break;
   }
   if (st) return st;
   SB200_CUDA_CHECK(cudaGetLastError());
@@ -1164,8 +1197,9 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
 
 static int check_lora(const sb200_lora* l, int N) {
   SB200_REQUIRE(l->down && l->up, "lora: NULL weights");
-  SB200_REQUIRE(l->r == 4 || l->r == 8, "lora: rank %d unsupported by the fused epilogue (4 or 8)", l->r);
-  SB200_REQUIRE(l->rt == 16 || l->rt == 32, "lora: rt must be 16 or 32");
+  SB200_REQUIRE(l->r == 4 || l->r == 8 || l->r == 16,
+                "lora: slot width %d unsupported by the fused epilogue (4, 8 or 16; pad lower ranks with zeros)", l->r);
+  SB200_REQUIRE(l->rt == 16 || l->rt == 32 || l->rt == 64, "lora: rt must be 16, 32 or 64");
   SB200_REQUIRE(l->group_n > 0 && l->group_n % 16 == 0, "lora: group_n must be a multiple of 16");
   const int groups = (N + l->group_n - 1) / l->group_n;
   SB200_REQUIRE(groups * l->r <= l->rt, "lora: %d groups of rank %d exceed rt=%d", groups, l->r, l->rt);
@@ -1313,13 +1347,14 @@ extern "C" int sb200_gemm_ln(void* handle, void* stream, const void* x0, int ldx
   }
   int bn, force_ctas;
   decode_bn(bn_arg, &bn, &force_ctas);
-  TileChoice tc = pick_tile(N, ctx->num_sms, p.kblocks, has_lora ? lora->rt : 0, force_ctas, p.num_sub, flags,
+  TileChoice tc = pick_tile(N, ctx->num_sms, p.kblocks, p.lora_r, p.lora_rt, force_ctas, p.num_sub, flags,
                             ln != nullptr, rowstats != nullptr);
   if (bn > 0) tc.bn = bn;
   if (force_ctas) tc.ctas = force_ctas;
   SB200_REQUIRE(bn_supported(tc.bn), "gemm: bn=%d invalid (64, 128 or 256)", tc.bn);
-  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(N, tc.ctas, ln != nullptr, rowstats != nullptr),
-                "gemm: bn=256 needs N %% 256 == 0 and single CTAs, without lnfold or rowstats (N=%d)", N);
+  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(N, tc.ctas, ln != nullptr, rowstats != nullptr, p.lora_r, p.lora_rt),
+                "gemm: bn=256 needs N %% 256 == 0 and single CTAs, without lnfold, rowstats or LoRA of rank 16 or rt 64 "
+                "(N=%d)", N);
   p.bn = tc.bn;
   p.ncols_out = geglu ? tc.bn / 2 : tc.bn;
   p.num_m_tiles = (p.num_sub + tc.ctas - 1) / tc.ctas;
@@ -1460,13 +1495,14 @@ extern "C" int sb200_conv3x3(void* handle, void* stream, const void* x0, int ldx
   }
   int bn, force_ctas;
   decode_bn(bn_arg, &bn, &force_ctas);
-  TileChoice tc = pick_tile(Cout, ctx->num_sms, p.kblocks, has_lora ? lora->rt : 0, force_ctas, p.num_sub, flags,
-                            false, false);
+  TileChoice tc = pick_tile(Cout, ctx->num_sms, p.kblocks, p.lora_r, p.lora_rt, force_ctas, p.num_sub, flags, false,
+                            false);
   if (bn > 0) tc.bn = bn;
   if (force_ctas) tc.ctas = force_ctas;
   SB200_REQUIRE(bn_supported(tc.bn), "conv3x3: bn=%d invalid (64, 128 or 256)", tc.bn);
-  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(Cout, tc.ctas, false, false),
-                "conv3x3: bn=256 needs Cout %% 256 == 0 and single CTAs (Cout=%d)", Cout);
+  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(Cout, tc.ctas, false, false, p.lora_r, p.lora_rt),
+                "conv3x3: bn=256 needs Cout %% 256 == 0 and single CTAs, without LoRA of rank 16 or rt 64 (Cout=%d)",
+                Cout);
   p.bn = tc.bn;
   p.ncols_out = tc.bn;
   p.num_m_tiles = (p.num_sub + tc.ctas - 1) / tc.ctas;

@@ -6,7 +6,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-from typing import Optional
+from typing import Optional, Tuple
 
 import torch
 
@@ -89,6 +89,23 @@ def _count(name: str = "", flops: float = 0.0) -> None:
         end.record()
         profile_log.append((name or "other", flops, _pending_start, end))
         _pending_start = None
+
+
+LORA_MAX_RANK = 16
+
+
+def lora_slots(r: int, groups: int = 1) -> Tuple[int, int]:
+    """(rp, rt) of `groups` adaptors of rank up to r fused into one call: each adaptor takes a slot of rp = 4, 8 or 16
+    down rows / up columns (the smallest that holds r; the rows and columns beyond r are zero, so the padded terms add
+    exact zeros to every fp32 sum), and the stacked down rows are padded to rt = 16, 32 or 64 (sb200_lora.rt)."""
+    if not 1 <= r <= LORA_MAX_RANK:
+        raise NotImplementedError(f"LoRA rank {r}: the fused kernels support ranks 1-{LORA_MAX_RANK}")
+    rp = next(w for w in (4, 8, 16) if r <= w)
+    need = groups * rp
+    if need > 64:
+        raise NotImplementedError(f"{groups} adaptors of rank {r} in one fused call need {need} > 64 LoRA rows")
+    rt = next(w for w in (16, 32, 64) if need <= w)
+    return rp, rt
 
 
 class Lora:

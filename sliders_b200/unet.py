@@ -404,7 +404,7 @@ class UNet2DConditionModel(nn.Module):
         if ent is None or ent[0] != ver:
             g, b = norm.weight.detach().float(), norm.bias.detach().float()
             down = la.down.float()
-            if ent is None:
+            if ent is None or ent[1].shape != la.down.shape:
                 ent = [ver, torch.empty_like(la.down), torch.empty(down.shape[0], device=down.device),
                        torch.empty(down.shape[0], device=down.device), norm, list(leaves)]
                 self._ln_lora_packs[key] = ent
@@ -424,12 +424,7 @@ class UNet2DConditionModel(nn.Module):
         scales = [float(a.multiplier) * float(a.scale) if a is not None else 0.0 for a in adaptors]
         if all(s == 0.0 for s in scales):
             return None
-        r = max(int(a.lora_dim) for a in adaptors if a is not None)
-        if r not in (4, 8):
-            raise NotImplementedError(f"LoRA rank {r}: the fused epilogue supports ranks 4 and 8")
-        rt = 16 if len(leaves) * r <= 16 else 32
-        if len(leaves) * r > 32:
-            raise NotImplementedError("too many adapted leaves fused into one call")
+        r, rt = ops.lora_slots(max(int(a.lora_dim) for a in adaptors if a is not None), len(leaves))
         nz = [s for s in scales if s != 0.0]
         common = nz[0] if all(abs(s - nz[0]) < 1e-12 for s in nz) else None
         if self._bake_scales:
@@ -447,7 +442,14 @@ class UNet2DConditionModel(nn.Module):
             dev = leaves[0].weight.device
             K = leaves[0].weight[0].numel()
             N = sum(l.weight.shape[0] for l in leaves)
-            if pack.down is None:
+            if pack.down is None or pack.down.shape != (rt, K) or pack.up.shape != (N, r):
+                # adaptor gi takes down rows [gi * r, +r) and up columns [0, r) with r the slot width (ops.lora_slots);
+                # the rows and columns beyond its own rank stay zero
+                if pack.down is not None:  # another slot width: captured graphs hold the old buffers
+                    if self._capturing:
+                        raise RuntimeError("sliders_b200: the LoRA slot width changed while a CUDA graph was captured")
+                    self._graphs.clear()
+                    self.__dict__.pop("_train_graphs", None)
                 pack.down = torch.zeros((rt, K), device=dev, dtype=BF16)
                 pack.up = torch.zeros((N, r), device=dev, dtype=torch.float32)  # sb200_lora.up is fp32
             else:
@@ -804,14 +806,17 @@ class UNet2DConditionModel(nn.Module):
         """(signature, common slider factor).  Which adaptors contribute is baked into a captured graph; when
         every active adaptor has the same multiplier*alpha/rank (the only thing `with network:` /
         `set_lora_slider` can produce, lora.py:249-258) that factor is a device-side scalar and the
-        signature does not depend on it; otherwise the individual factors are part of the signature."""
-        scales = [float(a.multiplier) * float(a.scale) for _, a in self._adapted_leaves()]
+        signature does not depend on it; otherwise the individual factors are part of the signature.  The adaptors'
+        ranks are part of it too: they set the sizes of the packed buffers a graph reads."""
+        adapted = self._adapted_leaves()
+        scales = [float(a.multiplier) * float(a.scale) for _, a in adapted]
+        ranks = tuple(int(a.lora_dim) for _, a in adapted)
         nz = [s for s in scales if s != 0.0]
         if not nz:
-            return (tuple(False for _ in scales), None), None
+            return (tuple(False for _ in scales), ranks, None), None
         if all(abs(s - nz[0]) < 1e-12 for s in nz):
-            return (tuple(s != 0.0 for s in scales), None), nz[0]
-        return (tuple(s != 0.0 for s in scales), tuple(scales)), None
+            return (tuple(s != 0.0 for s in scales), ranks, None), nz[0]
+        return (tuple(s != 0.0 for s in scales), ranks, tuple(scales)), None
 
     def _needs_grad(self) -> bool:
         """True when an active adaptor (multiplier != 0, i.e. inside `with network:`) has trainable weights."""

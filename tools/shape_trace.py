@@ -8,6 +8,7 @@ import collections
 import csv
 import os
 import sys
+import types
 
 import torch
 
@@ -17,6 +18,23 @@ from sliders_b200 import ops  # noqa: E402
 from sliders_b200.unet import UNet2DConditionModel, UNetConfig  # noqa: E402
 
 calls = []  # (kernel_name, description, flops)
+lora_rts = {}  # index in `calls` -> LoRA-down rows (sb200_lora.rt) of a call that carries adaptors
+
+
+def _note_lora(lora):
+    if lora is not None:
+        lora_rts[len(calls) - 1] = lora.rt
+
+
+def _lora_slots(leaves):
+    """Stand-in for UNet2DConditionModel._lora: the (slot width r, rt) that ops.lora_slots gives the call's adaptors."""
+    from sliders_b200.unet import _adaptor_of
+
+    ranks = [int(a.lora_dim) for a in map(_adaptor_of, leaves) if a is not None]
+    if not ranks:
+        return None
+    r, rt = ops.lora_slots(max(ranks), len(leaves))
+    return types.SimpleNamespace(r=r, rt=rt)
 
 
 def _meta(*shape):
@@ -32,6 +50,7 @@ def gemm(x, w, *, bias=None, rowbias=None, rows_per_batch=1, resid=None, geglu=F
                                  ("S", x1 is not None), ("N", ln is not None), ("s", rowstats is not None)) if f)
     ops.last_rowstats_parts = 1
     calls.append(("gemm_kernel", f"gemm M{M} N{N} K{K} {tag}", 2.0 * M * N * K))
+    _note_lora(lora)
     return _meta(M, N // 2 if geglu else N)
 
 
@@ -43,6 +62,7 @@ def conv3x3(x0, w, *, x1=None, stride=1, bias=None, rowbias=None, resid=None, lo
                                  ("S", x1 is not None)) if f)
     calls.append(("gemm_kernel", f"conv {H}x{W} C{C0 + C1}->{Cout} s{stride} {tag} (M{B * H * W // stride ** 2} K{9 * (C0 + C1)})",
                   2.0 * B * (H // stride) * (W // stride) * Cout * 9 * (C0 + C1)))
+    _note_lora(lora)
     return _meta(B, H // stride, W // stride, Cout)
 
 
@@ -74,6 +94,7 @@ def layernorm(x, gamma, beta, eps=1e-5):
 def small_linear(x, w, bias=None, *, act_in=False, act_out=0, lora=None, resid=None):
     tag = " L" if lora is not None else ""
     calls.append(("small_linear_kernel", f"small_linear M{x.shape[0]} N{w.shape[0]} K{x.shape[1]}{tag}", 0.0))
+    _note_lora(lora)
     return _meta(x.shape[0], w.shape[0])
 
 
@@ -100,10 +121,12 @@ def upsample2x(x):
     return _meta(B, 2 * H, 2 * W, C)
 
 
-def trace(batch, with_lora=True, train=False, extra_targets=()):
+def trace(batch, with_lora=True, train=False, extra_targets=(), rank=4):
     """The launch plan of one SDXL forward: the inference walk, or with `train` the training walk (tape kept).  The
-    LoRA network is `noxattn` on the default targets plus the conv targets (c3lier) plus `extra_targets`."""
+    LoRA network is `noxattn` of rank `rank` on the default targets plus the conv targets (c3lier) plus
+    `extra_targets`; `lora_rts` then maps each call that carries adaptors to its LoRA-down rows."""
     calls.clear()
+    lora_rts.clear()
     for name in ("gemm", "conv3x3", "attention", "geglu", "groupnorm", "layernorm", "small_linear", "sinusoid",
                  "conv_in", "conv_out", "upsample2x"):
         setattr(ops, name, globals()[name])
@@ -113,13 +136,12 @@ def trace(batch, with_lora=True, train=False, extra_targets=()):
         if with_lora:
             saved = list(plora.DEFAULT_TARGET_REPLACE)
             plora.DEFAULT_TARGET_REPLACE += plora.UNET_TARGET_REPLACE_MODULE_CONV + list(extra_targets)
-            net = plora.LoRANetwork(unet, rank=4, multiplier=1.0, alpha=1.0, train_method="noxattn")
+            net = plora.LoRANetwork(unet, rank=rank, multiplier=1.0, alpha=1.0, train_method="noxattn")
             del plora.DEFAULT_TARGET_REPLACE[len(saved):]
         unet._ln_pack = lambda norm, leaves: (_meta(sum(l.weight.shape[0] for l in leaves), leaves[0].weight.shape[1]), None, None)
         unet._ln_lora = lambda norm, leaves: (unet._lora(leaves), None, None)
         ops.LnFold = lambda *a, **k: object()
-        unet._lora = lambda leaves: (object() if any(__import__("sliders_b200.unet", fromlist=["_adaptor_of"])._adaptor_of(l)
-                                                     is not None for l in leaves) else None)
+        unet._lora = _lora_slots
         x = torch.empty(batch, 4, 128, 128, dtype=torch.float32)
         t = torch.empty(batch, dtype=torch.float32)
         ehs = torch.empty(batch, 77, 2048, dtype=torch.bfloat16)
