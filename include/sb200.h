@@ -83,36 +83,6 @@ int sb200_gemm(void* handle, void* stream, const void* x0, int ldx0, const void*
                const void* bias, const void* rowbias, int rows_per_batch, const void* resid, int ldr,
                const sb200_lora* lora, int bn);
 
-/* LayerNorm folded into the projection that consumes it (BasicTransformerBlock: norm1 -> attn1.to_q|k|v, norm2 ->
- * attn2.to_q, norm3 -> ff GEGLU; diffusers models/attention.py).  With W' = W * gamma (per input column),
- *   LN(x) . W^T + b  =  rstd[m] * (x . W'^T)[m, n]  -  rstd[m] * mean[m] * c[n]  +  d[n],
- *   c[n] = sum_k W'[n, k],  d[n] = sum_k beta[k] W[n, k] + b[n],
- * so the kernel multiplies the UN-normalised rows by W' and its epilogue applies the per-row (mean, rstd), which it
- * derives from per-row partial sums (sum x, sum x^2) that the GEMM producing x left behind (`rowstats` below).  The
- * LoRA-down rows are folded the same way (c_lora / d_lora over the rt stacked rows). */
-typedef struct sb200_lnfold {
-  const float* stats;   /* [parts, M, 2] partial (sum, sum of squares) per row of x, fp32 (part-major) */
-  int parts;
-  int C;                /* row length of x the statistics run over (= K) */
-  float eps;
-  const float* c;       /* [N] */
-  const float* d;       /* [N]  (includes the bias: call without SB200_EPI_BIAS) */
-  const float* c_lora;  /* [rt] or NULL */
-  const float* d_lora;  /* [rt] or NULL */
-} sb200_lnfold;
-
-/* sb200_gemm with the two LayerNorm-fusion hooks:
- *   ln        (optional) this projection consumes LN(x): see sb200_lnfold;
- *   rowstats  (optional) [rowstats_cap, M, 2] fp32: the epilogue leaves per-row partial (sum, sum of squares) of the
- *             bf16 values it writes, one slot per N tile (part-major); *rowstats_parts receives the number of slots
- *             used per row (<= rowstats_cap, else SB200_ERR_INVALID).  Written without atomics: every slot has one
- *             owner, so the statistics are bit-reproducible. */
-int sb200_gemm_ln(void* handle, void* stream, const void* x0, int ldx0, const void* x1, int ldx1, int K0,
-                  const void* w, int ldw, void* out, int ldo, int M, int N, int K, int flags,
-                  const void* bias, const void* rowbias, int rows_per_batch, const void* resid, int ldr,
-                  const sb200_lora* lora, int bn, const sb200_lnfold* ln, float* rowstats, int rowstats_cap,
-                  int* rowstats_parts);
-
 /* 3x3 convolution, padding 1, stride 1 or 2, as an implicit GEMM over NHWC activations.
  * Replaces: torch Conv2d inside diffusers ResnetBlock2D / Downsample2D / Upsample2D (same call site).
  *   x0/x1: [B, Hin, Win, C0] / [B, Hin, Win, C1] (x1 may be NULL), pixel strides ldx0 / ldx1 elements;

@@ -32,21 +32,6 @@ class LoraArgs(C.Structure):
     ]
 
 
-class LnFoldArgs(C.Structure):
-    """struct sb200_lnfold (include/sb200.h)."""
-
-    _fields_ = [
-        ("stats", C.c_void_p),
-        ("parts", C.c_int),
-        ("C", C.c_int),
-        ("eps", C.c_float),
-        ("c", C.c_void_p),
-        ("d", C.c_void_p),
-        ("c_lora", C.c_void_p),
-        ("d_lora", C.c_void_p),
-    ]
-
-
 _p, _i, _f, _i64, _d = C.c_void_p, C.c_int, C.c_float, C.c_int64, C.c_double
 _LP = C.POINTER(LoraArgs)
 
@@ -57,8 +42,6 @@ SIGNATURES = {
     "sb200_create": [_i, C.POINTER(_p)],
     "sb200_destroy": [_p],
     "sb200_gemm": [_p, _p, _p, _i, _p, _i, _i, _p, _i, _p, _i, _i, _i, _i, _i, _p, _p, _i, _p, _i, _LP, _i],
-    "sb200_gemm_ln": [_p, _p, _p, _i, _p, _i, _i, _p, _i, _p, _i, _i, _i, _i, _i, _p, _p, _i, _p, _i, _LP, _i, _p, _p, _i,
-                      _p],
     "sb200_conv3x3": [_p, _p, _p, _i, _p, _i, _i, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p, _i,
                       _LP, _i],
     "sb200_attention": [_p, _p, _p, _i, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _i, _f, _p],

@@ -10,12 +10,11 @@
 // one more wgmma (N = rt) per k-step accumulates t = A . down^T.
 // Epilogue: both warpgroups park their accumulators in shared memory as an fp32 [128 x (BN + rt)] tile (over the stage
 // ring, which is free once the main loop has ended).  Each thread then owns one row: rank-r LoRA up-projection,
-// LayerNorm fold, bias / time-embedding row bias / GEGLU / residual; residual tiles come in by cp.async and results
-// leave through a swizzled smem staging tile (also in the ring, behind the accumulator tile) so that global accesses
-// are coalesced.
+// bias / time-embedding row bias / GEGLU / residual; residual tiles come in by cp.async and results leave through a
+// swizzled smem staging tile (also in the ring, behind the accumulator tile) so that global accesses are coalesced.
 // Residency: two CTAs per SM wherever 96 registers per thread hold the accumulators without spills (BN = 64 with up
 // to 32 LoRA rows, or no LoRA), so one CTA's prologue and epilogue run while the other's wgmmas keep the tensor cores
-// busy; BN = 128 with LoRA needs ~160 registers and runs one CTA per SM, as do the 64 LoRA rows (rank-16 q|k|v) at
+// busy; BN = 128 with LoRA needs ~120 registers and runs one CTA per SM, as do the 64 LoRA rows (rank-16 q|k|v) at
 // either width.  Each CTA's ring is sized from its share of the SM's shared memory.
 // CTA pairs (kCtas = 2): a cluster of two CTAs on consecutive 128-row tiles of the same N tile.  Each CTA loads half
 // of the W (and LoRA-down) rows of a stage and multicasts them to both, which halves the weight traffic from L2.
@@ -50,7 +49,7 @@ constexpr int kAlignSlack = 1024;     // the dynamic smem base is rounded up to 
 constexpr int kSlab = 32;             // output columns staged per epilogue-warp iteration
 constexpr int kEpiBufBytes = 32 * 64; // [32 rows x 32 cols] bf16
 constexpr int kEpiBytes = kEpiWarps * kEpiBufBytes;  // + kEpiWarps x [32 cols][r] fp32 of lora_up rows with LoRA
-constexpr int kConsumerBar = 5;       // named barrier of the 256 consumer threads (1..4: row-statistics reduction)
+constexpr int kConsumerBar = 1;       // named barrier of the 256 consumer threads
 
 // CTAs per SM an instantiation is compiled for (its launch bounds): under two, ptxas caps a thread at 96 registers,
 // which holds BN = 64 with up to 32 LoRA rows and BN = 128 without them; BN = 128 with LoRA, and 64 LoRA rows at any
@@ -101,16 +100,6 @@ struct GemmParams {
   int lora_r, lora_rt, lora_group_n;
   float lora_scale;
   const float* lora_scale_dev;
-  // LayerNorm folded into this projection (struct sb200_lnfold) / row statistics left for the next one
-  const float* ln_stats;
-  int ln_parts;
-  float ln_inv_c, ln_eps;
-  const float* ln_c;
-  const float* ln_d;
-  const float* ln_cl;
-  const float* ln_dl;
-  float* rs_out;
-  int rs_parts;
   // split-K (sb200_gemm_splitk_f32): grid y = split index; split s runs k-blocks [s * sk_kb, (s + 1) * sk_kb) and stores
   // its raw fp32 tile to sk_ws[s][M][N] instead of running the epilogue
   float* sk_ws;
@@ -242,9 +231,11 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
   const uint32_t bar_full = base;            // S barriers
   const uint32_t bar_empty = base + 8u * S;  // S barriers
   const uint32_t tiles = base + kBarRegion;
-  // launch_gemm runs every LoRA call on an RT > 0 instantiation, so the RT = 0 ones carry no LoRA code
+  // launch_gemm runs every LoRA call on an RT > 0 instantiation, so the RT = 0 ones carry no LoRA code; GEGLU never
+  // comes with LoRA (sb200_gemm refuses it), so the RT > 0 ones carry no GEGLU code, whose gate registers would
+  // otherwise stay live across the LoRA update and spill the 96-register instantiations
   const bool has_lora = RT != 0 && (p.flags & SB200_EPI_LORA) != 0;
-  const bool geglu = (p.flags & SB200_EPI_GEGLU) != 0;
+  const bool geglu = RT == 0 && (p.flags & SB200_EPI_GEGLU) != 0;
   constexpr int rt = RT;  // LoRA-down rows of a stage (0 without LoRA)
 
   if (warp == 0 && lane == 0) {
@@ -426,22 +417,6 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
       }
     }
     const bool row_ok = my_row >= 0;
-    // LayerNorm fold: (mean, rstd) of this thread's row of x from the producer's partial sums, part-major
-    // [parts][M][2]: the 32 rows of a warp read consecutive addresses
-    float ln_rstd = 1.f, ln_rm = 0.f;
-    if (p.ln_stats != nullptr && row_ok) {
-      const float2* ln_sp = reinterpret_cast<const float2*>(p.ln_stats) + my_row;
-      float s1 = 0.f, s2 = 0.f;
-      for (int i = 0; i < p.ln_parts; ++i) {
-        const float2 v2 = __ldg(ln_sp + static_cast<size_t>(i) * p.M);
-        s1 += v2.x;
-        s2 += v2.y;
-      }
-      const float mean = s1 * p.ln_inv_c;
-      ln_rstd = rsqrtf(fmaxf(s2 * p.ln_inv_c - mean * mean, 0.f) + p.ln_eps);
-      ln_rm = ln_rstd * mean;
-    }
-    float rs1 = 0.f, rs2 = 0.f;  // row statistics of what this warp writes in this tile
     const int n_base = nt * p.ncols_out;
     const int ncols_valid = min(p.ncols_out, p.Nout - n_base);
     const int nslabs = (ncols_valid + kSlab - 1) / kSlab;
@@ -478,21 +453,13 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
         (p.flags & SB200_EPI_ROWBIAS) ? p.rowbias + static_cast<size_t>(row_ok ? my_batch : 0) * p.Nout : nullptr;
     float tl[8];
     int group_lo = 0, group_hi = 0;  // output-column range of the adaptor whose t = A.down^T is held in tl
-    // tl = lscale * (LayerNorm-folded) t, from the 8 t columns of this row at column j of the adaptor's r; columns
-    // r.. of the 8 are 0 (rank 4: the row's 4 padding floats cover the last adaptor's read)
-    auto load_t8 = [&](int j, int r_left) {
+    // tl = lscale * t, from the 8 t columns of this row starting at column j; rank 4 uses the first 4 (the row's 4
+    // padding floats cover the last adaptor's read)
+    auto load_t8 = [&](int j) {
       uint32_t tv[8];
       ld_acc<8>(arow + (BN + j) * 4, tv);
-      if (p.ln_cl != nullptr) {
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj)
-          tl[jj] = (jj < r_left) ? fmaf(__uint_as_float(tv[jj]), ln_rstd,
-                                        fmaf(-ln_rm, __ldg(p.ln_cl + j + jj), __ldg(p.ln_dl + j + jj))) * lscale
-                                 : 0.f;
-      } else {
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj) tl[jj] = __uint_as_float(tv[jj]) * lscale;
-      }
+      for (int jj = 0; jj < 8; ++jj) tl[jj] = __uint_as_float(tv[jj]) * lscale;
     };
     const uint32_t swz = static_cast<uint32_t>((lane >> 1) & 3);
     for (int k = 0; k < my_slabs; ++k) {
@@ -510,23 +477,11 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
           const int grp = n / p.lora_group_n;
           group_lo = grp * p.lora_group_n;
           group_hi = group_lo + p.lora_group_n;
-          load_t8(grp * p.lora_r, p.lora_r);
+          load_t8(grp * p.lora_r);
         }
         float f[16];
 #pragma unroll
         for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]);
-        if (p.ln_stats != nullptr) {
-          // LN(x) . W^T + b = rstd * acc - rstd * mean * c[n] + d[n]
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            const float4 cc = __ldg(reinterpret_cast<const float4*>(p.ln_c + n) + j4);
-            const float4 dd = __ldg(reinterpret_cast<const float4*>(p.ln_d + n) + j4);
-            f[4 * j4 + 0] = fmaf(f[4 * j4 + 0], ln_rstd, fmaf(-ln_rm, cc.x, dd.x));
-            f[4 * j4 + 1] = fmaf(f[4 * j4 + 1], ln_rstd, fmaf(-ln_rm, cc.y, dd.y));
-            f[4 * j4 + 2] = fmaf(f[4 * j4 + 2], ln_rstd, fmaf(-ln_rm, cc.z, dd.z));
-            f[4 * j4 + 3] = fmaf(f[4 * j4 + 3], ln_rstd, fmaf(-ln_rm, cc.w, dd.w));
-          }
-        }
         if (staged && sub == 0) {  // this slab's residual / lora_up rows have landed
           cp_async_wait<0>();
           __syncwarp();
@@ -540,11 +495,13 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
           } else {
             // rank 16: t is re-read for every 16 columns, ranks 0..7 then 8..15, so that the epilogue holds no more
             // registers than at rank 8 (the 96-register instantiations would spill); each element still adds its
-            // terms in rank order
+            // terms in rank order.  The __syncwarp keeps ptxas from hoisting the second half's shared-memory loads
+            // over the first half's FMAs, which would hold both halves live again.
             const int j = (n / p.lora_group_n) * 16;
-            load_t8(j, 8);
+            load_t8(j);
             lora_apply<16, 2>(f, tl, up);
-            load_t8(j + 8, 8);
+            __syncwarp();
+            load_t8(j + 8);
             lora_apply<16, 2>(f, tl, up + 32);
           }
         }
@@ -554,11 +511,6 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
           float gb[16];
 #pragma unroll
           for (int j = 0; j < 16; ++j) gb[j] = __uint_as_float(g[j]);
-          if (p.ln_stats != nullptr) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              gb[j] = fmaf(gb[j], ln_rstd, fmaf(-ln_rm, __ldg(p.ln_c + p.Nout + n + j), __ldg(p.ln_d + p.Nout + n + j)));
-          }
           if (p.flags & SB200_EPI_BIAS) add_bf16x16(gb, p.bias + p.Nout + n);
 #pragma unroll
           for (int j = 0; j < 16; ++j) f[j] *= gelu_erf_f(gb[j]);
@@ -575,14 +527,6 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
           const uint32_t rw[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
 #pragma unroll
           for (int j = 0; j < 8; ++j) o[j] = add_bf16x2(o[j], rw[j]);
-        }
-        if (p.rs_out != nullptr) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float lo = bf16_lo(o[j]), hi = bf16_hi(o[j]);
-            rs1 += lo + hi;
-            rs2 = fmaf(lo, lo, fmaf(hi, hi, rs2));
-          }
         }
         st_shared_v4(a0, make_uint4(o[0], o[1], o[2], o[3]));
         st_shared_v4(a1, make_uint4(o[4], o[5], o[6], o[7]));
@@ -605,27 +549,6 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
         prefetch_resid(ncol0, min(kSlab, ncols_valid - ncol0));
       }
     }
-    if (p.rs_out != nullptr) {
-      // The kEpiPerQuarter warps of a quarter hold partial sums of the SAME 32 rows (different slabs): combine them
-      // through the quarter's first warp's staging buffer (free after its last copy-out), so that a row has one slot
-      // per N tile.  Named barrier 1 + q, 32 * kEpiPerQuarter threads.
-      const uint32_t red = epi + static_cast<uint32_t>(q) * (kEpiBufBytes + p.up_buf_bytes);
-      asm volatile("bar.sync %0, %1;" ::"r"(1 + q), "r"(32 * kEpiPerQuarter) : "memory");  // first warp done with its buffer
-      if (hsel != 0)
-        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(red + ((hsel - 1) * 32 + lane) * 8), "f"(rs1), "f"(rs2)
-                     : "memory");
-      asm volatile("bar.sync %0, %1;" ::"r"(1 + q), "r"(32 * kEpiPerQuarter) : "memory");
-      if (hsel == 0) {
-#pragma unroll
-        for (int w = 0; w < kEpiPerQuarter - 1; ++w) {
-          float a, b;
-          asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(a), "=f"(b) : "r"(red + (w * 32 + lane) * 8));
-          rs1 += a;
-          rs2 += b;
-        }
-        if (row_ok) reinterpret_cast<float2*>(p.rs_out)[static_cast<size_t>(nt) * p.M + my_row] = make_float2(rs1, rs2);
-      }
-    }
   }
 
   if constexpr (kCtas == 2) {
@@ -646,8 +569,8 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
 // run on across tiles.  The epilogue works on the accumulator registers: per element it applies, in gemm_kernel's
 // order and with its expressions, the LoRA update, bias, row bias and GEGLU, rounds to bf16, adds the residual in bf16,
 // and leaves through a swizzled staging buffer (two per warpgroup, 64 rows x 64 columns each) with coalesced stores.
-// Only t = A.down^T and the tile's lora_up rows are staged in shared memory.  No LayerNorm fold, row statistics,
-// split-K or CTA pairs: those stay on gemm_kernel.
+// Only t = A.down^T and the tile's lora_up rows are staged in shared memory.  No split-K or CTA pairs: those stay on
+// gemm_kernel.
 constexpr int kWideBN = 256;
 constexpr int kWideThreads = 384;
 constexpr int kWideChunk = 64;                        // output columns per staging buffer
@@ -982,10 +905,10 @@ static bool pairs_always() {
 static bool bn_supported(int bn) { return bn == 64 || bn == 128 || bn == kWideBN; }
 
 // gemm_wide_kernel takes W with a multiple of 256 rows (with GEGLU: 128 rows per half, so a tile writes 128 output
-// columns), single CTAs, none of LayerNorm fold and row statistics, and LoRA of rank 4 or 8 in at most 32 rows.
+// columns), single CTAs, and LoRA of rank 4 or 8 in at most 32 rows.
 static bool wide_lora_ok(int lora_r, int lora_rt) { return lora_rt == 0 || (lora_rt <= 32 && lora_r <= 8); }
-static bool wide_eligible(int N, int ctas, bool lnfold, bool rowstats, int lora_r, int lora_rt) {
-  return N % kWideBN == 0 && ctas == 1 && !lnfold && !rowstats && wide_lora_ok(lora_r, lora_rt);
+static bool wide_eligible(int N, int ctas, int lora_r, int lora_rt) {
+  return N % kWideBN == 0 && ctas == 1 && wide_lora_ok(lora_r, lora_rt);
 }
 
 // Tile width from a cost model in SM cycles.  A 128 x bn tile's 64-deep k-block takes 4 bn cycles of tensor work (m64
@@ -1015,13 +938,13 @@ constexpr double kWideTile = 6500.0;
 constexpr double kWideLoraTile = 40000.0;
 constexpr double kWideFixed = 1500.0;
 static TileChoice pick_tile(int ncols, int num_sms, int kblocks, int lora_r, int lora_rt, int force_ctas, int sub_tiles,
-                            int flags, bool lnfold, bool rowstats) {
+                            int flags) {
   double best = -1;
   TileChoice bc{1, 64};
   const int ctas = force_ctas ? force_ctas : (pairs_always() ? 2 : 1);
   const bool geglu = (flags & SB200_EPI_GEGLU) != 0;
   const double epi_per_col = 21.0 + ((flags & SB200_EPI_RESID) ? 7.5 : 0.0) + (lora_rt ? 9.0 : 0.0) + (geglu ? 15.0 : 0.0);
-  const int max_bn = wide_eligible(ncols, ctas, lnfold, rowstats, lora_r, lora_rt) ? kWideBN : 128;
+  const int max_bn = wide_eligible(ncols, ctas, lora_r, lora_rt) ? kWideBN : 128;
   for (int bn = 64; bn <= max_bn; bn *= 2) {
     const long tiles = static_cast<long>(sub_tiles) * ((ncols + bn - 1) / bn);
     const long load = (tiles + num_sms - 1) / num_sms;
@@ -1299,15 +1222,6 @@ extern "C" int sb200_gemm(void* handle, void* stream, const void* x0, int ldx0, 
                           int K0, const void* w, int ldw, void* out, int ldo, int M, int N, int K,
                           int flags, const void* bias, const void* rowbias, int rows_per_batch,
                           const void* resid, int ldr, const sb200_lora* lora, int bn_arg) {
-  return sb200_gemm_ln(handle, stream, x0, ldx0, x1, ldx1, K0, w, ldw, out, ldo, M, N, K, flags, bias, rowbias,
-                       rows_per_batch, resid, ldr, lora, bn_arg, nullptr, nullptr, 0, nullptr);
-}
-
-extern "C" int sb200_gemm_ln(void* handle, void* stream, const void* x0, int ldx0, const void* x1, int ldx1,
-                             int K0, const void* w, int ldw, void* out, int ldo, int M, int N, int K,
-                             int flags, const void* bias, const void* rowbias, int rows_per_batch,
-                             const void* resid, int ldr, const sb200_lora* lora, int bn_arg,
-                             const sb200_lnfold* ln, float* rowstats, int rowstats_cap, int* rowstats_parts) {
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx, "gemm: NULL handle");
   SB200_REQUIRE(M > 0 && N > 0 && K > 0, "gemm: bad dims M=%d N=%d K=%d", M, N, K);
@@ -1347,14 +1261,12 @@ extern "C" int sb200_gemm_ln(void* handle, void* stream, const void* x0, int ldx
   }
   int bn, force_ctas;
   decode_bn(bn_arg, &bn, &force_ctas);
-  TileChoice tc = pick_tile(N, ctx->num_sms, p.kblocks, p.lora_r, p.lora_rt, force_ctas, p.num_sub, flags,
-                            ln != nullptr, rowstats != nullptr);
+  TileChoice tc = pick_tile(N, ctx->num_sms, p.kblocks, p.lora_r, p.lora_rt, force_ctas, p.num_sub, flags);
   if (bn > 0) tc.bn = bn;
   if (force_ctas) tc.ctas = force_ctas;
   SB200_REQUIRE(bn_supported(tc.bn), "gemm: bn=%d invalid (64, 128 or 256)", tc.bn);
-  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(N, tc.ctas, ln != nullptr, rowstats != nullptr, p.lora_r, p.lora_rt),
-                "gemm: bn=256 needs N %% 256 == 0 and single CTAs, without lnfold, rowstats or LoRA of rank 16 or rt 64 "
-                "(N=%d)", N);
+  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(N, tc.ctas, p.lora_r, p.lora_rt),
+                "gemm: bn=256 needs N %% 256 == 0 and single CTAs, without LoRA of rank 16 or rt 64 (N=%d)", N);
   p.bn = tc.bn;
   p.ncols_out = geglu ? tc.bn / 2 : tc.bn;
   p.num_m_tiles = (p.num_sub + tc.ctas - 1) / tc.ctas;
@@ -1366,26 +1278,6 @@ extern "C" int sb200_gemm_ln(void* handle, void* stream, const void* x0, int ldx
   p.ldr = ldr;
   p.out = static_cast<__nv_bfloat16*>(out);
   p.ldo = ldo;
-  if (ln != nullptr) {
-    SB200_REQUIRE(ln->stats && ln->parts > 0 && ln->C == K && ln->c && ln->d, "gemm: lnfold arguments (C must equal K)");
-    SB200_REQUIRE(!(flags & SB200_EPI_BIAS), "gemm: with lnfold the bias lives in d[]");
-    SB200_REQUIRE(!has_lora || (ln->c_lora && ln->d_lora), "gemm: lnfold with LoRA needs c_lora / d_lora");
-    p.ln_stats = ln->stats;
-    p.ln_parts = ln->parts;
-    p.ln_inv_c = 1.0f / static_cast<float>(ln->C);
-    p.ln_eps = ln->eps;
-    p.ln_c = ln->c;
-    p.ln_d = ln->d;
-    p.ln_cl = has_lora ? ln->c_lora : nullptr;
-    p.ln_dl = has_lora ? ln->d_lora : nullptr;
-  }
-  if (rowstats != nullptr) {
-    SB200_REQUIRE(!geglu, "gemm: rowstats of a GEGLU output are not supported");
-    p.rs_parts = p.num_n_tiles;
-    SB200_REQUIRE(p.rs_parts <= rowstats_cap, "gemm: rowstats needs %d slots per row, capacity %d", p.rs_parts, rowstats_cap);
-    p.rs_out = rowstats;
-    if (rowstats_parts) *rowstats_parts = p.rs_parts;
-  }
 
   int st;
   {
@@ -1495,12 +1387,11 @@ extern "C" int sb200_conv3x3(void* handle, void* stream, const void* x0, int ldx
   }
   int bn, force_ctas;
   decode_bn(bn_arg, &bn, &force_ctas);
-  TileChoice tc = pick_tile(Cout, ctx->num_sms, p.kblocks, p.lora_r, p.lora_rt, force_ctas, p.num_sub, flags, false,
-                            false);
+  TileChoice tc = pick_tile(Cout, ctx->num_sms, p.kblocks, p.lora_r, p.lora_rt, force_ctas, p.num_sub, flags);
   if (bn > 0) tc.bn = bn;
   if (force_ctas) tc.ctas = force_ctas;
   SB200_REQUIRE(bn_supported(tc.bn), "conv3x3: bn=%d invalid (64, 128 or 256)", tc.bn);
-  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(Cout, tc.ctas, false, false, p.lora_r, p.lora_rt),
+  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(Cout, tc.ctas, p.lora_r, p.lora_rt),
                 "conv3x3: bn=256 needs Cout %% 256 == 0 and single CTAs, without LoRA of rank 16 or rt 64 (Cout=%d)",
                 Cout);
   p.bn = tc.bn;

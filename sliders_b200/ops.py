@@ -11,7 +11,7 @@ from typing import Optional, Tuple
 import torch
 
 from . import _cabi
-from ._cabi import EPI_BIAS, EPI_GEGLU, EPI_LORA, EPI_RESID, EPI_ROWBIAS, LnFoldArgs, LoraArgs
+from ._cabi import EPI_BIAS, EPI_GEGLU, EPI_LORA, EPI_RESID, EPI_ROWBIAS, LoraArgs
 
 BF16 = torch.bfloat16
 
@@ -124,35 +124,10 @@ class Lora:
         return C.byref(self._c)
 
 
-class LnFold:
-    """LayerNorm folded into the consuming projection (struct sb200_lnfold): `stats` [M, parts, 2] fp32 partial row
-    sums left by the GEMM that produced x (its `rowstats=`), `c` / `d` the per-output-column terms of the fold."""
-
-    __slots__ = ("keep", "_c")
-
-    def __init__(self, stats: torch.Tensor, parts: int, C_: int, eps: float, c: torch.Tensor, d: torch.Tensor,
-                 c_lora: Optional[torch.Tensor] = None, d_lora: Optional[torch.Tensor] = None):
-        self.keep = (stats, c, d, c_lora, d_lora)
-        self._c = LnFoldArgs(stats.data_ptr(), int(parts), int(C_), float(eps), c.data_ptr(), d.data_ptr(),
-                             c_lora.data_ptr() if c_lora is not None else None,
-                             d_lora.data_ptr() if d_lora is not None else None)
-
-    def ref(self):
-        return C.byref(self._c)
-
-
-# slots per row the last `gemm(..., rowstats=...)` call wrote (host-side value, fixed by the tile choice)
-last_rowstats_parts = 0
-_parts_slot = C.c_int(0)  # module lifetime: recorded calls (bench.py's class graphs) re-issue with this pointer
-
-
 def gemm(x: torch.Tensor, w: torch.Tensor, *, bias=None, rowbias=None, rows_per_batch: int = 1, resid=None,
          geglu: bool = False, lora: Optional[Lora] = None, x1: Optional[torch.Tensor] = None,
-         out: Optional[torch.Tensor] = None, bn: int = 0, ln: Optional[LnFold] = None,
-         rowstats: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """out[M,N] = epilogue([x | x1] @ w.T): one wgmma `gemm_kernel` launch.  `ln`: the rows of x are un-normalised and
-    w is gamma-scaled (LayerNorm fold); `rowstats` [M, cap, 2] fp32: leave per-row partial (sum, sum of squares) of the
-    output for a later `ln` (the number of slots used is `ops.last_rowstats_parts`)."""
+         out: Optional[torch.Tensor] = None, bn: int = 0) -> torch.Tensor:
+    """out[M,N] = epilogue([x | x1] @ w.T): one wgmma `gemm_kernel` launch."""
     M, K0 = x.shape
     N, K = w.shape
     flags = 0
@@ -170,22 +145,10 @@ def gemm(x: torch.Tensor, w: torch.Tensor, *, bias=None, rowbias=None, rows_per_
     if out is None:
         out = torch.empty((M, nout), device=x.device, dtype=BF16)
     lib = _begin()
-    if ln is None and rowstats is None:
-        _cabi.check(lib.sb200_gemm(
-            _ctx(x), _stream(), _p(x), x.stride(0), _p(x1), x1.stride(0) if x1 is not None else 0, K0,
-            _p(w), w.stride(0), _p(out), out.stride(0), M, N, K, flags, _p(bias), _p(rowbias), rows_per_batch,
-            _p(resid), resid.stride(0) if resid is not None else 0, lora.ref() if lora is not None else None, bn))
-    else:
-        global last_rowstats_parts
-        parts = _parts_slot
-        _cabi.check(lib.sb200_gemm_ln(
-            _ctx(x), _stream(), _p(x), x.stride(0), _p(x1), x1.stride(0) if x1 is not None else 0, K0,
-            _p(w), w.stride(0), _p(out), out.stride(0), M, N, K, flags, _p(bias), _p(rowbias), rows_per_batch,
-            _p(resid), resid.stride(0) if resid is not None else 0, lora.ref() if lora is not None else None, bn,
-            ln.ref() if ln is not None else None, _p(rowstats),
-            rowstats.numel() // (2 * M) if rowstats is not None else 0, C.cast(C.pointer(parts), C.c_void_p)))
-        if rowstats is not None:
-            last_rowstats_parts = parts.value
+    _cabi.check(lib.sb200_gemm(
+        _ctx(x), _stream(), _p(x), x.stride(0), _p(x1), x1.stride(0) if x1 is not None else 0, K0,
+        _p(w), w.stride(0), _p(out), out.stride(0), M, N, K, flags, _p(bias), _p(rowbias), rows_per_batch,
+        _p(resid), resid.stride(0) if resid is not None else 0, lora.ref() if lora is not None else None, bn))
     _count("gemm", 2.0 * M * N * K)
     return out
 

@@ -302,12 +302,6 @@ class UNet2DConditionModel(nn.Module):
         # engine state (not part of the state dict)
         self._packed: Dict[int, torch.Tensor] = {}
         self._lora_packs: Dict[tuple, _LoraPack] = {}
-        self._ln_lora_packs: Dict[tuple, list] = {}
-        self.fuse_layernorm_min_c = 0
-        # inference forward with LayerNorm folded into the consuming projection (sb200_gemm_ln): parity-tested, 798 instead
-        # of 1 008 launches, but 1-1.5 % SLOWER than the separate launches in three same-box A/Bs (the extra epilogue work
-        # lands on epilogue-bound tiles; profiles/r02_lnfold_ab.log), so it stays off by default
-        self.fuse_layernorm = False
         self._graphs: Dict[tuple, "_CapturedForward"] = {}
         self._slider_scale_dev: Optional[torch.Tensor] = None
         self.use_cuda_graph = False
@@ -330,7 +324,6 @@ class UNet2DConditionModel(nn.Module):
         self.__dict__.pop("_leaf_by_id", None)
         self._packed.clear()
         self._lora_packs.clear()
-        self._ln_lora_packs.clear()
         self._graphs.clear()
         self.__dict__.pop("_train_graphs", None)
         self._slider_scale_dev = None
@@ -375,44 +368,6 @@ class UNet2DConditionModel(nn.Module):
             w = torch.cat([l.weight.detach().to(BF16) for l in leaves], dim=0).contiguous()
             self._packed[key] = w
         return w
-
-    # ---- LayerNorm folded into the consuming projection (inference forward) ------------------------------
-    def _ln_pack(self, norm: nn.Module, leaves: List[nn.Module]):
-        """(W' [N,K] bf16 = W * gamma, c [N] fp32 = row sums of W', d [N] fp32 = W . beta + bias) of the projection(s)
-        `leaves` that consume LayerNorm `norm` (include/sb200.h: sb200_lnfold).  Frozen weights: packed once."""
-        key = ("lnfold", id(norm)) + tuple(id(l) for l in leaves)
-        v = self._packed.get(key)
-        if v is None:
-            g, b = norm.weight.detach().float(), norm.bias.detach().float()
-            w = torch.cat([l.weight.detach().float() for l in leaves], dim=0)
-            bias = torch.cat([(l.bias.detach().float() if l.bias is not None else
-                               torch.zeros(l.weight.shape[0], device=w.device)) for l in leaves])
-            wp = (w * g[None, :]).to(BF16).contiguous()
-            v = (wp, wp.float().sum(dim=1).contiguous(), (w @ b + bias).contiguous())
-            self._packed[key] = v
-        return v
-
-    def _ln_lora(self, norm: nn.Module, leaves: List[nn.Module]):
-        """The LoRA side inputs of a LayerNorm-folded call: down rows scaled by gamma, plus their (c, d) terms.
-        Re-derived whenever the plain pack changes (an optimizer step, a new slider factor)."""
-        la = self._lora(leaves)
-        if la is None:
-            return None, None, None
-        key = (id(norm),) + tuple(id(l) for l in leaves)
-        ver = (la.down.data_ptr(), la.down._version)
-        ent = self._ln_lora_packs.get(key)
-        if ent is None or ent[0] != ver:
-            g, b = norm.weight.detach().float(), norm.bias.detach().float()
-            down = la.down.float()
-            if ent is None or ent[1].shape != la.down.shape:
-                ent = [ver, torch.empty_like(la.down), torch.empty(down.shape[0], device=down.device),
-                       torch.empty(down.shape[0], device=down.device), norm, list(leaves)]
-                self._ln_lora_packs[key] = ent
-            ent[0] = ver
-            ent[1].copy_((down * g[None, :]).to(BF16))
-            ent[2].copy_(ent[1].float().sum(dim=1))
-            ent[3].copy_(down @ b)
-        return Lora(ent[1], la.up, la.r, la.group_n, la.scale, la.scale_dev), ent[2], ent[3]
 
     # ---- LoRA packing --------------------------------------------------------------------------------
     def _lora(self, leaves: List[nn.Module]) -> Optional[Lora]:
@@ -593,9 +548,7 @@ class UNet2DConditionModel(nn.Module):
         keep = tape is not None
         ws = ops.gn_ws(B, gn.num_groups, x.device) if keep else None
         hn = ops.groupnorm(x, *self._w_norm(gn), gn.num_groups, gn.eps, False, stats_ws=ws).view(B * S, C_)
-        if not keep and self.fuse_layernorm and C_ >= self.fuse_layernorm_min_c:
-            return self._transformer_lnfold(tr, hn, res, ctx, Sctx, kv_all, B, S).view(B, H, W, C_)
-        h = ops.gemm(hn, self._w(tr.proj_in), bias=self._b(tr.proj_in), lora=self._lora([tr.proj_in]))
+        h =ops.gemm(hn, self._w(tr.proj_in), bias=self._b(tr.proj_in), lora=self._lora([tr.proj_in]))
         blocks = []
         for blk in tr.transformer_blocks:
             h1 = h
@@ -621,48 +574,6 @@ class UNet2DConditionModel(nn.Module):
         if keep:
             tape.append(("tr", (tr, x, ops.gn_stats(ws, B, gn.num_groups), hn, blocks, h)))
         return out.view(B, H, W, C_)
-
-    def _transformer_lnfold(self, tr: Transformer2DModel, h, res, ctx, Sctx, kv_all, B, S) -> torch.Tensor:
-        """The same block sequence without LayerNorm launches: every GEMM that writes the residual stream (proj_in, the
-        two attention out-projections, the feed-forward output) leaves per-row partial (sum, sum of squares) of what it
-        wrote, and the projection consuming the LayerNorm of that stream (fused q|k|v, attn2.to_q, the GEGLU) multiplies
-        the raw rows by gamma-scaled weights and applies (mean, rstd) in its epilogue (include/sb200.h: sb200_gemm_ln).
-        210 launches and one read + write of the stream per norm disappear from an SDXL forward."""
-        M, C_ = h.shape[0], tr.proj_in.weight.shape[0]
-        cap = (C_ + 15) // 16                            # slots per row: one per N tile (tiles are >= 16 columns wide)
-        bufs = [torch.empty(M * cap * 2, device=h.device, dtype=torch.float32) for _ in range(2)]
-        turn = 0
-
-        def produce(x, leaf, resid, lora=None):
-            nonlocal turn
-            st = bufs[turn]
-            turn ^= 1
-            out = ops.gemm(x, self._w(leaf), bias=self._b(leaf), resid=resid, lora=lora, rowstats=st)
-            return out, (st, ops.last_rowstats_parts)
-
-        def consume(x, stats, norm, leaves, geglu=False):
-            wp, c, d = self._ln_pack(norm, leaves)
-            la, cl, dl = self._ln_lora(norm, leaves)
-            fold = ops.LnFold(stats[0], stats[1], C_, norm.eps, c, d, cl, dl)
-            if geglu and la is not None:  # the GEGLU epilogue carries no LoRA
-                return ops.geglu(ops.gemm(x, wp, lora=la, ln=fold))
-            return ops.gemm(x, wp, geglu=geglu, lora=la, ln=fold)
-
-        h, st = produce(h, tr.proj_in, None, self._lora([tr.proj_in]))
-        for blk in tr.transformer_blocks:
-            a1, a2 = blk.attn1, blk.attn2
-            qkv = consume(h, st, blk.norm1, [a1.to_q, a1.to_k, a1.to_v])
-            o = ops.attention(qkv[:, :C_], qkv[:, C_:2 * C_], qkv[:, 2 * C_:], B, a1.heads, S, S, a1.dim_head ** -0.5,
-                              a1.dim_head)
-            h, st = produce(o, a1.to_out[0], h, self._lora([a1.to_out[0]]))
-            q = consume(h, st, blk.norm2, [a2.to_q])
-            k, v = self._kv(a2, ctx, kv_all)
-            o = ops.attention(q, k, v, B, a2.heads, S, Sctx, a2.dim_head ** -0.5, a2.dim_head)
-            h, st = produce(o, a2.to_out[0], h, self._lora([a2.to_out[0]]))
-            ffp, ffo = blk.ff.net[0].proj, blk.ff.net[2]
-            f = consume(h, st, blk.norm3, [ffp], geglu=True)
-            h, st = produce(f, ffo, h, self._lora([ffo]))
-        return ops.gemm(h, self._w(tr.proj_out), bias=self._b(tr.proj_out), resid=res, lora=self._lora([tr.proj_out]))
 
     def _embeddings(self, timesteps_f32, B, added_cond_kwargs):
         """Returns SiLU(emb) [B, temb].  In diffusers `emb` has exactly one kind of consumer — every
@@ -915,8 +826,6 @@ def _refresh(self: UNet2DConditionModel):
     for key in list(self._lora_packs.keys()):
         leaves = [leaves_by_id[i] for i in key]
         self._lora(leaves)
-    for ent in list(self._ln_lora_packs.values()):   # gamma-scaled copies follow their plain packs
-        self._ln_lora(ent[4], ent[5])
 
 
 UNet2DConditionModel._refresh_lora_packs = _refresh

@@ -128,9 +128,6 @@ def test_wide_ineligible_returns_errors(dev):
     with pytest.raises(_cabi.Sb200Error, match="bn=256"):
         ops.gemm(x, torch.zeros(512, 640, device=dev, dtype=torch.bfloat16), bn=256 | PAIR)  # CTA pairs
     with pytest.raises(_cabi.Sb200Error, match="bn=256"):
-        ops.gemm(x, torch.zeros(512, 640, device=dev, dtype=torch.bfloat16), bn=WIDE,
-                 rowstats=torch.zeros(256, 8, 2, device=dev))                                 # row statistics
-    with pytest.raises(_cabi.Sb200Error, match="bn=256"):
         ops.conv3x3(torch.zeros(1, 16, 16, 64, device=dev, dtype=torch.bfloat16),
                     torch.zeros(320, 3, 3, 64, device=dev, dtype=torch.bfloat16), bn=WIDE)    # Cout 320
     torch.cuda.synchronize()

@@ -553,64 +553,3 @@ def test_bad_arguments_return_errors_not_crashes(dev):
         ops.attention_bwd(q, q, q, q, q, lse, 1, 2, 64, 64, 0.125, 64, torch.zeros(128, 64, device=dev, dtype=BF))
     with pytest.raises(ValueError, match="row-strided"):
         ops.layernorm_bwd(q, q[0], q, out=q.t())
-
-
-@pytest.mark.parametrize("force", [SINGLE, PAIR, 0])
-@pytest.mark.parametrize("M,C_,N,geglu,lora,resid", [
-    (1000, 640, 1920, False, (4, 640, 1.0), False),    # norm1 -> fused q|k|v with three adaptors
-    (2048, 1280, 1280, False, None, True),             # norm2 -> attn2.to_q; the producer carries bias + residual
-    (512, 640, 5120, True, None, True),                # norm3 -> GEGLU
-    (300, 320, 960, False, (8, 320, -0.5), False),     # rank 8, ragged M
-])
-def test_layernorm_folded_into_projection(dev, force, M, C_, N, geglu, lora, resid):
-    """sb200_gemm_ln: a GEMM leaves per-row (sum, sum of squares) of the stream it writes; the next projection consumes
-    LayerNorm(stream) without a LayerNorm launch (gamma folded into W, mean / rstd applied in the epilogue)."""
-    from sliders_b200 import ops
-
-    g = torch.Generator().manual_seed(M + C_ + N)
-    # producer: stream = a @ wp^T + bp (+ r), written by the kernel together with its row statistics
-    a = torch.randn(M, 256, generator=g).to(dev, BF)
-    wp = (torch.randn(C_, 256, generator=g) / 16).to(dev, BF)
-    bp = (torch.randn(C_, generator=g) * 3).to(dev, BF)          # a large row mean stresses E[x^2] - mean^2
-    r = torch.randn(M, C_, generator=g).to(dev, BF) if resid else None
-    cap = (C_ + 15) // 16
-    stats = torch.full((M * cap * 2,), float("nan"), device=dev)
-    x = ops.gemm(a, wp, bias=bp, resid=r, rowstats=stats, bn=force)
-    parts = ops.last_rowstats_parts
-    assert 0 < parts <= cap
-    st = stats[: M * parts * 2].view(parts, M, 2).double().sum(0)
-    xf = x.double()
-    assert torch.allclose(st[:, 0], xf.sum(1), rtol=1e-4, atol=1e-2)
-    assert torch.allclose(st[:, 1], (xf * xf).sum(1), rtol=1e-4, atol=1e-2)
-    # consumer
-    gamma = (1 + 0.3 * torch.randn(C_, generator=g)).to(dev)
-    beta = (0.2 * torch.randn(C_, generator=g)).to(dev)
-    w = (torch.randn(N, C_, generator=g) / C_ ** 0.5).to(dev, BF)
-    b = torch.randn(N, generator=g).to(dev, BF).float()
-    wq = (w.float() * gamma[None, :]).to(BF).contiguous()
-    c = wq.float().sum(1).contiguous()
-    d = (w.float() @ beta + b).contiguous()
-    la = cl = dl = None
-    if lora:
-        rr, group_n, scale = lora
-        down, up, rt = make_lora(C_, N, rr, group_n, dev, 5)
-        downq = (down.float() * gamma[None, :]).to(BF).contiguous()
-        la = ops.Lora(downq, up, rr, group_n, scale)
-        cl, dl = downq.float().sum(1).contiguous(), (down.float() @ beta).contiguous()
-    fold = ops.LnFold(stats, parts, C_, 1e-5, c, d, cl, dl)
-    out = ops.gemm(x, wq, geglu=geglu, lora=la, ln=fold, bn=force)
-    torch.cuda.synchronize()
-    n = F.layer_norm(x.float(), (C_,), gamma, beta, 1e-5)
-    ref = n @ w.float().t() + b
-    if lora:
-        t = n @ down.float().t()
-        for g0 in range(0, N, group_n):
-            grp = g0 // group_n
-            ref[:, g0:g0 + group_n] += (t[:, grp * rr:(grp + 1) * rr] @ up[g0:g0 + group_n].t()) * scale
-    if geglu:
-        v, gate = ref.chunk(2, dim=-1)
-        ref = v * F.gelu(gate)
-    assert rel_rms(out, ref) < 1e-2
-    # the fold cancels in E[x^2] - mean^2 per row, so it is checked row by row rather than element by element
-    row_rel = (out.float() - ref).norm(dim=1) / ref.norm(dim=1)
-    assert row_rel.max().item() <= 2e-2, f"row {int(row_rel.argmax())}: rel-RMS {row_rel.max().item():.3g}"

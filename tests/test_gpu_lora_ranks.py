@@ -1,5 +1,5 @@
 """GPU tests of LoRA ranks 1-16: the rank-16 fused kernels (gemm_kernel<*, *, 64>, the rank-16 epilogue at 16 / 32 /
-64 LoRA-down rows, conv, LayerNorm fold, small_linear, the six backward kernels) element by element against float64,
+64 LoRA-down rows, conv, small_linear, the six backward kernels) element by element against float64,
 and on tiny UNets that an adaptor of rank r gives bit for bit what the same weights zero-padded to the slot width give
 (forward eager and under graph replay, gradients, one AdamW step), rank 16 against the fp32 oracle, and a rank-1
 slider file through the eval sweep."""
@@ -150,15 +150,6 @@ def test_wide_tiles_refuse_rank16(dev, rank16):
         c = gemm_case(512, 768 if lora[1] == 256 else 1280, 640, "L", lora, dev, 5)
         with pytest.raises(_cabi.Sb200Error, match="bn=256"):
             run_gemm(c, 256)
-
-
-@pytest.mark.parametrize("force", [SINGLE, PAIR, 0])
-@pytest.mark.parametrize("M,C_,N,lora", [
-    (1000, 640, 1920, (16, 640, 1.0)),    # norm1 -> fused q|k|v, three rank-16 adaptors: rt = 64
-    (300, 320, 320, (16, 320, -0.5)),     # one adaptor: rt = 16, ragged M
-])
-def test_layernorm_fold_rank16(dev, rank16, force, M, C_, N, lora):
-    gk.test_layernorm_folded_into_projection(dev, force, M, C_, N, False, lora, False)
 
 
 @pytest.mark.parametrize("M,N,K,xpad,act_in,act_out,lora,resid", [

@@ -41,14 +41,12 @@ def _meta(*shape):
     return torch.empty(shape, device="meta", dtype=torch.bfloat16)
 
 
-def gemm(x, w, *, bias=None, rowbias=None, rows_per_batch=1, resid=None, geglu=False, lora=None, x1=None, out=None, bn=0,
-         ln=None, rowstats=None):
+def gemm(x, w, *, bias=None, rowbias=None, rows_per_batch=1, resid=None, geglu=False, lora=None, x1=None, out=None, bn=0):
     M, K0 = x.shape
     N, K = w.shape
-    # b bias, R residual, G GEGLU, L LoRA, S split-K sources, N LayerNorm folded in, s leaves row statistics
+    # b bias, R residual, G GEGLU, L LoRA, S split-K sources
     tag = "".join(c for c, f in (("b", bias is not None), ("R", resid is not None), ("G", geglu), ("L", lora is not None),
-                                 ("S", x1 is not None), ("N", ln is not None), ("s", rowstats is not None)) if f)
-    ops.last_rowstats_parts = 1
+                                 ("S", x1 is not None)) if f)
     calls.append(("gemm_kernel", f"gemm M{M} N{N} K{K} {tag}", 2.0 * M * N * K))
     _note_lora(lora)
     return _meta(M, N // 2 if geglu else N)
@@ -138,9 +136,6 @@ def trace(batch, with_lora=True, train=False, extra_targets=(), rank=4):
             plora.DEFAULT_TARGET_REPLACE += plora.UNET_TARGET_REPLACE_MODULE_CONV + list(extra_targets)
             net = plora.LoRANetwork(unet, rank=rank, multiplier=1.0, alpha=1.0, train_method="noxattn")
             del plora.DEFAULT_TARGET_REPLACE[len(saved):]
-        unet._ln_pack = lambda norm, leaves: (_meta(sum(l.weight.shape[0] for l in leaves), leaves[0].weight.shape[1]), None, None)
-        unet._ln_lora = lambda norm, leaves: (unet._lora(leaves), None, None)
-        ops.LnFold = lambda *a, **k: object()
         unet._lora = _lora_slots
         x = torch.empty(batch, 4, 128, 128, dtype=torch.float32)
         t = torch.empty(batch, dtype=torch.float32)
