@@ -278,6 +278,15 @@ int sb200_guided_step_loss(void* handle, void* stream, const float* eps_u, const
                            float cx, float ce, const float* target, int64_t n, int mode, float* loss, float* ws,
                            const float* dloss, float* d_eps_u);
 
+/* Composite LoRA packs of a SliderStack (several sliders in the columns of one LoRA slot): eff = raw * col_mult,
+ * with raw / eff [rows, rp] fp32 row-major and col_mult [rp] fp32, one multiplier per slot column.  The chained hooks
+ * of the reference scale each network's delta by its own multiplier (lora.py:108-112: up(down(x)) * multiplier *
+ * scale); the stack keeps alpha / rank folded into raw and applies the runtime multipliers here, once per forward over
+ * every pack, so the fused kernels read eff with scale 1.  rp in [1, 64]; 16-byte vector path when rp % 4 == 0 and
+ * both buffers are 16-byte aligned. */
+int sb200_lora_compose(void* handle, void* stream, const float* raw, const float* col_mult, float* eff, int64_t rows,
+                       int rp);
+
 #ifdef __cplusplus
 }
 #endif

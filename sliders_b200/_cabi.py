@@ -77,6 +77,7 @@ SIGNATURES = {
     "sb200_upsample2x": [_p, _p, _p, _p, _i, _i, _i, _i],
     "sb200_cfg_ddim": [_p, _p, _p, _i, _f, _p, _f, _f, _p, _p, _i, _i64],
     "sb200_cfg_step": [_p, _p, _p, _i, _f, _p, _f, _f, _p, _p, _i, _i64],
+    "sb200_lora_compose": [_p, _p, _p, _p, _p, _i64, _i],
 }
 _RESTYPE = {"sb200_version": C.c_char_p, "sb200_last_error": C.c_char_p}
 

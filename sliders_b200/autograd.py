@@ -120,6 +120,10 @@ def _pad_rank(t: torch.Tensor, dim: int, rp: int) -> torch.Tensor:
 
 def _new_tape(unet) -> list:
     """A tape for `unet._walk`, opened with the snapshot of the active adaptors that `_Grads` reads."""
+    if unet._stack_status() is not None:
+        # the backward kernels read one adaptor per leaf; a SliderStack's composite hooks carry several
+        raise NotImplementedError("sliders_b200: a gradient through an active SliderStack is not implemented "
+                                  "(stacks are for inference)")
     scales = {}
     for leaf, a in unet._adapted_leaves():
         s = float(a.multiplier) * float(a.scale)

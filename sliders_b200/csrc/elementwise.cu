@@ -528,3 +528,55 @@ static int launch_cfg(void* handle, void* stream, const void* eps2, int eps_is_f
   SB200_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
+
+// ---- composite LoRA packs of a SliderStack ----------------------------------------------------------------------
+// eff[n, j] = raw[n, j] * col_mult[j] over `rows` rows of rp fp32 columns.  Every composite pack of a UNet lives in one
+// arena (sliders_b200/unet.py), so one launch per forward applies each slider's runtime multiplier to its columns of
+// the packed lora_up; the fused GEMM / conv / small_linear kernels then read `eff` with scale 1.  A plain product, so
+// the result equals torch's fp32 `raw * col_mult` bit for bit.
+namespace sb200 {
+
+__global__ void lora_compose_vec_kernel(const float4* __restrict__ raw, const float* __restrict__ col_mult,
+                                        float4* __restrict__ eff, int64_t n4, int rp4) {
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4; i += stride) {
+    const float* m = col_mult + static_cast<int>(i % rp4) * 4;
+    float4 v = __ldg(raw + i);
+    v.x *= __ldg(m + 0);
+    v.y *= __ldg(m + 1);
+    v.z *= __ldg(m + 2);
+    v.w *= __ldg(m + 3);
+    eff[i] = v;
+  }
+}
+
+__global__ void lora_compose_kernel(const float* __restrict__ raw, const float* __restrict__ col_mult,
+                                    float* __restrict__ eff, int64_t n, int rp) {
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride)
+    eff[i] = __ldg(raw + i) * __ldg(col_mult + static_cast<int>(i % rp));
+}
+
+}  // namespace sb200
+
+extern "C" int sb200_lora_compose(void* handle, void* stream, const float* raw, const float* col_mult, float* eff,
+                                  int64_t rows, int rp) {
+  Ctx* ctx = as_ctx(handle);
+  SB200_REQUIRE(ctx && raw && col_mult && eff, "lora_compose: NULL argument");
+  SB200_REQUIRE(rows > 0, "lora_compose: rows=%lld must be positive", static_cast<long long>(rows));
+  SB200_REQUIRE(rp > 0 && rp <= 64, "lora_compose: rp=%d must be in [1, 64]", rp);
+  SB200_REQUIRE(raw != eff, "lora_compose: raw and eff must be distinct buffers");
+  const int64_t n = rows * rp;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const bool vec = rp % 4 == 0 && (reinterpret_cast<uintptr_t>(raw) | reinterpret_cast<uintptr_t>(eff)) % 16 == 0;
+  const int64_t work = vec ? n / 4 : n;
+  int blocks = static_cast<int>((work + 255) / 256);
+  if (blocks > ctx->num_sms * 8) blocks = ctx->num_sms * 8;
+  if (vec)
+    lora_compose_vec_kernel<<<blocks, 256, 0, s>>>(reinterpret_cast<const float4*>(raw), col_mult,
+                                                   reinterpret_cast<float4*>(eff), work, rp / 4);
+  else
+    lora_compose_kernel<<<blocks, 256, 0, s>>>(raw, col_mult, eff, n, rp);
+  SB200_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}

@@ -18,7 +18,7 @@ from __future__ import annotations
 import argparse
 import csv
 import os
-from typing import Callable, Dict, List, Optional, Sequence
+from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -78,10 +78,13 @@ def build_network(unet, slider_path: str, device, dtype, rank: Optional[int] = N
 def sweep(unet, network, scheduler, rows: Sequence[dict], embed: Callable[[str], tuple], save_dir: str, *,
           scales: Sequence[float] = SCALES, num_samples: int = 1, num_inference_steps: int = 50,
           guidance_scale: float = 5.0, start_noise: int = 750, image_size: int = 1024, xl: bool = True,
-          decode: Optional[Callable[[torch.Tensor], list]] = None, dtype=torch.bfloat16) -> int:
+          decode: Optional[Callable[[torch.Tensor], list]] = None, dtype=torch.bfloat16,
+          fixed_scales: Sequence[float] = ()) -> int:
     """For every CSV row and every scale: same seed -> same initial noise -> `denoise_loop` with the slider gated on
     `t <= start_noise` -> `<save_dir>/<scale>/<case>_<sample>.pt` (+ .png through `decode`).  Returns the number of
-    latents written.  `embed(prompt)` -> (prompt_embeds [2,77,D] as (negative ; positive), add_text_embeds [2,1280] | None)."""
+    latents written.  `embed(prompt)` -> (prompt_embeds [2,77,D] as (negative ; positive), add_text_embeds [2,1280] | None).
+    fixed_scales: with a `lora.SliderStack` as `network`, the scales of its second, third, ... sliders, held while the
+    first one sweeps `scales`."""
     dev = next(unet.parameters()).device
     for s in scales:
         os.makedirs(os.path.join(save_dir, str(s)), exist_ok=True)
@@ -99,7 +102,8 @@ def sweep(unet, network, scheduler, rows: Sequence[dict], embed: Callable[[str],
             lat = initial_latents(row["seed"], num_samples, image_size, image_size, scheduler.init_noise_sigma, dev, dtype)
             out = generate.denoise_loop(unet, network, scheduler, lat, pe, added.get("add_text_embeds"),
                                         added.get("add_time_ids"), num_inference_steps=num_inference_steps,
-                                        guidance_scale=guidance_scale, scale=s, start_noise=start_noise)
+                                        guidance_scale=guidance_scale,
+                                        scale=[s, *fixed_scales] if fixed_scales else s, start_noise=start_noise)
             images = decode(out) if decode is not None else None
             for j in range(num_samples):
                 stem = os.path.join(save_dir, str(s), f"{row['case_number']}_{j}")
@@ -108,6 +112,17 @@ def sweep(unet, network, scheduler, rows: Sequence[dict], embed: Callable[[str],
                     images[j].save(stem + ".png")
                 written += 1
     return written
+
+
+def parse_compose(value: str) -> Tuple[str, float]:
+    """`--compose PATH:SCALE` -> (PATH, SCALE); the last colon separates them, so PATH may contain colons."""
+    path, sep, scale = value.rpartition(":")
+    try:
+        if not sep or not path:
+            raise ValueError
+        return path, float(scale)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"--compose expects PATH:SCALE (e.g. smile_rank4.pt:-1.0), got {value!r}")
 
 
 def build_parser() -> argparse.ArgumentParser:
@@ -131,6 +146,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--embeds", type=str, default=None, help="torch file {prompt: (text_embeds, pooled_embeds)}")
     p.add_argument("--scheduler", type=str, default="euler", help="euler (the SDXL pipeline's), ddim, lms, ddpm, euler_a")
     p.add_argument("--device", type=int, default=0)
+    p.add_argument("--compose", type=parse_compose, action="append", default=[], metavar="PATH:SCALE",
+                   help="another slider held at SCALE while --model_name sweeps its scales (repeatable); the sliders "
+                        "run as one lora.SliderStack with --model_name first")
     return p
 
 
@@ -143,7 +161,11 @@ def main(argv: Optional[Sequence[str]] = None, xl: bool = True) -> int:
     load = model_util.load_models_xl if xl else model_util.load_models
     toks, encs, unet, _ = load(args.unet, "ddim", weight_dtype=dtype, device=dev)
     unet.use_cuda_graph = True
-    network = build_network(unet, args.model_name, dev, dtype)
+    fixed = [s for _, s in args.compose]
+    if args.compose:
+        network = lora.SliderStack.from_files(unet, [args.model_name] + [p for p, _ in args.compose], dev, dtype)
+    else:
+        network = build_network(unet, args.model_name, dev, dtype)
     table = torch.load(args.embeds, map_location="cpu") if args.embeds else {}
     neg = args.negative_prompts or ""
 
@@ -167,6 +189,6 @@ def main(argv: Optional[Sequence[str]] = None, xl: bool = True) -> int:
     n = sweep(unet, network, create_noise_scheduler(args.scheduler), rows, embed, save_dir,
               num_samples=args.num_samples, num_inference_steps=50 if xl else args.ddim_steps,
               guidance_scale=5.0 if xl else args.guidance_scale, start_noise=args.start_noise,
-              image_size=1024 if xl else args.image_size, xl=xl, dtype=dtype)
+              image_size=1024 if xl else args.image_size, xl=xl, dtype=dtype, fixed_scales=fixed)
     print(f"wrote {n} latents under {save_dir}")
     return n

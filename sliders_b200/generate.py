@@ -10,7 +10,7 @@ device-side values, so the `t > start_noise` gating and a whole `scales` sweep r
 """
 from __future__ import annotations
 
-from typing import Callable, Optional, Sequence
+from typing import Callable, Optional, Sequence, Union
 
 import torch
 
@@ -35,13 +35,16 @@ def check_negative_embeds_per_step(negative_embeds_per_step, prompt_embeds: torc
 @torch.no_grad()
 def denoise_loop(unet, network, scheduler, latents: torch.Tensor, prompt_embeds: torch.Tensor,
                  add_text_embeds: Optional[torch.Tensor] = None, add_time_ids: Optional[torch.Tensor] = None, *,
-                 num_inference_steps: int = 50, guidance_scale: float = 5.0, scale: float = 0.0,
+                 num_inference_steps: int = 50, guidance_scale: float = 5.0,
+                 scale: Union[float, Sequence[float]] = 0.0,
                  start_noise: int = 750, callback: Optional[Callable] = None,
                  generator: Optional[torch.Generator] = None,
                  negative_embeds_per_step: Optional[Sequence[torch.Tensor]] = None) -> torch.Tensor:
     """latents: [N,4,h,w] already multiplied by `scheduler.init_noise_sigma`; prompt_embeds: [2N,77,D] as
     (negative ; positive) like `encode_prompt` + `torch.cat` produce (generate_images_xl.py:251-307);
     add_text_embeds [2N,1280] / add_time_ids [2N,6] for SDXL, None for SD1.x.  Returns the final latents.
+    network: a LoRANetwork, or a `lora.SliderStack` with `scale` a scalar (every slider) or one value per slider; above
+    `start_noise` every slider is off.
     negative_embeds_per_step: step i uses the i-th [1,77,D] embedding as the unconditional half of every sample (the
     null-text inversion edit, demo_image_editing.ipynb cell 13: `uncond_embeddings_copy[cnt]`); it is copied into one
     buffer, so a CUDA-graphed UNet keeps replaying the same graph."""
@@ -75,6 +78,7 @@ def denoise_loop(unet, network, scheduler, latents: torch.Tensor, prompt_embeds:
 @torch.no_grad()
 def scale_sweep(unet, network, scheduler, latents, prompt_embeds, add_text_embeds=None, add_time_ids=None, *,
                 scales=(-2, -1, 0, 1, 2), **kw):
-    """generate_images_xl.py:495-508: the same seed / latents denoised once per slider scale."""
+    """generate_images_xl.py:495-508: the same seed / latents denoised once per slider scale.  With a
+    `lora.SliderStack` each entry of `scales` is a scalar (every slider) or a sequence (one value per slider)."""
     return [denoise_loop(unet, network, scheduler, latents.clone(), prompt_embeds, add_text_embeds, add_time_ids,
                          scale=s, **kw) for s in scales]

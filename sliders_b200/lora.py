@@ -17,7 +17,7 @@ from __future__ import annotations
 
 import math
 import os
-from typing import List, Literal, Optional
+from typing import Dict, List, Literal, Optional, Sequence, Union
 
 import torch
 import torch.nn as nn
@@ -79,6 +79,10 @@ class LoRANetwork(nn.Module):
     def __init__(self, unet: nn.Module, rank: int = 4, multiplier: float = 1.0, alpha: float = 1.0,
                  train_method: TRAINING_METHODS = "full", init_a: float = 1.0) -> None:
         super().__init__()
+        if self._hooks_leaves and getattr(unet, "__dict__", {}).get("_slider_stack") is not None:
+            # the composite hooks of a stack own the leaves; chaining a network on top would be silently dropped
+            raise RuntimeError("sliders_b200: a LoRANetwork cannot be built on a UNet that carries a SliderStack; add "
+                               "the slider to the stack instead (SliderStack(unet, [...]) takes every slider at once)")
         self.lora_scale = 1
         self.multiplier = multiplier
         self.lora_dim = rank
@@ -93,12 +97,18 @@ class LoRANetwork(nn.Module):
             assert lora.lora_name not in seen, f"duplicated lora name: {lora.lora_name}"
             seen.add(lora.lora_name)
         for lora in self.unet_loras:
-            lora.apply_to()
+            self._attach(lora)
             self.add_module(lora.lora_name, lora)
         # the engine caches which leaves are adapted
         if hasattr(unet, "__dict__"):
             unet.__dict__.pop("_adapted_cache", None)
         del unet
+
+    # a plain network hooks each adaptor into its leaf (lora.py:103-106); the sliders of a SliderStack do not
+    _hooks_leaves = True
+
+    def _attach(self, lora: LoRAModule) -> None:
+        lora.apply_to()
 
     @staticmethod
     def _skip_module(name: str, train_method: str) -> bool:
@@ -173,3 +183,161 @@ class LoRANetwork(nn.Module):
     def __exit__(self, exc_type, exc_value, tb):
         for lora in self.unet_loras:
             lora.multiplier = 0
+
+
+# --------------------------------------------------------------------------------------------------
+# composition: several sliders on one UNet, each with its own runtime scale
+# --------------------------------------------------------------------------------------------------
+class _StackedLoRANetwork(LoRANetwork):
+    """One slider of a SliderStack: a LoRANetwork in every respect (keys, state_dict, save_weights, optimiser params,
+    set_lora_slider, `with`) except that its adaptors are not hooked into the leaves one by one; the stack installs a
+    single composite hook per adapted leaf instead."""
+
+    _hooks_leaves = False
+
+    def _attach(self, lora: LoRAModule) -> None:
+        self._leaves[lora.lora_name] = lora.org_module
+        del lora.org_module  # what apply_to drops, so the state dict holds the adaptor only
+
+    def __init__(self, unet: nn.Module, **kw) -> None:
+        self.__dict__["_leaves"] = {}  # lora_name -> adapted leaf, filled before nn.Module registration matters
+        super().__init__(unet, **kw)
+        self.name = None
+
+
+class SliderHook:
+    """The one hook a SliderStack installs on an adapted leaf (as `leaf.forward`, where the reference's chained networks
+    put their adaptor's forward, lora.py:103-106).  `slider_entries` lists (slider index, LoRAModule) of every slider that
+    adapts the leaf; the engine packs them into the columns each slider owns in the leaf's LoRA slot."""
+
+    def __init__(self, stack: "SliderStack", leaf_name: str):
+        self.stack = stack
+        self.leaf_name = leaf_name
+        self.slider_entries: List[tuple] = []
+
+    def forward(self, x):
+        raise RuntimeError(
+            f"{self.leaf_name}: the leaf of a SliderStack was called through PyTorch.  In sliders_b200 the sliders' "
+            "deltas are fused into the wgmma GEMM/conv kernels (UNet2DConditionModel.forward); there is no eager path.")
+
+
+def _has_adaptor(leaf: nn.Module) -> bool:
+    owner = getattr(leaf.__dict__.get("forward"), "__self__", None)
+    return owner is not None and (hasattr(owner, "lora_down") or hasattr(owner, "slider_entries"))
+
+
+class SliderStack(nn.Module):
+    """Several sliders composed on one UNet, each at its own strength (an age slider at 2 and a smile slider at -1).
+
+    The reference composes by building one LoRANetwork after another on the same UNet, which chains the leaves'
+    forwards (lora.py:103-112) so every network adds its own `up(down(x)) * multiplier * scale`.  Here the sliders are
+    built in the same order, with the same seeded initial weights, but one composite hook per leaf carries all of
+    them: slider i owns the columns [o_i, o_i + r_i) of the leaf's LoRA slot (o_i = the sum of the earlier ranks, the
+    total rank at most 16), and its runtime multiplier scales those columns on the device, so one captured CUDA graph
+    serves every combination of scales.
+
+    `specs`: one dict per slider with LoRANetwork's keyword arguments (rank, alpha, train_method, multiplier, init_a)
+    and optionally network_type="c3lier" to add the conv targets (train_lora_xl.py:50-52) for that slider only.
+    Inference only: a gradient through an active stack raises NotImplementedError."""
+
+    def __init__(self, unet: nn.Module, specs: Sequence[Dict]) -> None:
+        super().__init__()
+        specs = [dict(s) for s in specs]
+        if not specs:
+            raise ValueError("SliderStack needs at least one slider")
+        ranks = [int(s.get("rank", 4)) for s in specs]
+        if any(r < 1 for r in ranks):
+            raise ValueError(f"SliderStack: every slider rank must be at least 1, got {ranks}")
+        if sum(ranks) > 16:
+            raise NotImplementedError(f"SliderStack: total rank {sum(ranks)} (ranks {ranks}) exceeds 16, the width of "
+                                      "the fused kernels' LoRA slot")
+        if unet.__dict__.get("_slider_stack") is not None:
+            raise RuntimeError("sliders_b200: this UNet already carries a SliderStack; put every slider in one stack")
+        if any(_has_adaptor(m) for m in unet.modules()):
+            raise RuntimeError("sliders_b200: a SliderStack cannot be built on a UNet that already carries a "
+                               "LoRANetwork; build every slider through the stack")
+        sliders = []
+        for spec in specs:
+            conv = spec.pop("network_type", None) == "c3lier"
+            saved = list(DEFAULT_TARGET_REPLACE)
+            if conv:
+                DEFAULT_TARGET_REPLACE.extend(t for t in UNET_TARGET_REPLACE_MODULE_CONV if t not in saved)
+            try:
+                sliders.append(_StackedLoRANetwork(unet, **spec))
+            finally:
+                del DEFAULT_TARGET_REPLACE[len(saved):]
+        self.sliders = nn.ModuleList(sliders)
+        self.ranks = tuple(ranks)
+        self.offsets = tuple(sum(ranks[:i]) for i in range(len(ranks)))
+        names = {id(m): n for n, m in unet.named_modules()}
+        hooks: Dict[int, SliderHook] = {}
+        leaves = {}
+        for i, net in enumerate(sliders):
+            for lora in net.unet_loras:
+                leaf = net._leaves[lora.lora_name]
+                hook = hooks.get(id(leaf))
+                if hook is None:
+                    hook = hooks[id(leaf)] = SliderHook(self, names.get(id(leaf), lora.lora_name))
+                    leaves[id(leaf)] = leaf
+                hook.slider_entries.append((i, lora))
+        for key, hook in hooks.items():
+            leaves[key].forward = hook.forward
+        self.n_leaves = len(hooks)
+        # identifies the slot layout a captured graph was built for (not the scales: those are device-side values)
+        self.structure = (id(self), self.ranks, tuple(len(n.unet_loras) for n in sliders), self.n_leaves)
+        unet.__dict__["_slider_stack"] = self
+        unet.__dict__.pop("_adapted_cache", None)
+
+    @classmethod
+    def from_files(cls, unet: nn.Module, paths: Sequence[str], device=None, dtype=None) -> "SliderStack":
+        """One slider per checkpoint, like `eval_sweep.build_network`: rank, alpha, train method and the c3lier conv
+        targets are read from each file's name (generate_images_xl.py:460-485), then the weights are loaded."""
+        from . import io as sio
+        from .eval_sweep import parse_slider_name
+
+        infos = [parse_slider_name(p) for p in paths]
+        stack = cls(unet, [dict(rank=i["rank"], alpha=i["alpha"], train_method=i["train_method"],
+                                network_type=i["network_type"]) for i in infos])
+        if device is not None or dtype is not None:
+            stack.to(device=device, dtype=dtype)
+        for net, path in zip(stack.sliders, paths):
+            net.name = path
+            sio.load_slider(net, path)
+        return stack
+
+    @property
+    def total_rank(self) -> int:
+        return sum(self.ranks)
+
+    def set_lora_slider(self, scale: Union[float, Sequence[float]]) -> None:
+        """A scalar sets every slider (so `generate.denoise_loop`'s start_noise gating turns all of them off); a
+        sequence gives one value per slider."""
+        if isinstance(scale, (int, float)) or (torch.is_tensor(scale) and scale.dim() == 0):
+            values = [float(scale)] * len(self.sliders)
+        else:
+            values = [float(v) for v in scale]
+            if len(values) != len(self.sliders):
+                raise ValueError(f"SliderStack.set_lora_slider: {len(values)} scales for {len(self.sliders)} sliders")
+        for net, v in zip(self.sliders, values):
+            net.set_lora_slider(v)
+
+    def __enter__(self):
+        for net in self.sliders:
+            net.__enter__()
+        return self
+
+    def __exit__(self, exc_type, exc_value, tb):
+        for net in self.sliders:
+            net.__exit__(exc_type, exc_value, tb)
+
+    def slider_multipliers(self) -> List[float]:
+        """The runtime multiplier of each slider: the common `multiplier` of its modules (what `with slider:` sets)."""
+        out = []
+        for i, net in enumerate(self.sliders):
+            ms = {float(l.multiplier) for l in net.unet_loras}
+            if len(ms) > 1:
+                name = net.name or f"slider {i}"
+                raise ValueError(f"SliderStack: {name} has modules with different multipliers {sorted(ms)}; a stack "
+                                 "applies one runtime scale per slider")
+            out.append(ms.pop() if ms else 0.0)
+        return out

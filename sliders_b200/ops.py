@@ -574,6 +574,24 @@ def add(a: torch.Tensor, b: torch.Tensor, c: Optional[torch.Tensor] = None, out:
     return out
 
 
+def lora_compose(raw: torch.Tensor, col_mult: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[n, j] = raw[n, j] * col_mult[j]: the effective lora_up of composite LoRA packs (fp32 [rows, rp], contiguous),
+    one `lora_compose` launch."""
+    if raw.dtype != torch.float32 or col_mult.dtype != torch.float32 or raw.dim() != 2 or not raw.is_contiguous():
+        raise ValueError("lora_compose: raw must be a contiguous fp32 [rows, rp] matrix and col_mult fp32")
+    rows, rp = raw.shape
+    if col_mult.numel() != rp or not col_mult.is_contiguous():
+        raise ValueError(f"lora_compose: col_mult has {col_mult.numel()} values for {rp} columns")
+    if out is None:
+        out = torch.empty_like(raw)
+    elif out.shape != raw.shape or out.dtype != torch.float32 or not out.is_contiguous():
+        raise ValueError("lora_compose: out must be a contiguous fp32 matrix shaped like raw")
+    lib = _begin()
+    _cabi.check(lib.sb200_lora_compose(_ctx(raw), _stream(), _p(raw), _p(col_mult), _p(out), rows, rp))
+    _count("lora_compose")
+    return out
+
+
 def upsample2x_bwd(dy: torch.Tensor) -> torch.Tensor:
     B, H2, W2, Cc = dy.shape
     dx = torch.empty((B, H2 // 2, W2 // 2, Cc), device=dy.device, dtype=BF16)

@@ -233,6 +233,9 @@ def _adaptor_of(leaf: nn.Module):
     owner = getattr(fwd, "__self__", None)
     if owner is not None and hasattr(owner, "lora_down") and hasattr(owner, "lora_up"):
         inner = getattr(getattr(owner, "org_forward", None), "__self__", None)
+        if inner is not None and hasattr(inner, "slider_entries"):
+            raise RuntimeError(f"{getattr(owner, 'lora_name', 'leaf')}: a LoRANetwork was applied on top of a "
+                               "SliderStack; the stack's composite hook owns this leaf, so add the slider to the stack")
         if inner is not None and hasattr(inner, "lora_down"):
             # the reference chains `org_forward`, so two networks on one UNet both apply there; the fused kernels carry
             # one adaptor per leaf — refuse loudly instead of silently dropping the first network
@@ -243,13 +246,86 @@ def _adaptor_of(leaf: nn.Module):
     return None
 
 
+_UNSET = object()
+
+
+def _hook_of(leaf: nn.Module):
+    """The composite hook a SliderStack installed on `leaf` (sliders_b200.lora.SliderHook), or None."""
+    owner = getattr(leaf.__dict__.get("forward"), "__self__", None)
+    return owner if owner is not None and hasattr(owner, "slider_entries") else None
+
+
+def _fill_composite(down: torch.Tensor, raw: torch.Tensor, leaves, hooks, offsets, rp: int) -> None:
+    """Writes the sliders of one fused call into zeroed packs: leaf gi's slider i takes down rows
+    [gi * rp + o_i, + r) and raw up columns [o_i, o_i + r) of the leaf's output rows, with its alpha / r (the conv rank
+    clamp of lora.py:78 included) folded in; r is the adaptor's own rank, so a leaf a slider does not adapt, and the
+    columns past a clamped rank, keep zeros."""
+    n0 = 0
+    for gi, (leaf, h) in enumerate(zip(leaves, hooks)):
+        n1 = n0 + leaf.weight.shape[0]
+        for i, a in (h.slider_entries if h is not None else ()):
+            d = a.lora_down.weight.detach()
+            if d.dim() == 4:
+                d = d.permute(0, 2, 3, 1)
+            rr = d.shape[0]
+            c0 = offsets[i]
+            down[gi * rp + c0: gi * rp + c0 + rr].copy_(d.reshape(rr, -1))
+            u = a.lora_up.weight.detach().reshape(leaf.weight.shape[0], -1)
+            raw[n0:n1, c0:c0 + rr].copy_(u.float() * float(a.scale))
+        n0 = n1
+
+
 class _LoraPack:
-    """Packed (down [rt,K], up [N,r]) buffers of one fused call site; repacked only when a parameter changes."""
+    """Packed (down [rt,K], up [N,r]) buffers of one fused call site; repacked only when a parameter changes.  A
+    composite pack (SliderStack) also keeps `raw`: the sliders' up columns with alpha / r folded in, before the runtime
+    multipliers; `up` is then the effective pack sb200_lora_compose writes."""
 
     def __init__(self):
         self.key = None
         self.down = None
         self.up = None
+        self.raw = None
+
+
+class _StackArena:
+    """Device state of a UNet's SliderStack.  Every composite pack's raw and effective up columns are row slices of one
+    fp32 arena each, so a single sb200_lora_compose launch per forward applies the per-column multipliers `mult` (one
+    fp32 value per slot column: slider i's multiplier on its columns [o_i, o_i + r_i), 0 on padding)."""
+
+    def __init__(self, stack, device):
+        self.stack = stack
+        self.rp = ops.lora_slots(stack.total_rank)[0]
+        self.mult = torch.zeros(self.rp, device=device, dtype=torch.float32)
+        self.packs: List[_LoraPack] = []
+        self.raw = None
+        self.eff = None
+        self.dirty = False
+
+    def load(self, mults) -> None:
+        """Writes the multipliers into `mult` with one fill per slider: kernel launches with the value as an argument, so
+        the host never waits for the stream (a copy from pageable host memory would)."""
+        for o, r, m in zip(self.stack.offsets, self.stack.ranks, mults):
+            self.mult[o:o + r].fill_(float(m))
+
+    def settle(self) -> bool:
+        """Moves packs built since the last call into a new arena; True when packs that a captured graph may read
+        moved (there was an arena before)."""
+        if not self.dirty:
+            return False
+        moved = self.raw is not None
+        rows = sum(p.raw.shape[0] for p in self.packs)
+        dev = self.packs[0].raw.device
+        raw = torch.empty((rows, self.rp), device=dev, dtype=torch.float32)
+        eff = torch.empty((rows, self.rp), device=dev, dtype=torch.float32)
+        n0 = 0
+        for p in self.packs:
+            n1 = n0 + p.raw.shape[0]
+            raw[n0:n1].copy_(p.raw)
+            eff[n0:n1].copy_(p.up)
+            p.raw, p.up = raw[n0:n1], eff[n0:n1]
+            n0 = n1
+        self.raw, self.eff, self.dirty = raw, eff, False
+        return moved
 
 
 class UNet2DConditionModel(nn.Module):
@@ -304,6 +380,8 @@ class UNet2DConditionModel(nn.Module):
         self._lora_packs: Dict[tuple, _LoraPack] = {}
         self._graphs: Dict[tuple, "_CapturedForward"] = {}
         self._slider_scale_dev: Optional[torch.Tensor] = None
+        self._stack_arena: Optional[_StackArena] = None
+        self._stack_mults: Optional[List[float]] = None  # per-slider multipliers of the current walk; None: stack off
         self.use_cuda_graph = False
 
     # ---- diffusers-API shims used by the reference trainers (train_lora_xl.py:78-82) ----------------
@@ -327,6 +405,7 @@ class UNet2DConditionModel(nn.Module):
         self._graphs.clear()
         self.__dict__.pop("_train_graphs", None)
         self._slider_scale_dev = None
+        self._stack_arena = None
         return out
 
     def load_state_dict(self, *a, **k):
@@ -373,6 +452,8 @@ class UNet2DConditionModel(nn.Module):
     def _lora(self, leaves: List[nn.Module]) -> Optional[Lora]:
         """sb200_lora for one fused call over `leaves` (all sharing the same input), or None when no leaf is
         adapted or every multiplier is 0 (lora.py:256-258: outside `with network:` the delta is exactly 0)."""
+        if "_slider_stack" in self.__dict__:
+            return self._lora_composite(leaves)
         adaptors = [_adaptor_of(l) for l in leaves]
         if all(a is None for a in adaptors):
             return None
@@ -435,6 +516,82 @@ class UNet2DConditionModel(nn.Module):
     _capturing = False
     _bake_scales = False
 
+    # ---- SliderStack: composite LoRA packs -------------------------------------------------------------------------
+    def _stack_status(self) -> Optional[List[float]]:
+        """The stack's per-slider multipliers, or None when the UNet has no stack or every slider is at 0.  Read once
+        per `forward` (the snapshot below); outside a forward each call reads the sliders again."""
+        snap = self.__dict__.get("_stack_snapshot", _UNSET)
+        return self._stack_scan() if snap is _UNSET else snap
+
+    def _stack_scan(self) -> Optional[List[float]]:
+        stack = self.__dict__.get("_slider_stack")
+        if stack is None:
+            return None
+        if self._adapted_leaves():
+            raise RuntimeError("sliders_b200: a LoRANetwork was applied to a UNet that carries a SliderStack; add the "
+                               "slider to the stack instead")
+        mults = stack.slider_multipliers()
+        if all(m == 0.0 for m in mults):
+            return None
+        if self._stack_arena is None:
+            self._stack_arena = _StackArena(stack, self.conv_in.weight.device)
+        return mults
+
+    def _stack_begin(self, compose: bool = True) -> None:
+        """Start of a walk (or of a graph replay, compose=False): the current multipliers go to the device vector and,
+        once the packs are in their arena, one sb200_lora_compose writes every effective up pack."""
+        mults = self._stack_status()
+        self._stack_mults = mults
+        if mults is None:
+            return
+        arena = self._stack_arena
+        if not self._capturing:  # replays get the vector from _GraphInputs.load
+            arena.load(mults)
+        if compose and arena.raw is not None:
+            ops.lora_compose(arena.raw, arena.mult, out=arena.eff)
+
+    def _stack_end(self) -> None:
+        arena = self._stack_arena
+        if arena is not None and not self._capturing and arena.settle():
+            # graphs captured before hold the packs' old buffers
+            self._graphs.clear()
+
+    def _lora_composite(self, leaves: List[nn.Module]) -> Optional[Lora]:
+        """sb200_lora of one fused call on a UNet with a SliderStack: slider i's rows / columns [o_i, o_i + r_i) of every
+        leaf's slot, alpha / r folded into the raw up pack, the runtime multipliers applied by sb200_lora_compose; the
+        kernels run with scale 1.  None when no leaf is hooked or every slider is at 0."""
+        hooks = [_hook_of(l) for l in leaves]
+        if self._stack_mults is None or all(h is None for h in hooks):
+            return None
+        arena = self._stack_arena
+        rp = arena.rp
+        _, rt = ops.lora_slots(rp, len(leaves))
+        pack = self._lora_packs.setdefault(tuple(id(l) for l in leaves), _LoraPack())
+        ver = tuple(tuple((i, a.lora_down.weight.data_ptr(), a.lora_down.weight._version, a.lora_up.weight.data_ptr(),
+                           a.lora_up.weight._version) for i, a in h.slider_entries) if h is not None else None
+                    for h in hooks)
+        if pack.key != ver:
+            if pack.raw is None:
+                if self._capturing:
+                    raise RuntimeError("sliders_b200: a SliderStack call site was first met while a CUDA graph was "
+                                       "captured")
+                dev = leaves[0].weight.device
+                K = leaves[0].weight[0].numel()
+                N = sum(l.weight.shape[0] for l in leaves)
+                pack.down = torch.zeros((rt, K), device=dev, dtype=BF16)
+                pack.raw = torch.zeros((N, rp), device=dev, dtype=torch.float32)
+                pack.up = torch.empty((N, rp), device=dev, dtype=torch.float32)
+                arena.packs.append(pack)
+                arena.dirty = True
+            else:
+                pack.down.zero_()
+                pack.raw.zero_()
+            _fill_composite(pack.down, pack.raw, leaves, hooks, arena.stack.offsets, rp)
+            pack.key = ver
+            # the walk's compose has run already: compose this pack now
+            ops.lora_compose(pack.raw, arena.mult, out=pack.up)
+        return Lora(pack.down, pack.up, rp, leaves[0].weight.shape[0], 1.0)
+
     # ---- forward pieces ------------------------------------------------------------------------------
     # One walk serves inference and training.  `tape` is None for inference; for training it is a list to which every
     # block appends what its backward reads (sliders_b200/autograd.py): the GroupNorm statistics, the attention
@@ -494,9 +651,12 @@ class UNet2DConditionModel(nn.Module):
 
     def _cross_kv_adapted(self) -> bool:
         """True when an active adaptor sits on a to_k / to_v of attn2 (train methods xattn / full)."""
+        stack_on = self._stack_status() is not None
         for _, _, mods in self._kv_plan().values():
             for a in mods:
                 for leaf in (a.to_k, a.to_v):
+                    if stack_on and _hook_of(leaf) is not None:
+                        return True  # every hooked leaf runs its composite pack while any slider is on
                     ad = _adaptor_of(leaf)
                     if ad is not None and float(ad.multiplier) * float(ad.scale) != 0.0:
                         return True
@@ -603,6 +763,11 @@ class UNet2DConditionModel(nn.Module):
                 tape.append((kind, rec))
 
         B = sample.shape[0]
+        if "_slider_stack" in self.__dict__:
+            if tape is not None and self._stack_status() is not None:
+                raise NotImplementedError("sliders_b200: a gradient through an active SliderStack is not implemented "
+                                          "(stacks are for inference)")
+            self._stack_begin()
         Sctx = ehs.shape[1]
         ctx = ehs.reshape(B * Sctx, ehs.shape[-1])
         kv_all = self._cross_kv(ctx)
@@ -643,14 +808,32 @@ class UNet2DConditionModel(nn.Module):
         hn = ops.groupnorm(h, *self._w_norm(gn), gn.num_groups, gn.eps, True, stats_ws=ws)
         if tape is not None:
             tape.append(("out", (h, ops.gn_stats(ws, B, gn.num_groups))))
-        return ops.conv_out(hn, self._w(self.conv_out), self._b(self.conv_out), out_dtype=out_dtype)
+        out = ops.conv_out(hn, self._w(self.conv_out), self._b(self.conv_out), out_dtype=out_dtype)
+        if "_slider_stack" in self.__dict__:
+            self._stack_end()
+        return out
 
     # ---- public forward --------------------------------------------------------------------------------
     def forward(self, sample, timestep, encoder_hidden_states=None, added_cond_kwargs=None,
                 cross_attention_kwargs=None, return_dict: bool = True, **unused):
+        if "_slider_stack" not in self.__dict__:
+            return self._forward(sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict)
+        # the sliders' multipliers are read once per forward: the graph signature, the graph inputs, the walk and the
+        # cross-attention K / V decision all see this snapshot
+        self.__dict__["_stack_snapshot"] = self._stack_scan()
+        try:
+            return self._forward(sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict)
+        finally:
+            self.__dict__.pop("_stack_snapshot", None)
+
+    def _forward(self, sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict):
         ehs_grad = (torch.is_grad_enabled() and torch.is_tensor(encoder_hidden_states)
                     and encoder_hidden_states.requires_grad)
         if torch.is_grad_enabled() and (self._needs_grad() or ehs_grad):
+            if self._stack_status() is not None:
+                raise NotImplementedError("sliders_b200: training or a gradient w.r.t. encoder_hidden_states while a "
+                                          "SliderStack slider is active is not implemented (stacks are for inference; "
+                                          "run under torch.no_grad())")
             # training: keep activations and hand torch.autograd a node whose backward runs the sb200 backward kernels
             return self._forward_nograd(sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict,
                                         train=True, ehs_grad=ehs_grad)
@@ -723,6 +906,9 @@ class UNet2DConditionModel(nn.Module):
         scales = [float(a.multiplier) * float(a.scale) for _, a in adapted]
         ranks = tuple(int(a.lora_dim) for _, a in adapted)
         nz = [s for s in scales if s != 0.0]
+        if "_slider_stack" in self.__dict__ and self._stack_status() is not None:
+            # the stack's layout, not its multipliers (device-side): one graph serves every combination of scales
+            return (tuple(s != 0.0 for s in scales), ranks, None, self.__dict__["_slider_stack"].structure), None
         if not nz:
             return (tuple(False for _ in scales), ranks, None), None
         if all(abs(s - nz[0]) < 1e-12 for s in nz):
@@ -734,6 +920,11 @@ class UNet2DConditionModel(nn.Module):
         for _, a in self._adapted_leaves():
             if float(a.multiplier) * float(a.scale) != 0.0 and a.lora_down.weight.requires_grad:
                 return True
+        stack = self.__dict__.get("_slider_stack")
+        if stack is not None:
+            for net, m in zip(stack.sliders, self._stack_status() or ()):
+                if m != 0.0 and any(p.requires_grad for p in net.parameters()):
+                    return True
         return False
 
     def _graphed(self, x, t, ehs, added, out_dtype):
@@ -778,6 +969,8 @@ class _GraphInputs:
         _, common = unet._lora_signature()
         if unet._slider_scale_dev is not None:
             unet._slider_scale_dev.fill_(1.0 if common is None else common)
+        if "_slider_stack" in unet.__dict__:
+            unet._stack_begin(compose=False)  # per-slider multipliers; the graph's own compose applies them
         unet._bake_scales = bake
         try:
             unet._refresh_lora_packs()

@@ -27,10 +27,12 @@ def _note_lora(lora):
 
 
 def _lora_slots(leaves):
-    """Stand-in for UNet2DConditionModel._lora: the (slot width r, rt) that ops.lora_slots gives the call's adaptors."""
-    from sliders_b200.unet import _adaptor_of
+    """Stand-in for UNet2DConditionModel._lora: the (slot width r, rt) that ops.lora_slots gives the call's adaptors.
+    A leaf of a SliderStack takes the stack's composite slot, as wide as its total rank."""
+    from sliders_b200.unet import _adaptor_of, _hook_of
 
     ranks = [int(a.lora_dim) for a in map(_adaptor_of, leaves) if a is not None]
+    ranks += [h.stack.total_rank for h in map(_hook_of, leaves) if h is not None]
     if not ranks:
         return None
     r, rt = ops.lora_slots(max(ranks), len(leaves))
