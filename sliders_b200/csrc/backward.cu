@@ -1177,6 +1177,7 @@ extern "C" int sb200_adamw(void* handle, void* stream, const void* table, int n_
   pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && table && n_tensors > 0 && max_numel > 0 && step >= 1, "adamw: arguments");
+  SB200_REQUIRE(n_tensors <= 65535, "adamw: %d tensors exceed the grid's 65535 y-blocks", n_tensors);
   static_assert(sizeof(AdamTensor) == 40, "AdamTensor layout");
   const double bc1 = 1.0 - pow(beta1, static_cast<double>(step));
   const double bc2 = 1.0 - pow(beta2, static_cast<double>(step));
@@ -1194,6 +1195,7 @@ extern "C" int sb200_adam_f32(void* handle, void* stream, const void* table, int
   pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && table && n_tensors > 0 && max_numel > 0 && step >= 1, "adam_f32: arguments");
+  SB200_REQUIRE(n_tensors <= 65535, "adam_f32: %d tensors exceed the grid's 65535 y-blocks", n_tensors);
   const double bc1 = 1.0 - pow(beta1, step), bc2 = 1.0 - pow(beta2, step);
   const int bx = grid_for(static_cast<size_t>(max_numel), 256, ctx->num_sms);
   SB200_CUDA_CHECK(launch_pdl(adam_f32_kernel, dim3(bx, n_tensors), dim3(256), 0, static_cast<cudaStream_t>(stream),

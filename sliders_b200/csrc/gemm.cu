@@ -1176,6 +1176,9 @@ extern "C" int sb200_gemm_splitk_f32(void* handle, void* stream, const void* x, 
   SB200_REQUIRE(M > 0 && N > 0 && K > 0 && N % 16 == 0, "gemm_splitk_f32: bad dims M=%d N=%d K=%d", M, N, K);
   SB200_REQUIRE(K % 8 == 0 && ldx % 8 == 0 && ldw % 8 == 0 && ldo % 4 == 0,
                 "gemm_splitk_f32: K and the bf16 leading dims must be multiples of 8, ldo of 4");
+  // the split tiles store 16-byte vectors to ws and the reduction 16-byte vectors to out
+  SB200_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0 && (reinterpret_cast<uintptr_t>(ws) & 15) == 0,
+                "gemm_splitk_f32: out and ws must be 16-byte aligned");
   const size_t need = SB200_GEMM_SPLITK_WS_FLOATS(M, N, K);
   SB200_REQUIRE(ws_floats >= need, "gemm_splitk_f32: scratch of %zu floats, %zu needed", ws_floats, need);
   GemmParams p;

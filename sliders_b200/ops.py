@@ -411,12 +411,16 @@ def splitk_ws_floats(M: int, N: int, K: int) -> int:
 
 
 def gemm_splitk_f32(x: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """fp32 out[M, N] = x[M, K] @ w[N, K].T (bf16 operands): `gemm_kernel` in split-K mode + `splitk_reduce_kernel`."""
+    """fp32 out[M, N] = x[M, K] @ w[N, K].T (bf16 operands): `gemm_kernel` in split-K mode + `splitk_reduce_kernel`.
+    `out`: an fp32 [M, N] row-strided matrix on x's device (e.g. a column slice of a wider buffer)."""
     M, K = x.shape
     N = w.shape[0]
     assert w.shape[1] == K
     if out is None:
         out = torch.empty((M, N), device=x.device, dtype=torch.float32)
+    _row_matrix(out, (M, N), "gemm_splitk_f32", dtype=torch.float32)
+    if out.device != x.device:
+        raise ValueError(f"gemm_splitk_f32: out is on {out.device}, x on {x.device}")
     n_ws = splitk_ws_floats(M, N, K)
     ws = torch.empty(n_ws, device=x.device, dtype=torch.float32)
     lib = _begin()

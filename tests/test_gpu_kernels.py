@@ -553,3 +553,35 @@ def test_bad_arguments_return_errors_not_crashes(dev):
         ops.attention_bwd(q, q, q, q, q, lse, 1, 2, 64, 64, 0.125, 64, torch.zeros(128, 64, device=dev, dtype=BF))
     with pytest.raises(ValueError, match="row-strided"):
         ops.layernorm_bwd(q, q[0], q, out=q.t())
+
+
+def test_splitk_and_optimizer_arguments_return_errors(dev):
+    """The split-K GEMM stores 16-byte vectors to out and ws: a misaligned pointer is refused on the host, before any
+    launch; the optimisers refuse more tensors than the grid's y dimension holds."""
+    from sliders_b200 import _cabi, ops
+    from test_gpu_backward_bounds import _lib_call
+
+    M, N, K = 77, 64, 128
+    x = torch.zeros(M, K, device=dev, dtype=BF)
+    w = torch.zeros(N, K, device=dev, dtype=BF)
+    wide = torch.zeros(M, N + 8, device=dev)
+    with pytest.raises(_cabi.Sb200Error, match="16-byte aligned"):   # ldo = 72 is fine, the start 8 bytes off
+        ops.gemm_splitk_f32(x, w, out=wide[:, 2:2 + N])
+    n_ws = ops.splitk_ws_floats(M, N, K)
+    ws = torch.zeros(n_ws + 4, device=dev)
+    out = torch.zeros(M, N, device=dev)
+    with pytest.raises(_cabi.Sb200Error, match="16-byte aligned"):
+        _lib_call("sb200_gemm_splitk_f32", ops._p(x), K, ops._p(w), K, ops._p(out), N, M, N, K, ops._p(ws[1:]), n_ws)
+    with pytest.raises(ValueError, match="row-strided"):
+        ops.gemm_splitk_f32(x, w, out=torch.zeros(M, N, device=dev, dtype=BF))
+    with pytest.raises(ValueError, match="row-strided"):
+        ops.gemm_splitk_f32(x, w, out=torch.zeros(N, M, device=dev).t())
+    with pytest.raises(ValueError, match="is on cpu"):
+        ops.gemm_splitk_f32(x, w, out=torch.zeros(M, N))
+    table = torch.zeros(1, 5, device=dev, dtype=torch.int64)
+    with pytest.raises(_cabi.Sb200Error, match="65535"):
+        ops.adamw(table, 65536, 1, 1e-3, 0.9, 0.999, 1e-8, 0.0, 1)
+    with pytest.raises(_cabi.Sb200Error, match="65535"):
+        ops.adam_f32(table, 65536, 1, 1e-3, 0.9, 0.999, 1e-8, 0.0, 1)
+    torch.cuda.synchronize()
+    assert torch.equal(out, torch.zeros_like(out)) and torch.equal(ws, torch.zeros_like(ws))
