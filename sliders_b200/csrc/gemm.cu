@@ -560,8 +560,8 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
 // -------------------------------------------------------------------------------------------------
 // Wide tiles: a persistent kernel for layers whose W has a multiple of 256 rows
 // -------------------------------------------------------------------------------------------------
-// gemm_wide_kernel<RT>: 128 x 256 tiles (GEGLU: 256 W rows, 128 output columns), 384 threads, one CTA per SM, each CTA
-// walking the tiles blockIdx.x, blockIdx.x + gridDim.x, ... in launch_gemm's order:
+// gemm_wide_kernel<RT, GEGLU>: 128 x 256 tiles (GEGLU: 256 W rows, 128 output columns), 384 threads, one CTA per SM,
+// each CTA walking the tiles blockIdx.x, blockIdx.x + gridDim.x, ... in launch_gemm's order:
 //   warpgroup 2    producer: gives its registers to the consumers (setmaxnreg 40); one elected thread of warp 8 issues
 //                  the TMA loads, running ahead into the next tile while the consumers finish the current epilogue
 //   warpgroups 0/1 consumers (setmaxnreg 232): rows 0..63 / 64..127, an m64 x 256 accumulator of 128 registers
@@ -570,7 +570,12 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
 // order and with its expressions, the LoRA update, bias, row bias and GEGLU, rounds to bf16, adds the residual in bf16,
 // and leaves through a swizzled staging buffer (two per warpgroup, 64 rows x 64 columns each) with coalesced stores.
 // Only t = A.down^T and the tile's lora_up rows are staged in shared memory.  No split-K or CTA pairs: those stay on
-// gemm_kernel.
+// gemm_kernel.  GEGLU is a template parameter (only with RT = 0: GEGLU never comes with LoRA) rather than a flag: with
+// a runtime flag every element's gate code sat between the plain path's instructions and the chunk loop spanned
+// ~29 KB of SASS; a chunk took 2 000-2 500 cycles for 32 elements per thread with no global access on the way (clock64
+// stamps per phase on an H100 SXM at 700 W), far above its instruction count and in line with instruction fetch from
+// a loop that does not stay in the instruction cache.  Split, and with 16-byte output stores, a plain tile's epilogue
+// takes half the cycles (DESIGN §8 item 1).
 constexpr int kWideBN = 256;
 constexpr int kWideThreads = 384;
 constexpr int kWideChunk = 64;                        // output columns per staging buffer
@@ -600,7 +605,7 @@ __device__ __forceinline__ int tile_out_row(const GemmParams& p, int st, int r) 
   return (ib < p.bb && b < p.B && h < p.H && w < p.W) ? (b * p.H + h) * p.W + w : -1;
 }
 
-template <int RT>
+template <int RT, bool GEGLU>
 __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid_constant__ GemmParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
@@ -613,7 +618,7 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
   const uint32_t stage_bytes = static_cast<uint32_t>(p.stage_bytes);
   constexpr uint32_t a_bytes = kBM * 128;
   constexpr uint32_t b_bytes = kWideBN * 128;
-  const bool geglu = (p.flags & SB200_EPI_GEGLU) != 0;
+  constexpr bool geglu = GEGLU;
   const int num_tiles = p.num_m_tiles * p.num_n_tiles;
 
   if (threadIdx.x == 0) {
@@ -680,7 +685,7 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
   const bool has_rb = (p.flags & SB200_EPI_ROWBIAS) != 0;
   const int r = has_lora ? p.lora_r : 0;
   const float lscale = has_lora ? (p.lora_scale_dev ? p.lora_scale * __ldg(p.lora_scale_dev) : p.lora_scale) : 0.f;
-  const int nchunks = p.ncols_out / kWideChunk;  // 4, or 2 with GEGLU
+  constexpr int nchunks = (GEGLU ? kWideBN / 2 : kWideBN) / kWideChunk;  // p.ncols_out / kWideChunk
   const uint32_t epi = tiles + static_cast<uint32_t>(S) * stage_bytes +
                        static_cast<uint32_t>(wg) * static_cast<uint32_t>(wide_epi_bytes(RT, r));
   const uint32_t tbuf = epi + 2 * kWideStgBytes;  // [64][RT + 4] fp32: t of this warpgroup's rows
@@ -696,6 +701,31 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
   for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
     const int mt = p.n_fast ? t / p.num_n_tiles : t % p.num_m_tiles;
     const int nt = p.n_fast ? t % p.num_n_tiles : t / p.num_m_tiles;
+    const int st = mt;
+    const int n_base = nt * p.ncols_out;
+    int orow[4];  // output rows this thread copies
+#pragma unroll
+    for (int i = 0; i < 4; ++i) orow[i] = tile_out_row(p, st, wg * 64 + crow + 16 * i);
+    auto prefetch_resid = [&](int c, uint32_t buf) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int row = crow + 16 * i;
+        if (orow[i] >= 0)
+          cp_async_16(buf + row * 128 + ((cch ^ (row & 7)) << 4),
+                      p.resid + static_cast<size_t>(orow[i]) * p.ldr + n_base + c * kWideChunk + cch * 8);
+      }
+      cp_async_commit();
+    };
+    // The tile's lora_up rows and its first residual chunk are loaded while its k-blocks run, so that the epilogue
+    // does not start with a global-memory round trip.  Their buffers are free once every thread of the warpgroup is
+    // done with the previous tile's epilogue.
+    wg_sync();
+    if constexpr (RT != 0) {
+      const float* up_src = p.lora_up + static_cast<size_t>(n_base) * r;
+      for (int i = tid; i < kWideBN * r / 4; i += 128) cp_async_16(ubuf + i * 16, up_src + i * 4);
+      cp_async_commit();
+    }
+    if (has_resid) prefetch_resid(0, epi);
     float acc[kWideBN / 2];
     float accl[RT ? RT / 2 : 1];
 #pragma unroll
@@ -734,24 +764,8 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
     for (int i = 0; i < (RT ? RT / 2 : 1); ++i) reg_fence(accl[i]);
 
     // ------------------------------------------------------------------ epilogue
-    const int st = mt;
-    const int n_base = nt * p.ncols_out;
-    int orow[4];  // output rows this thread copies
-#pragma unroll
-    for (int i = 0; i < 4; ++i) orow[i] = tile_out_row(p, st, wg * 64 + crow + 16 * i);
-    auto prefetch_resid = [&](int c, uint32_t buf) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int row = crow + 16 * i;
-        if (orow[i] >= 0)
-          cp_async_16(buf + row * 128 + ((cch ^ (row & 7)) << 4),
-                      p.resid + static_cast<size_t>(orow[i]) * p.ldr + n_base + c * kWideChunk + cch * 8);
-      }
-      cp_async_commit();
-    };
-    wg_sync();  // every thread of the warpgroup is done with the previous tile's staging, t and lora_up buffers
     if constexpr (RT != 0) {
-      // t = A.down^T of this warpgroup's rows (fragment layout as in wgmma.cuh), and the tile's lora_up rows
+      // t = A.down^T of this warpgroup's rows (fragment layout as in wgmma.cuh)
 #pragma unroll
       for (int i = 0; i < RT / 2; i += 2) {
         const int row = fr0 + 8 * ((i >> 1) & 1);
@@ -760,11 +774,7 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
                      "f"(accl[i + 1])
                      : "memory");
       }
-      const float* up_src = p.lora_up + static_cast<size_t>(n_base) * r;
-      for (int i = tid; i < kWideBN * r / 4; i += 128) cp_async_16(ubuf + i * 16, up_src + i * 4);
-      cp_async_commit();
     }
-    if (has_resid) prefetch_resid(0, epi);
     if (has_resid || has_lora) {
       cp_async_wait<0>();
       wg_sync();
@@ -779,8 +789,8 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
     }
     float tl[2][8];  // lscale * t of the current adaptor, rows fr0 and fr0 + 8
     int cur_grp = -1;
-    // A runtime loop over the chunks keeps one copy of the epilogue code (unrolled four times it outgrows the
-    // instruction cache); each pass first selects its chunk's 32 accumulator registers (and 32 gate registers).
+    // A runtime loop over the chunks keeps one copy of the epilogue code (unrolled it outgrows the instruction cache);
+    // each pass first selects its chunk's 32 accumulator registers (and with GEGLU its 32 gate registers).
 #pragma unroll 1
     for (int c = 0; c < nchunks; ++c) {
       {
@@ -870,8 +880,7 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
           const int row = crow + 16 * i;
           const uint4 v = ld_shared_v4(buf + row * 128 + ((cch ^ (row & 7)) << 4));
           if (orow[i] >= 0)
-            *reinterpret_cast<uint4*>(p.out + static_cast<size_t>(orow[i]) * p.ldo + n_base + c * kWideChunk +
-                                      cch * 8) = v;
+            st_global_v4(p.out + static_cast<size_t>(orow[i]) * p.ldo + n_base + c * kWideChunk + cch * 8, v);
         }
       }
     }
@@ -922,21 +931,23 @@ static bool wide_eligible(int N, int ctas, int lora_r, int lora_rt) {
 // 8192 x 1280 x 5120 + residual 293 / 245, 8192 x 3840 x 1280 LoRA 299 / 241, 32768 x 5120 x 640 GEGLU 833 / 625,
 // 32768 x 1920 x 640 LoRA 361 / 315, 32768 x 640 x 640 LoRA + residual 137 / 131, 616 x 153600 x 2048 1225 / 949,
 // LoRA convs 32x32 1280 -> 1280 850 / 620, 64x64 640 -> 640 831 / 630, 128x128 320 -> 320 881 / 832 (B = 8).
-// gemm_wide_kernel in the same units: 4 (256 + rt) + kWidePerKb cycles per k-block, kWideTile per tile (epilogue and
-// pipeline refill; the wide epilogue does not overlap the tensor cores), kWideLoraTile more per tile with LoRA, and
-// the fixed cost once per CTA.  Fitted to the same shapes timed with each width forced on an H100 80GB HBM3 SXM at
-// 700 W (us, BN 64 / 128 / 256): 8192 x 10240 x 1280 GEGLU 616 / 459 / 429, 8192 x 1280 x 5120 + residual
-// 268 / 215 / 179, 32768 x 5120 x 640 GEGLU 812 / 557 / 552, 616 x 153600 x 2048 1099 / 749 / 653,
-// 8192 x 1280 x 1280 bias 70 / 64 / 65, 8192 x 3840 x 1280 LoRA 240 / 209 / 245, 8192 x 1280 x 1280 LoRA + residual
-// 93 / 85 / 101, LoRA convs 32x32 1280 -> 1280 676 / 462 / 480, 2560 -> 1280 1502 / 933 / 1175 (B = 8); SD-1.5 at
-// B = 1 (CFG pair): 512 x 1280 x 1280 + residual 9.8 / 13.7 / 22.2, 512 x 3840 x 1280 LoRA 19.7 / 15.3 / 32.0,
-// 512 x 10240 x 1280 GEGLU 47.3 / 44.1 / 43.2, 2048 x 5120 x 640 GEGLU 54.4 / 42.7 / 45.1, convs 16x16 and 8x8
-// 1280 -> 1280 + residual 72 / 84 / 117 and 71 / 84 / 116.  The wide tile wins on the GEGLU, deep-K and many-tile
-// shapes and loses with LoRA and on grids of few tiles; the fit reproduces every choice but the 512 x 10240 GEGLU tie.
-constexpr double kWidePerKb = 136.0;
-constexpr double kWideTile = 6500.0;
-constexpr double kWideLoraTile = 40000.0;
-constexpr double kWideFixed = 1500.0;
+// gemm_wide_kernel in the same units: 4 (256 + rt) cycles per k-block, kWideLoraPerKb more with LoRA, and kWideTile per
+// tile (epilogue and pipeline refill; the wide epilogue does not overlap the tensor cores).  Fitted to the same shapes
+// timed with each width forced on an H100 80GB HBM3 SXM at 700 W, each wide time scaled by the BN = 128 model's cycles
+// over the BN = 128 time of the same shape so that the choice compares like with like (us, BN 64 / 128 / 256): 8192 x
+// 10240 x 1280 GEGLU 583 / 437 / 389, 8192 x 1280 x 5120 + residual 274 / 214 / 169, 32768 x 5120 x 640 GEGLU 742 / 525
+// / 476, 616 x 153600 x 2048 1104 / 734 / 587, 8192 x 1280 x 1280 bias 72.7 / 61.7 / 54.7, the same + residual 79.3 /
+// 69.7 / 57.9, 8192 x 3840 x 1280 LoRA 239 / 202 / 183, 8192 x 1280 x 1280 LoRA + residual 91.5 / 82.0 / 71.8, LoRA
+// convs 32x32 1280 -> 1280 + residual 677 / 456 / 462, 2560 -> 1280 1515 / 937 / 1121, 8192 x 1280 x 2560 LoRA (two
+// sources) - / 123 / 131 (B = 8); SD-1.5 at B = 1 (CFG pair): 512 x 1280 x 1280 + residual 10.9 / 13.3 / 18.6, 512 x
+// 3840 x 1280 LoRA 19.8 / 15.1 / 23.8, 512 x 10240 x 1280 GEGLU 46.2 / 42.4 / 39.3, 2048 x 5120 x 640 GEGLU 51.0 / 40.4
+// / 40.2, convs 16x16 and 8x8 1280 -> 1280 + residual 73 / 83 / 111 and 73 / 82 / 110.  A LoRA k-block costs the wide
+// tile more than its 16 extra columns (there the LoRA ring has three stages, gemm_kernel's six; the cause was not
+// measured), so LoRA wins on the wide tile only where it saves waves at moderate K: the q|k|v and attention-out
+// projections, not the deep-K LoRA convs or the 2.4-wave K = 2560 shortcut. The fit reproduces every choice but the 512
+// x 10240 GEGLU, which stays at 128 (8 % slower than 256).
+constexpr double kWideTile = 5400.0;
+constexpr double kWideLoraPerKb = 370.0;
 static TileChoice pick_tile(int ncols, int num_sms, int kblocks, int lora_r, int lora_rt, int force_ctas, int sub_tiles,
                             int flags) {
   double best = -1;
@@ -951,9 +962,8 @@ static TileChoice pick_tile(int ncols, int num_sms, int kblocks, int lora_r, int
     const int cols_out = geglu ? bn / 2 : bn;
     double cost;
     if (bn == kWideBN) {
-      // persistent, one CTA per SM: the fixed cost once per CTA
-      cost = load * (kblocks * (4.0 * (bn + lora_rt) + kWidePerKb) + kWideTile + (lora_rt ? kWideLoraTile : 0.0)) +
-             kWideFixed;
+      // persistent, one CTA per SM
+      cost = load * (kblocks * (4.0 * (bn + lora_rt) + (lora_rt ? kWideLoraPerKb : 0.0)) + kWideTile);
     } else {
       const int slots = gemm_slots(bn, lora_rt);
       const double perkb = 4.0 * (bn + lora_rt) + 208.0;
@@ -1017,17 +1027,17 @@ static int launch_gemm_bn(Ctx* ctx, cudaStream_t stream, const GemmParams& p, in
   return 0;
 }
 
-template <int RT>
+template <int RT, bool GEGLU>
 static int launch_gemm_wide(Ctx* ctx, cudaStream_t stream, const GemmParams& p, int smem) {
   static bool attr_set = false;  // one flag per instantiation
-  const auto kernel = gemm_wide_kernel<RT>;
+  const auto kernel = gemm_wide_kernel<RT, GEGLU>;
   if (!attr_set) {
     SB200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin));
     SB200_CUDA_CHECK(
         cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     int resident = 0;
     SB200_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kernel, kWideThreads, smem));
-    if (resident < 1) return set_error(SB200_ERR_CUDA, "gemm_wide_kernel<%d>: no CTA fits an SM", RT);
+    if (resident < 1) return set_error(SB200_ERR_CUDA, "gemm_wide_kernel<%d, %d>: no CTA fits an SM", RT, GEGLU);
     attr_set = true;
   }
   cudaLaunchConfig_t cfg = {};
@@ -1073,9 +1083,12 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
                   p.lora_r, rt);
     int st;
     switch (rt) {
-      case 0: st = launch_gemm_wide<0>(ctx, stream, p, smem); break;
-      case 16: st = launch_gemm_wide<16>(ctx, stream, p, smem); break;
-      default: st = launch_gemm_wide<32>(ctx, stream, p, smem); break;
+      case 0:
+        st = (p.flags & SB200_EPI_GEGLU) ? launch_gemm_wide<0, true>(ctx, stream, p, smem)
+                                         : launch_gemm_wide<0, false>(ctx, stream, p, smem);
+        break;
+      case 16: st = launch_gemm_wide<16, false>(ctx, stream, p, smem); break;
+      default: st = launch_gemm_wide<32, false>(ctx, stream, p, smem); break;
     }
     if (st) return st;
     SB200_CUDA_CHECK(cudaGetLastError());

@@ -202,6 +202,11 @@ __device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint4& v) {
   asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
                : "memory");
 }
+// One 16-byte global store.  Spelled out because NVVM splits a `*reinterpret_cast<uint4*>(p) = v` whose value comes
+// from ld_shared_v4 into four 4-byte stores in gemm_wide_kernel (each a partial-sector write to L2).
+__device__ __forceinline__ void st_global_v4(void* ptr, const uint4& v) {
+  asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(ptr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
 __device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
   uint32_t v;
   asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
