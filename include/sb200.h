@@ -38,7 +38,8 @@ enum {
   SB200_EPI_ROWBIAS = 2,  /* + rowbias[(m / rows_per_batch) * N + n]   (ResnetBlock2D time-embedding add) */
   SB200_EPI_RESID = 4,    /* + resid[m * ldr + n] */
   SB200_EPI_GEGLU = 8,    /* out[m, j] = acc[m, j] * gelu_erf(acc[m, N/2 + j]),  j < N/2 */
-  SB200_EPI_LORA = 16     /* + scale * (X . down^T) . up^T, rank r, computed in the same tile loop */
+  SB200_EPI_LORA = 16     /* + scale [* sample_scale[m / rows_per_sample]] * (X . down^T) . up^T, rank r, computed in
+                             the same tile loop */
 };
 
 /* ABI / build identification: "sb200 <version> sm_90a". */
@@ -60,7 +61,13 @@ int sb200_destroy(void* handle);
  *   scale: multiplier * alpha / rank, a run-time scalar (the slider value changes per denoise step,
  *          eval-scripts/generate_images_xl.py:327-330).
  *   scale_dev: optional device pointer to one float multiplied into scale when the kernel runs, so a
- *          captured CUDA graph can be replayed with a different slider value (NULL = unused). */
+ *          captured CUDA graph can be replayed with a different slider value (NULL = unused).
+ *   sample_scale: optional device fp32 vector of per-sample factors (NULL = unused): output row m of the LoRA term is
+ *          multiplied by sample_scale[m / rows_per_sample] on top of scale (and *scale_dev), so one batched launch can
+ *          run every batch entry at its own slider value.  The caller sizes it to M / rows_per_sample entries.
+ *   rows_per_sample: output rows per batch entry when sample_scale != NULL (tokens per sample: H * W of a transformer
+ *          block, 77 for the text context, Ho * Wo of a conv, 1 for sb200_small_linear); it must be > 0 and divide M,
+ *          else the launcher returns SB200_ERR_INVALID.  Ignored when sample_scale is NULL. */
 typedef struct sb200_lora {
   const void* down;
   const void* up;
@@ -69,6 +76,8 @@ typedef struct sb200_lora {
   int group_n;
   float scale;
   const float* scale_dev;
+  const float* sample_scale;
+  int rows_per_sample;
 } sb200_lora;
 
 /* out[M, N] = epilogue( X[M, K] . W[N, K]^T )  — every nn.Linear on the path and the 1x1 conv_shortcut.

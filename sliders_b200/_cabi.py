@@ -29,6 +29,8 @@ class LoraArgs(C.Structure):
         ("group_n", C.c_int),
         ("scale", C.c_float),
         ("scale_dev", C.c_void_p),
+        ("sample_scale", C.c_void_p),
+        ("rows_per_sample", C.c_int),
     ]
 
 

@@ -128,6 +128,11 @@ def _new_tape(unet) -> list:
     for leaf, a in unet._adapted_leaves():
         s = float(a.multiplier) * float(a.scale)
         if s != 0.0:
+            if getattr(a, "sample_scales", None) is not None:
+                # the backward kernels (lora_wgrad, lora_rank_update and their conv forms) take one scale per launch
+                raise NotImplementedError("sliders_b200: a gradient through a forward with per-sample slider scales is "
+                                          "not implemented (per-sample scales are for inference; set a scalar with "
+                                          "set_lora_slider, or run under torch.no_grad())")
             scales[id(leaf)] = (a, s, bool(a.lora_down.weight.requires_grad))
     return [("scales", scales)]
 

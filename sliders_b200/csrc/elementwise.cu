@@ -48,6 +48,8 @@ struct SmallLinearArgs {
   int r, group_n;
   float scale;
   const float* scale_dev;
+  const float* sample_scale;  // per-sample factors (NULL = none): row m uses [m / rows_per_sample]
+  int rows_per_sample;
 };
 
 __device__ __forceinline__ float dot8(const uint4& a, const uint4& b, bool silu_a) {
@@ -67,7 +69,9 @@ __device__ __forceinline__ float dot8(const uint4& a, const uint4& b, bool silu_
   return s;
 }
 
-__global__ void __launch_bounds__(kSlWarps * 32) small_linear_kernel(SmallLinearArgs a) {
+// five CTAs per SM (48 registers, no spills): without the bound, the per-sample factor's loads, hoisted out of the
+// unrolled row loop, would take the kernel to 62 registers and four CTAs per SM
+__global__ void __launch_bounds__(kSlWarps * 32, 5) small_linear_kernel(SmallLinearArgs a) {
   pdl_trigger();
   pdl_wait();
   // LoRA down-projection of every row, [M][groups * r]: a block's kSlWarps * kSlColsPerWarp columns touch at most two
@@ -131,7 +135,9 @@ __global__ void __launch_bounds__(kSlWarps * 32) small_linear_kernel(SmallLinear
             float l = 0.f;
             for (int j = 0; j < a.r; ++j)
               l += t_sh[m0 + i][gj + j] * a.up[static_cast<size_t>(n) * a.r + j];
-            y += (a.scale_dev ? a.scale * __ldg(a.scale_dev) : a.scale) * l;
+            float s = a.scale_dev ? a.scale * __ldg(a.scale_dev) : a.scale;
+            if (a.sample_scale) s *= __ldg(a.sample_scale + (m0 + i) / a.rows_per_sample);
+            y += s * l;
           }
           if (a.act_out == 1) y = silu_f(y);
           if (a.resid) y += __bfloat162float(a.resid[static_cast<size_t>(m0 + i) * a.N + n]);
@@ -416,6 +422,10 @@ extern "C" int sb200_small_linear(void* handle, void* stream, const void* x, int
     a.group_n = lora->group_n;
     a.scale = lora->scale;
     a.scale_dev = lora->scale_dev;
+    SB200_REQUIRE(!lora->sample_scale || (lora->rows_per_sample > 0 && M % lora->rows_per_sample == 0),
+                  "small_linear: lora rows_per_sample=%d must be positive and divide M=%d", lora->rows_per_sample, M);
+    a.sample_scale = lora->sample_scale;
+    a.rows_per_sample = lora->rows_per_sample;
   }
   const int cols_per_block = kSlWarps * kSlColsPerWarp;
   SB200_CUDA_CHECK(launch_pdl(small_linear_kernel, dim3((N + cols_per_block - 1) / cols_per_block),

@@ -100,6 +100,8 @@ struct GemmParams {
   int lora_r, lora_rt, lora_group_n;
   float lora_scale;
   const float* lora_scale_dev;
+  const float* lora_sample_scale;  // per-sample factors (NULL = none): row m uses [m / lora_rows_per_sample]
+  int lora_rows_per_sample;
   // split-K (sb200_gemm_splitk_f32): grid y = split index; split s runs k-blocks [s * sk_kb, (s + 1) * sk_kb) and stores
   // its raw fp32 tile to sk_ws[s][M][N] instead of running the epilogue
   float* sk_ws;
@@ -384,8 +386,6 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
 
     const int q = warp & 3;      // 32-row quarter of the tile this warp writes
     const int hsel = warp >> 2;  // which of the kEpiPerQuarter warps of this quarter (slab index mod that)
-    const float lscale =
-        has_lora ? (p.lora_scale_dev ? p.lora_scale * __ldg(p.lora_scale_dev) : p.lora_scale) : 0.f;
     const bool has_resid = (p.flags & SB200_EPI_RESID) != 0;
     // per-warp staging buffer ([32 rows x 32 cols] bf16, 64 B rows, 16-byte chunks XOR-swizzled by (row >> 1) & 3):
     // residual tiles arrive here by cp.async with coalesced global reads, results leave from here with coalesced global
@@ -417,6 +417,10 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
       }
     }
     const bool row_ok = my_row >= 0;
+    float lscale = has_lora ? (p.lora_scale_dev ? p.lora_scale * __ldg(p.lora_scale_dev) : p.lora_scale) : 0.f;
+    // this thread's row factor, read once per tile; without a vector nothing is loaded and lscale keeps its bits
+    if (has_lora && p.lora_sample_scale != nullptr && row_ok)
+      lscale *= __ldg(p.lora_sample_scale + my_row / p.lora_rows_per_sample);
     const int n_base = nt * p.ncols_out;
     const int ncols_valid = min(p.ncols_out, p.Nout - n_base);
     const int nslabs = (ncols_valid + kSlab - 1) / kSlab;
@@ -787,7 +791,16 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
         rb[h] = p.rowbias + static_cast<size_t>(orw >= 0 ? orw / p.rows_per_batch : 0) * p.Nout;
       }
     }
-    float tl[2][8];  // lscale * t of the current adaptor, rows fr0 and fr0 + 8
+    // lscale with the per-sample factors of rows fr0 and fr0 + 8, read once per tile outside the chunk loop
+    float lsc[2] = {lscale, lscale};
+    if (RT != 0 && p.lora_sample_scale != nullptr) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int orw = tile_out_row(p, st, wg * 64 + fr0 + 8 * h);
+        if (orw >= 0) lsc[h] *= __ldg(p.lora_sample_scale + orw / p.lora_rows_per_sample);
+      }
+    }
+    float tl[2][8];  // lsc * t of the current adaptor, rows fr0 and fr0 + 8
     int cur_grp = -1;
     // A runtime loop over the chunks keeps one copy of the epilogue code (unrolled it outgrows the instruction cache);
     // each pass first selects its chunk's 32 accumulator registers (and with GEGLU its 32 gate registers).
@@ -819,7 +832,7 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
                 const uint4 b = r == 8 ? ld_shared_v4(ta + 16) : make_uint4(0, 0, 0, 0);
                 const uint32_t tv[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
 #pragma unroll
-                for (int jt = 0; jt < 8; ++jt) tl[h][jt] = __uint_as_float(tv[jt]) * lscale;
+                for (int jt = 0; jt < 8; ++jt) tl[h][jt] = __uint_as_float(tv[jt]) * lsc[h];
               }
             }
 #pragma unroll
@@ -1131,7 +1144,7 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
   return 0;
 }
 
-static int check_lora(const sb200_lora* l, int N) {
+static int check_lora(const sb200_lora* l, int M, int N) {
   SB200_REQUIRE(l->down && l->up, "lora: NULL weights");
   SB200_REQUIRE(l->r == 4 || l->r == 8 || l->r == 16,
                 "lora: slot width %d unsupported by the fused epilogue (4, 8 or 16; pad lower ranks with zeros)", l->r);
@@ -1139,6 +1152,8 @@ static int check_lora(const sb200_lora* l, int N) {
   SB200_REQUIRE(l->group_n > 0 && l->group_n % 16 == 0, "lora: group_n must be a multiple of 16");
   const int groups = (N + l->group_n - 1) / l->group_n;
   SB200_REQUIRE(groups * l->r <= l->rt, "lora: %d groups of rank %d exceed rt=%d", groups, l->r, l->rt);
+  SB200_REQUIRE(!l->sample_scale || (l->rows_per_sample > 0 && M % l->rows_per_sample == 0),
+                "lora: rows_per_sample=%d must be positive and divide M=%d", l->rows_per_sample, M);
   return 0;
 }
 
@@ -1156,6 +1171,8 @@ static void fill_lora(GemmParams& p, const sb200_lora* lora) {
   p.lora_group_n = lora->group_n;
   p.lora_scale = lora->scale;
   p.lora_scale_dev = lora->scale_dev;
+  p.lora_sample_scale = lora->sample_scale;
+  p.lora_rows_per_sample = lora->rows_per_sample;
 }
 
 // out[m, n] = sum over s (in order) of ws[s][m][n]; four columns per thread
@@ -1271,7 +1288,7 @@ extern "C" int sb200_gemm(void* handle, void* stream, const void* x0, int ldx0, 
   p.a_tx = kBM * 128;
   p.num_sub = (M + kBM - 1) / kBM;
   if (has_lora) {
-    int st = check_lora(lora, N);
+    int st = check_lora(lora, M, N);
     if (st) return st;
     fill_lora(p, lora);
   }
@@ -1397,7 +1414,7 @@ extern "C" int sb200_conv3x3(void* handle, void* stream, const void* x0, int ldx
   p.num_sub = p.tiles_w * p.tiles_h * ((B + bb - 1) / bb);
   p.a_tx = bw * bh * bb * 128;
   if (has_lora) {
-    int st = check_lora(lora, Cout);
+    int st = check_lora(lora, M, Cout);
     if (st) return st;
     fill_lora(p, lora);
   }

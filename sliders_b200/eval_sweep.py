@@ -79,12 +79,15 @@ def sweep(unet, network, scheduler, rows: Sequence[dict], embed: Callable[[str],
           scales: Sequence[float] = SCALES, num_samples: int = 1, num_inference_steps: int = 50,
           guidance_scale: float = 5.0, start_noise: int = 750, image_size: int = 1024, xl: bool = True,
           decode: Optional[Callable[[torch.Tensor], list]] = None, dtype=torch.bfloat16,
-          fixed_scales: Sequence[float] = ()) -> int:
+          fixed_scales: Sequence[float] = (), scales_per_batch: int = 1) -> int:
     """For every CSV row and every scale: same seed -> same initial noise -> `denoise_loop` with the slider gated on
     `t <= start_noise` -> `<save_dir>/<scale>/<case>_<sample>.pt` (+ .png through `decode`).  Returns the number of
     latents written.  `embed(prompt)` -> (prompt_embeds [2,77,D] as (negative ; positive), add_text_embeds [2,1280] | None).
     fixed_scales: with a `lora.SliderStack` as `network`, the scales of its second, third, ... sliders, held while the
-    first one sweeps `scales`."""
+    first one sweeps `scales`.
+    scales_per_batch: K > 1 denoises K scales of a row in one batch after running their shared steps once
+    (`generate.scale_sweep`); the files written are the same, their latents agree with K = 1 up to the last bits (see
+    scale_sweep).  A LoRANetwork only."""
     dev = next(unet.parameters()).device
     for s in scales:
         os.makedirs(os.path.join(save_dir, str(s)), exist_ok=True)
@@ -97,13 +100,24 @@ def sweep(unet, network, scheduler, rows: Sequence[dict], embed: Callable[[str],
             ids = torch.tensor([[image_size, image_size, 0, 0, image_size, image_size]], dtype=torch.float32, device=dev)
             added = dict(add_text_embeds=ae.to(dev, dtype).repeat_interleave(num_samples, dim=0),
                          add_time_ids=ids.repeat(2 * num_samples, 1))
-        for s in scales:
+        if scales_per_batch > 1:
             scheduler.set_timesteps(num_inference_steps, device=dev)
             lat = initial_latents(row["seed"], num_samples, image_size, image_size, scheduler.init_noise_sigma, dev, dtype)
-            out = generate.denoise_loop(unet, network, scheduler, lat, pe, added.get("add_text_embeds"),
-                                        added.get("add_time_ids"), num_inference_steps=num_inference_steps,
-                                        guidance_scale=guidance_scale,
-                                        scale=[s, *fixed_scales] if fixed_scales else s, start_noise=start_noise)
+            outs = generate.scale_sweep(unet, network, scheduler, lat, pe, added.get("add_text_embeds"),
+                                        added.get("add_time_ids"), scales=scales, scales_per_batch=scales_per_batch,
+                                        num_inference_steps=num_inference_steps, guidance_scale=guidance_scale,
+                                        start_noise=start_noise)
+        for si, s in enumerate(scales):
+            if scales_per_batch > 1:
+                out = outs[si]
+            else:
+                scheduler.set_timesteps(num_inference_steps, device=dev)
+                lat = initial_latents(row["seed"], num_samples, image_size, image_size, scheduler.init_noise_sigma, dev,
+                                      dtype)
+                out = generate.denoise_loop(unet, network, scheduler, lat, pe, added.get("add_text_embeds"),
+                                            added.get("add_time_ids"), num_inference_steps=num_inference_steps,
+                                            guidance_scale=guidance_scale,
+                                            scale=[s, *fixed_scales] if fixed_scales else s, start_noise=start_noise)
             images = decode(out) if decode is not None else None
             for j in range(num_samples):
                 stem = os.path.join(save_dir, str(s), f"{row['case_number']}_{j}")
@@ -149,13 +163,28 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--compose", type=parse_compose, action="append", default=[], metavar="PATH:SCALE",
                    help="another slider held at SCALE while --model_name sweeps its scales (repeatable); the sliders "
                         "run as one lora.SliderStack with --model_name first")
+    p.add_argument("--scales_per_batch", type=int, default=1, metavar="K",
+                   help="denoise K scales of a case in one batch after their shared steps (t > start_noise) run once; "
+                        "a batch size like --num_samples: it changes the latents' last bits and the activation memory "
+                        "(about K times); not with --compose")
     return p
+
+
+def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
+    """build_parser().parse_args plus the checks that span several flags."""
+    p = build_parser()
+    args = p.parse_args(argv)
+    if args.scales_per_batch < 1:
+        p.error(f"--scales_per_batch must be at least 1, got {args.scales_per_batch}")
+    if args.compose and args.scales_per_batch > 1:
+        p.error("--scales_per_batch > 1 needs per-sample slider scales, which a --compose SliderStack does not have")
+    return args
 
 
 def main(argv: Optional[Sequence[str]] = None, xl: bool = True) -> int:
     from .cli import synthetic_embedding
 
-    args = build_parser().parse_args(argv)
+    args = parse_args(argv)
     dev = torch.device(f"cuda:{args.device}")
     dtype = torch.bfloat16   # the reference runs this loop in fp16 (:443); bf16 is the kernels' dtype (DESIGN.md §1)
     load = model_util.load_models_xl if xl else model_util.load_models
@@ -189,6 +218,7 @@ def main(argv: Optional[Sequence[str]] = None, xl: bool = True) -> int:
     n = sweep(unet, network, create_noise_scheduler(args.scheduler), rows, embed, save_dir,
               num_samples=args.num_samples, num_inference_steps=50 if xl else args.ddim_steps,
               guidance_scale=5.0 if xl else args.guidance_scale, start_noise=args.start_noise,
-              image_size=1024 if xl else args.image_size, xl=xl, dtype=dtype, fixed_scales=fixed)
+              image_size=1024 if xl else args.image_size, xl=xl, dtype=dtype, fixed_scales=fixed,
+              scales_per_batch=args.scales_per_batch)
     print(f"wrote {n} latents under {save_dir}")
     return n

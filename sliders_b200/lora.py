@@ -17,6 +17,7 @@ from __future__ import annotations
 
 import math
 import os
+import weakref
 from typing import Dict, List, Literal, Optional, Sequence, Union
 
 import torch
@@ -31,6 +32,8 @@ DEFAULT_TARGET_REPLACE = UNET_TARGET_REPLACE_MODULE_TRANSFORMER
 TRAINING_METHODS = Literal["noxattn", "innoxattn", "selfattn", "xattn", "full", "xattn-strict",
                            "noxattn-hspace", "noxattn-hspace-last"]
 _LEAF_CLASS_NAMES = ("Linear", "Conv2d", "LoRACompatibleLinear", "LoRACompatibleConv")
+# networks inside `with network:` with per-sample slider values: while it is empty the UNet skips looking for them
+PER_SAMPLE_NETWORKS: "weakref.WeakSet" = weakref.WeakSet()
 
 
 class LoRAModule(nn.Module):
@@ -62,6 +65,7 @@ class LoRAModule(nn.Module):
         nn.init.kaiming_uniform_(self.lora_down.weight, a=init_a)  # a=1 text sliders, sqrt(5) image sliders
         nn.init.zeros_(self.lora_up.weight)
         self.multiplier = multiplier
+        self.sample_scales = None  # per-sample slider values inside `with network:` (LoRANetwork.set_lora_slider)
         self.org_module = org_module  # dropped in apply_to, like the reference
 
     def apply_to(self):
@@ -174,15 +178,56 @@ class LoRANetwork(nn.Module):
             torch.save(state_dict, file)
 
     def set_lora_slider(self, scale):
-        self.lora_scale = scale
+        """A scalar: every sample of the next UNet calls runs at that slider value (the reference's behaviour).
+        A 1-D sequence or CPU tensor of n values: inside `with network:`, batch entry b of the next UNet calls runs at
+        scale[b % n], so with the CFG layout (negatives; positives) of N samples, n = N gives sample i the same value in
+        both halves.  The value multiplies each module's alpha / rank exactly as the scalar does; the batch size must
+        be a multiple of n (the UNet raises ValueError otherwise).  Inference only: a gradient through a forward run
+        with per-sample values raises NotImplementedError."""
+        values = _per_sample_values(scale)
+        self.lora_scale = scale if values is None else values
 
     def __enter__(self):
+        if isinstance(self.lora_scale, tuple):
+            # per-sample values: the modules run at multiplier 1 and the UNet multiplies in each sample's value; all
+            # zeros is the adaptors-off state of a scalar 0
+            on = any(v != 0.0 for v in self.lora_scale)
+            for lora in self.unet_loras:
+                lora.multiplier = 1.0 if on else 0.0
+                lora.sample_scales = self.lora_scale if on else None
+            if on:
+                PER_SAMPLE_NETWORKS.add(self)
+            else:
+                PER_SAMPLE_NETWORKS.discard(self)
+            return
+        PER_SAMPLE_NETWORKS.discard(self)
         for lora in self.unet_loras:
             lora.multiplier = 1.0 * self.lora_scale
+            lora.sample_scales = None
 
     def __exit__(self, exc_type, exc_value, tb):
+        PER_SAMPLE_NETWORKS.discard(self)
         for lora in self.unet_loras:
             lora.multiplier = 0
+            lora.sample_scales = None
+
+
+def _per_sample_values(scale) -> Optional[tuple]:
+    """The per-sample slider values of a 1-D sequence / tensor as a tuple of floats, or None for a scalar."""
+    if torch.is_tensor(scale):
+        if scale.dim() == 0:
+            return None
+        if scale.dim() != 1 or scale.is_cuda:
+            raise ValueError(f"set_lora_slider: per-sample scales must be a 1-D CPU tensor, got {tuple(scale.shape)} "
+                             f"on {scale.device}")
+        values = tuple(float(v) for v in scale.tolist())
+    elif isinstance(scale, (list, tuple)):
+        values = tuple(float(v) for v in scale)
+    else:
+        return None
+    if not values:
+        raise ValueError("set_lora_slider: an empty sequence of per-sample scales")
+    return values
 
 
 # --------------------------------------------------------------------------------------------------
@@ -203,6 +248,13 @@ class _StackedLoRANetwork(LoRANetwork):
         self.__dict__["_leaves"] = {}  # lora_name -> adapted leaf, filled before nn.Module registration matters
         super().__init__(unet, **kw)
         self.name = None
+
+    def set_lora_slider(self, scale):
+        if _per_sample_values(scale) is not None:
+            raise NotImplementedError("sliders_b200: per-sample slider scales are not implemented for a SliderStack "
+                                      "(its composite packs fold one multiplier per slider); sweep the stack's scales "
+                                      "one denoise at a time")
+        super().set_lora_slider(scale)
 
 
 class SliderHook:
@@ -315,6 +367,9 @@ class SliderStack(nn.Module):
         if isinstance(scale, (int, float)) or (torch.is_tensor(scale) and scale.dim() == 0):
             values = [float(scale)] * len(self.sliders)
         else:
+            if any(_per_sample_values(v) is not None for v in scale):
+                raise NotImplementedError("sliders_b200: per-sample slider scales are not implemented for a "
+                                          "SliderStack; pass one scalar per slider")
             values = [float(v) for v in scale]
             if len(values) != len(self.sliders):
                 raise ValueError(f"SliderStack.set_lora_slider: {len(values)} scales for {len(self.sliders)} sliders")

@@ -109,18 +109,31 @@ def lora_slots(r: int, groups: int = 1) -> Tuple[int, int]:
 
 
 class Lora:
-    """Packed LoRA side inputs of one fused GEMM/conv call (see struct sb200_lora)."""
+    """Packed LoRA side inputs of one fused GEMM/conv call (see struct sb200_lora).
 
-    __slots__ = ("down", "up", "r", "rt", "group_n", "scale", "scale_dev", "_c")
+    sample_scale: optional fp32 device vector of per-sample factors; output row m of the LoRA term is multiplied by
+    sample_scale[m // rows_per_sample].  rows_per_sample 0 lets `gemm` / `conv3x3` / `small_linear` derive it from the
+    call as M // sample_scale.numel() (the vector then has one entry per batch entry of that call)."""
+
+    __slots__ = ("down", "up", "r", "rt", "group_n", "scale", "scale_dev", "sample_scale", "rows_per_sample", "_c")
 
     def __init__(self, down: torch.Tensor, up: torch.Tensor, r: int, group_n: int, scale: float,
-                 scale_dev: Optional[torch.Tensor] = None):
+                 scale_dev: Optional[torch.Tensor] = None, sample_scale: Optional[torch.Tensor] = None,
+                 rows_per_sample: int = 0):
         self.down, self.up, self.r, self.rt, self.group_n = down, up, r, down.shape[0], group_n
         self.scale, self.scale_dev = float(scale), scale_dev
+        self.sample_scale, self.rows_per_sample = sample_scale, int(rows_per_sample)
         self._c = LoraArgs(down.data_ptr(), up.data_ptr(), r, self.rt, group_n, self.scale,
-                           scale_dev.data_ptr() if scale_dev is not None else None)
+                           scale_dev.data_ptr() if scale_dev is not None else None,
+                           sample_scale.data_ptr() if sample_scale is not None else None, self.rows_per_sample)
 
-    def ref(self):
+    def ref(self, M: int = 0):
+        """The struct for a launch with M output rows; fills a derived rows_per_sample (see the class docstring)."""
+        if self.sample_scale is not None and self.rows_per_sample == 0:
+            n = self.sample_scale.numel()
+            if M % n != 0:
+                raise ValueError(f"LoRA sample_scale: {n} per-sample factors do not divide the call's {M} rows")
+            self._c.rows_per_sample = M // n
         return C.byref(self._c)
 
 
@@ -148,7 +161,7 @@ def gemm(x: torch.Tensor, w: torch.Tensor, *, bias=None, rowbias=None, rows_per_
     _cabi.check(lib.sb200_gemm(
         _ctx(x), _stream(), _p(x), x.stride(0), _p(x1), x1.stride(0) if x1 is not None else 0, K0,
         _p(w), w.stride(0), _p(out), out.stride(0), M, N, K, flags, _p(bias), _p(rowbias), rows_per_batch,
-        _p(resid), resid.stride(0) if resid is not None else 0, lora.ref() if lora is not None else None, bn))
+        _p(resid), resid.stride(0) if resid is not None else 0, lora.ref(M) if lora is not None else None, bn))
     _count("gemm", 2.0 * M * N * K)
     return out
 
@@ -182,7 +195,7 @@ def conv3x3(x0: torch.Tensor, w_packed: torch.Tensor, *, x1: Optional[torch.Tens
     _cabi.check(lib.sb200_conv3x3(
         _ctx(x0), _stream(), _p(x0), x0.stride(2), _p(x1), x1.stride(2) if x1 is not None else 0, C0, C1,
         _p(w_packed), _p(out), out.stride(2), B, H, W, Cout, stride, flags, _p(bias), _p(rowbias), _p(resid),
-        resid.stride(2) if resid is not None else 0, lora.ref() if lora is not None else None, bn))
+        resid.stride(2) if resid is not None else 0, lora.ref(B * Ho * Wo) if lora is not None else None, bn))
     _count("conv3x3", 2.0 * B * (H // stride) * (W // stride) * Cout * 9 * (C0 + C1))
     return out
 
@@ -258,7 +271,7 @@ def small_linear(x: torch.Tensor, w: torch.Tensor, bias=None, *, act_in: bool = 
     lib = _begin()
     _cabi.check(lib.sb200_small_linear(_ctx(x), _stream(), _p(x), x.stride(0), _p(w), w.stride(0), _p(bias),
                                        _p(out), N, M, N, K, int(act_in), int(act_out),
-                                       lora.ref() if lora is not None else None, _p(resid)))
+                                       lora.ref(M) if lora is not None else None, _p(resid)))
     _count("small_linear")
     return out
 

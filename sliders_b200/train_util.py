@@ -147,11 +147,12 @@ def _denoise_loop(unet, scheduler, latents, text_embeddings, added, guidance_sca
 
 
 def guided_step(scheduler, noise_pred: torch.Tensor, timestep, latents: torch.Tensor, guidance_scale: float,
-                generator: Optional[torch.Generator] = None) -> torch.Tensor:
+                generator: Optional[torch.Generator] = None, noise_repeat: int = 1) -> torch.Tensor:
     """eps = u + g (c - u) followed by `scheduler.step(eps, t, x).prev_sample` (train_util.py:165-171 + :193 /
     generate_images_xl.py:349-358).  For the schedulers whose step is affine in (x, eps) with host-side coefficients the
     two are ONE `cfg_ddim_kernel` launch; the ancestral ones add their noise term on top; the rest (LMS) take the
-    guided eps through their own `step`."""
+    guided eps through their own `step`.  noise_repeat: the ancestral noise is drawn for 1 / noise_repeat of the samples
+    and repeated, so that latents tiled noise_repeat times (a batched scale sweep) see the noise of one untiled run."""
     kind = getattr(scheduler, "step_kind", "generic")
     noise_pred = noise_pred.contiguous()
     if kind == "ddim":
@@ -166,8 +167,10 @@ def guided_step(scheduler, noise_pred: torch.Tensor, timestep, latents: torch.Te
             if std > 0.0:
                 n = noise_pred.shape[0] // 2
                 dev = generator.device if generator is not None else out.device
-                z = torch.randn((n,) + tuple(noise_pred.shape[1:]), generator=generator, device=dev,
+                z = torch.randn((n // noise_repeat,) + tuple(noise_pred.shape[1:]), generator=generator, device=dev,
                                 dtype=noise_pred.dtype).to(out.device)
+                if noise_repeat > 1:
+                    z = z.repeat((noise_repeat,) + (1,) * (z.dim() - 1))
                 out = out + std * z.to(out.dtype)
         return out
     guided, _ = ops.cfg_ddim(noise_pred, guidance_scale, out_dtype=noise_pred.dtype)

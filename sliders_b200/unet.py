@@ -24,6 +24,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 import torch.nn as nn
 
+from . import lora as _lora_mod
 from . import ops
 from .ops import BF16, Lora
 
@@ -380,6 +381,11 @@ class UNet2DConditionModel(nn.Module):
         self._lora_packs: Dict[tuple, _LoraPack] = {}
         self._graphs: Dict[tuple, "_CapturedForward"] = {}
         self._slider_scale_dev: Optional[torch.Tensor] = None
+        # per-sample slider values (LoRANetwork.set_lora_slider with a sequence): one fp32 device vector per (batch
+        # size, adaptor factor), entry b = value[b % n] * factor; `_sample_values` holds the walk's values
+        self._sample_vecs: Dict[tuple, torch.Tensor] = {}
+        self._sample_values: Optional[tuple] = None
+        self._sample_filled: set = set()
         self._stack_arena: Optional[_StackArena] = None
         self._stack_mults: Optional[List[float]] = None  # per-slider multipliers of the current walk; None: stack off
         self.use_cuda_graph = False
@@ -405,6 +411,7 @@ class UNet2DConditionModel(nn.Module):
         self._graphs.clear()
         self.__dict__.pop("_train_graphs", None)
         self._slider_scale_dev = None
+        self._sample_vecs.clear()
         self._stack_arena = None
         return out
 
@@ -506,6 +513,11 @@ class UNet2DConditionModel(nn.Module):
                     pack.up[n0:n1, :rr].copy_(u)
                 n0 = n1
             pack.key = ver
+        if self._sample_values is not None:
+            # per-sample values: the factor common to the call site (1 when folded into `up`) goes into the vector, so
+            # a constant vector reproduces the scalar path's fp32 scale exactly
+            vec = self._sample_vec(common if common is not None else 1.0)
+            return Lora(pack.down, pack.up, r, group_n, 1.0, sample_scale=vec)
         if self._slider_scale_dev is None:
             self._slider_scale_dev = torch.ones(1, device=leaves[0].weight.device, dtype=torch.float32)
         if self._capturing and common is not None:
@@ -515,6 +527,54 @@ class UNet2DConditionModel(nn.Module):
 
     _capturing = False
     _bake_scales = False
+
+    # ---- per-sample slider values ------------------------------------------------------------------------------------
+    def _sample_scan(self, B: int) -> Optional[tuple]:
+        """The per-sample slider values the active adaptors carry (`LoRANetwork.set_lora_slider` with a sequence), or
+        None.  B, the batch of the call, must be a multiple of their count."""
+        values = None
+        if not _lora_mod.PER_SAMPLE_NETWORKS:
+            return None
+        for _, a in self._adapted_leaves():
+            v = getattr(a, "sample_scales", None)
+            if v is None or float(a.multiplier) * float(a.scale) == 0.0:
+                continue
+            if values is not None and v != values:
+                raise ValueError("sliders_b200: active adaptors carry different per-sample slider values")
+            values = v
+        if values is not None and B % len(values) != 0:
+            raise ValueError(f"sliders_b200: a batch of {B} is not a multiple of the {len(values)} per-sample slider "
+                             "values")
+        return values
+
+    def _sample_vec(self, factor: float) -> torch.Tensor:
+        """The device vector of the current walk's batch for adaptor factor `factor`, filled once per walk (a captured
+        graph gets its values from _GraphInputs.load instead)."""
+        B = self.__dict__["_sample_batch"]
+        key = (B, factor)
+        vec = self._sample_vecs.get(key)
+        if vec is None:
+            if self._capturing:
+                raise RuntimeError("sliders_b200: a per-sample scale vector was first needed while a CUDA graph was "
+                                   "captured")
+            vec = torch.empty(B, device=self.conv_in.weight.device, dtype=torch.float32)
+            self._sample_vecs[key] = vec
+        if not self._capturing and key not in self._sample_filled:
+            self._fill_sample_vec(vec, factor, self._sample_values)
+            self._sample_filled.add(key)
+        return vec
+
+    @staticmethod
+    def _fill_sample_vec(vec: torch.Tensor, factor: float, values: tuple) -> None:
+        """vec[b] = fp32(values[b % n] * factor), with one fill per run of equal entries: kernel launches with the value
+        as an argument, so the host never waits for the stream (a copy from pageable host memory would)."""
+        n = len(values)
+        entries = [values[b % n] * factor for b in range(vec.numel())]
+        b0 = 0
+        for b in range(1, len(entries) + 1):
+            if b == len(entries) or entries[b] != entries[b0]:
+                vec[b0:b].fill_(entries[b0])
+                b0 = b
 
     # ---- SliderStack: composite LoRA packs -------------------------------------------------------------------------
     def _stack_status(self) -> Optional[List[float]]:
@@ -763,6 +823,15 @@ class UNet2DConditionModel(nn.Module):
                 tape.append((kind, rec))
 
         B = sample.shape[0]
+        self._sample_values = self._sample_scan(B)
+        self.__dict__["_sample_batch"] = B
+        self._sample_filled = set()
+        try:
+            return self._walk_body(sample, timesteps_f32, ehs, added_cond_kwargs, out_dtype, tape, record, B)
+        finally:
+            self._sample_values = None
+
+    def _walk_body(self, sample, timesteps_f32, ehs, added_cond_kwargs, out_dtype, tape, record, B):
         if "_slider_stack" in self.__dict__:
             if tape is not None and self._stack_status() is not None:
                 raise NotImplementedError("sliders_b200: a gradient through an active SliderStack is not implemented "
@@ -904,7 +973,10 @@ class UNet2DConditionModel(nn.Module):
         ranks are part of it too: they set the sizes of the packed buffers a graph reads."""
         adapted = self._adapted_leaves()
         scales = [float(a.multiplier) * float(a.scale) for _, a in adapted]
-        ranks = tuple(int(a.lora_dim) for _, a in adapted)
+        # per-sample values are device-side too, but a graph captured with them reads a vector the scalar graph does not
+        ranks = (tuple(int(a.lora_dim) for _, a in adapted),
+                 bool(_lora_mod.PER_SAMPLE_NETWORKS) and
+                 any(getattr(a, "sample_scales", None) is not None for _, a in adapted))
         nz = [s for s in scales if s != 0.0]
         if "_slider_stack" in self.__dict__ and self._stack_status() is not None:
             # the stack's layout, not its multipliers (device-side): one graph serves every combination of scales
@@ -971,6 +1043,11 @@ class _GraphInputs:
             unet._slider_scale_dev.fill_(1.0 if common is None else common)
         if "_slider_stack" in unet.__dict__:
             unet._stack_begin(compose=False)  # per-slider multipliers; the graph's own compose applies them
+        values = unet._sample_scan(x.shape[0])
+        if values is not None:
+            for (B, factor), vec in unet._sample_vecs.items():
+                if B == x.shape[0]:
+                    unet._fill_sample_vec(vec, factor, values)
         unet._bake_scales = bake
         try:
             unet._refresh_lora_packs()
