@@ -1,12 +1,14 @@
 """Edit a real image with a slider on sliders_b200 — demo_image_editing.ipynb end to end: null-text inversion of the
 image latent (cells 6-7), then the slider sweep from x_T with the per-step optimised unconditional embeddings and
-start_noise = 500 (cell 13).  The VAE and the text encoder are off the denoise path: the image latent and the two
-[1, 77, 768] embeddings come from a file (`torch.save({"latent": vae_latent * 0.18215, "uncond": ..., "cond": ...})`)
-or, with --synthetic, from a seed with synthetic UNet weights (shape check / throughput only).  Writes the edited
-latents as .pt files; decode them with the VAE.
+start_noise = 500 (cell 13).  With a VAE (`--vae`, `auto` = the `vae/` of a `--unet` diffusers directory) the photo
+given by --image is resized to 512 px and encoded to its latent mean (`vae.encode(x).latent_dist.mean * 0.18215`, as the
+notebook does), and every edit is decoded to `edit_scale<s>.png` beside its latent.  Without one the image latent comes
+from --inputs.  The two [1, 77, 768] embeddings come from a file (`torch.save({"latent": vae_latent * 0.18215,
+"uncond": ..., "cond": ...})`; "latent" is not needed with --image) or, with --synthetic, from a seed with synthetic
+UNet weights (shape check / throughput only).  The edited latents are always written as .pt files.
 
     python examples/edit_real_image_sd1.py --synthetic --steps 10 --inner 3 --out edited/
-    python examples/edit_real_image_sd1.py --unet /path/unet/diffusion_pytorch_model.safetensors --inputs img.pt \
+    python examples/edit_real_image_sd1.py --unet /path/to/sd-1.5 --image photo.jpg --inputs embeds.pt \
         --slider models/ageslider/slider_last.pt --scales 0 2 4 --out edited/
 
 Needs an H100 (there is no CPU path).
@@ -18,7 +20,8 @@ import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from sliders_b200 import generate, io as sio, lora, synthetic  # noqa: E402
+from sliders_b200 import cli, generate, lora, model_util, synthetic  # noqa: E402
+from sliders_b200 import vae as svae  # noqa: E402
 from sliders_b200.inversion import NullInversion  # noqa: E402
 from sliders_b200.scheduler import DDIMScheduler  # noqa: E402
 from sliders_b200.unet import UNet2DConditionModel, UNetConfig  # noqa: E402
@@ -26,8 +29,10 @@ from sliders_b200.unet import UNet2DConditionModel, UNetConfig  # noqa: E402
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--unet", default=None, help="HF unet/diffusion_pytorch_model.safetensors (SD1.x)")
+    ap.add_argument("--unet", default=None, help="SD1.x diffusers directory or unet/diffusion_pytorch_model.safetensors")
     ap.add_argument("--inputs", default=None, help="torch file with latent [1,4,64,64], uncond / cond [1,77,768]")
+    ap.add_argument("--image", default=None, help="photo to edit (needs a VAE); replaces the file's latent")
+    ap.add_argument("--vae", default="auto", help="auto | none | VAE path | synthetic[:seed]")
     ap.add_argument("--slider", default=None, help="slider weights saved by the trainers (LoRANetwork.save_weights)")
     ap.add_argument("--synthetic", action="store_true")
     ap.add_argument("--rank", type=int, default=4)
@@ -43,7 +48,7 @@ def main():
     dt = torch.bfloat16
 
     if args.unet:
-        unet = sio.load_unet(UNetConfig.sd15(), args.unet, device=dev, dtype=dt)
+        unet = model_util.load_unet(args.unet, UNetConfig.sd15(), dt, dev)
     else:
         with torch.device(dev):
             unet = UNet2DConditionModel(UNetConfig.sd15()).to(dt)
@@ -57,7 +62,16 @@ def main():
         uncond, cond = (torch.randn(1, 77, 768, generator=g).to(dev) for _ in range(2))
     else:
         raw = torch.load(args.inputs, map_location=dev)
-        latent, uncond, cond = raw["latent"].float(), raw["uncond"].float(), raw["cond"].float()
+        latent, uncond, cond = raw.get("latent"), raw["uncond"].float(), raw["cond"].float()
+    vae_source = svae.resolve_vae_source(args.vae, args.unet)
+    vae = svae.load_vae(vae_source, svae.VAEConfig.sd15(), device=dev) if vae_source is not None else None
+    if args.image:
+        if vae is None:
+            raise SystemExit("--image needs a VAE: --vae PATH, or a --unet diffusers directory with vae/")
+        latent = cli.encode_image(vae, args.image, 512, sample=False)
+    if latent is None:
+        raise SystemExit(f"{args.inputs}: no 'latent'; pass --image with a VAE")
+    latent = latent.float()
 
     # cell 4: DDIMScheduler(..., clip_sample=False, set_alpha_to_one=False); cells 6-7: invert
     scheduler = DDIMScheduler(beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear", clip_sample=False,
@@ -86,6 +100,10 @@ def main():
                                     negative_embeds_per_step=uncond_list)
         path = os.path.join(args.out, f"latent_scale{s:g}.pt")
         torch.save(out.cpu(), path)
+        if vae is not None:                                                    # cell 13: vae.decode + numpy_to_pil
+            png = os.path.join(args.out, f"edit_scale{s:g}.png")
+            svae.to_pil(vae.decode(out.float()))[0].save(png)
+            path += f", {png}"
         print(f"scale {s:g}: {path}", flush=True)
 
 

@@ -38,8 +38,11 @@ enum {
   SB200_EPI_ROWBIAS = 2,  /* + rowbias[(m / rows_per_batch) * N + n]   (ResnetBlock2D time-embedding add) */
   SB200_EPI_RESID = 4,    /* + resid[m * ldr + n] */
   SB200_EPI_GEGLU = 8,    /* out[m, j] = acc[m, j] * gelu_erf(acc[m, N/2 + j]),  j < N/2 */
-  SB200_EPI_LORA = 16     /* + scale [* sample_scale[m / rows_per_sample]] * (X . down^T) . up^T, rank r, computed in
+  SB200_EPI_LORA = 16,    /* + scale [* sample_scale[m / rows_per_sample]] * (X . down^T) . up^T, rank r, computed in
                              the same tile loop */
+  SB200_CONV_PAD_BR = 32  /* sb200_conv3x3 with stride 2 only: pad 1 at the bottom and right and none at the top and left,
+                             so tap (kh, kw) reads input pixel (2 ho + kh, 2 wo + kw) — diffusers Downsample2D with
+                             padding=0, F.pad(x, (0, 1, 0, 1)) then a stride-2 conv (the VAE encoder) */
 };
 
 /* ABI / build identification: "sb200 <version> sm_90a". */
@@ -92,7 +95,8 @@ int sb200_gemm(void* handle, void* stream, const void* x0, int ldx0, const void*
                const void* bias, const void* rowbias, int rows_per_batch, const void* resid, int ldr,
                const sb200_lora* lora, int bn);
 
-/* 3x3 convolution, padding 1, stride 1 or 2, as an implicit GEMM over NHWC activations.
+/* 3x3 convolution, padding 1 (or, with SB200_CONV_PAD_BR, 0 top-left and 1 bottom-right), stride 1 or 2, as an
+ * implicit GEMM over NHWC activations.
  * Replaces: torch Conv2d inside diffusers ResnetBlock2D / Downsample2D / Upsample2D (same call site).
  *   x0/x1: [B, Hin, Win, C0] / [B, Hin, Win, C1] (x1 may be NULL), pixel strides ldx0 / ldx1 elements;
  *   w    : [Cout, 3, 3, C0 + C1] bf16 (tap-major repack of the HF [Cout, Cin, 3, 3] weight);
@@ -102,6 +106,9 @@ int sb200_conv3x3(void* handle, void* stream, const void* x0, int ldx0, const vo
                   int C1, const void* w, void* out, int ldo, int B, int Hin, int Win, int Cout,
                   int stride, int flags, const void* bias, const void* rowbias, const void* resid,
                   int ldr, const sb200_lora* lora, int bn);
+
+/* The SD / SDXL VAE's own entry points (image and latent ends, mid-block attention softmax) are declared in
+ * sb200_vae.h, with the same conventions; its downsamplers use sb200_conv3x3 with SB200_CONV_PAD_BR. */
 
 /* softmax(Q K^T * scale) V per (batch, head); head_dim a multiple of 8 up to 192 (SDXL 64; SD1.x 40 / 80 / 160).
  * Q/K/V/O are token matrices with row strides in elements; head h occupies columns [h*head_dim, (h+1)*head_dim).

@@ -12,6 +12,7 @@ from typing import Optional
 _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libsb200.so")
 
 EPI_BIAS, EPI_ROWBIAS, EPI_RESID, EPI_GEGLU, EPI_LORA = 1, 2, 4, 8, 16
+CONV_PAD_BR = 32
 
 
 class Sb200Error(RuntimeError):
@@ -80,6 +81,11 @@ SIGNATURES = {
     "sb200_cfg_ddim": [_p, _p, _p, _i, _f, _p, _f, _f, _p, _p, _i, _i64],
     "sb200_cfg_step": [_p, _p, _p, _i, _f, _p, _f, _f, _p, _p, _i, _i64],
     "sb200_lora_compose": [_p, _p, _p, _p, _p, _i64, _i],
+    "sb200_vae_conv_in_u8": [_p, _p, _p, _p, _p, _p, _i, _i, _i, _i],
+    "sb200_vae_conv_out_u8": [_p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i],
+    "sb200_vae_moments": [_p, _p, _p, _p, _p, _p, _p, _p, _f, _p, _i, _i, _i, _i],
+    "sb200_vae_post_quant": [_p, _p, _p, _p, _p, _f, _p, _i, _i],
+    "sb200_softmax_rows": [_p, _p, _p, _i, _p, _i, _i, _i, _f],
 }
 _RESTYPE = {"sb200_version": C.c_char_p, "sb200_last_error": C.c_char_p}
 

@@ -12,9 +12,14 @@ Added, because this container has neither the hub nor the text encoders' / VAE's
                   `torch.save({prompt: (text_embeds, pooled_embeds)})` for SDXL, `{prompt: text_embeds}` for SD1.x
   (no flag)       `pretrained_model.name_or_path: synthetic[:seed]` draws seeded embeddings per prompt string
   --iterations N  overrides `train.iterations` (smoke runs)
+  --vae SOURCE    image sliders: `auto` (default: the `vae/` of a diffusers model directory), `none`, a VAE path or
+                  `synthetic[:seed]`
 Image sliders read `<folder_main>/<folder>/<name>.pt` latent files ([4,h,w], already VAE-encoded and scaled, what
-`get_noisy_image` computes before `add_noise`, imagesliders/train_util.py:201-235): the VAE is diffusers code off the
-denoise path.  One process per GPU under torchrun shards the step (sliders_b200.trainer); single process otherwise.
+`get_noisy_image` computes before `add_noise`, imagesliders/train_util.py:201-235) when the folder has them.  With a VAE
+(`sliders_b200.vae`) they read image folders as the reference does (train_lora-scale-xl.py:215-246): the files of the
+low folder, the same file name from the high folder, both resized to 512 px (SDXL) or 256 px (SD1.x) and encoded to a
+fresh latent sample on every iteration.  One process per GPU under torchrun shards the step (sliders_b200.trainer);
+single process otherwise.
 """
 from __future__ import annotations
 
@@ -30,6 +35,7 @@ import torch
 import torch.distributed as dist
 
 from . import config_util, lora, model_util, parallel, prompt_util, train_util, trainer
+from . import vae as svae
 from .config_util import RootConfig
 from .prompt_util import PromptEmbedsCache, PromptEmbedsPair, PromptEmbedsXL, PromptSettings
 
@@ -58,6 +64,9 @@ def build_parser(kind: str) -> argparse.ArgumentParser:
                        help="folders with different attribute-scaled images")
         p.add_argument("--scales", type=str, required=False, default="-2, -1, 1, 2",
                        help="scales for different attribute-scaled images")
+        p.add_argument("--vae", type=str, required=False, default="auto", metavar="auto|none|PATH|synthetic[:seed]",
+                       help="VAE that encodes image folders (.png/.jpg/.jpeg/.webp): auto = the vae/ of the model "
+                            "directory; folders of .pt latents need none")
     # not in the reference: offline substitutes for the hub
     p.add_argument("--embeds", type=str, default=None, help="torch file {prompt: embedding(s)} (see module docstring)")
     p.add_argument("--iterations", type=int, default=None, help="override train.iterations")
@@ -252,16 +261,53 @@ def list_pairs(folder_main: str, folder_low: str, folder_high: str) -> List[str]
     return names
 
 
+def list_image_pairs(folder_main: str, folder_low: str, folder_high: str) -> List[str]:
+    """The image files of the low folder (sorted) whose name the high folder also has; the reference takes the same
+    file name from both folders (train_lora-scale-xl.py:215-221).  A name missing from the high folder raises."""
+    low = os.path.join(folder_main, folder_low)
+    names = sorted(f for f in os.listdir(low) if f.lower().endswith(_IMAGE_EXT))
+    if not names:
+        raise FileNotFoundError(f"{low}: no .pt latent files and no {'/'.join(_IMAGE_EXT)} images")
+    high = set(os.listdir(os.path.join(folder_main, folder_high)))
+    missing = [n for n in names if n not in high]
+    if missing:
+        raise FileNotFoundError(f"{folder_main}/{folder_high}: no {missing[0]} to pair with {low}/{missing[0]} "
+                                f"({len(missing)} of {len(names)} names missing)")
+    return names
+
+
+def encode_image(vae: svae.AutoencoderKL, path: str, size: int, generator=None, sample: bool = True) -> torch.Tensor:
+    """`Image.open(path).resize((size, size))` + `vae.encode(...).latent_dist.sample() * scaling_factor`
+    (get_noisy_image, imagesliders/train_util.py:216-217; `.mean` with sample=False) -> fp32 [1, 4, size/8, size/8] on
+    the VAE's device."""
+    import numpy as np
+    from PIL import Image
+
+    img = Image.open(path).convert("RGB").resize((size, size))
+    x = torch.from_numpy(np.asarray(img, dtype=np.uint8).copy()).unsqueeze(0).to(vae.device)
+    return vae.encode(x, sample=sample, generator=generator)
+
+
+def _has_latents(folder: str) -> bool:
+    return any(f.endswith(_LATENT_EXT) for f in os.listdir(folder))
+
+
 def load_latent(path: str) -> torch.Tensor:
     t = torch.load(path, map_location="cpu")
     return t.reshape(1, 4, *t.shape[-2:])
 
 
 def train_image(config: RootConfig, prompts: Sequence[PromptSettings], device, xl: bool, folder_main: str,
-                folders: Sequence[str], scales: Sequence[int], embeds_file: Optional[str] = None):
-    """`train()` of train_lora-scale-xl.py:41-414 / train_lora-scale.py:41-370."""
+                folders: Sequence[str], scales: Sequence[int], embeds_file: Optional[str] = None,
+                vae_source: Optional[str] = None):
+    """`train()` of train_lora-scale-xl.py:41-414 / train_lora-scale.py:41-370.  vae_source: the VAE that encodes
+    image folders (`sliders_b200.vae.load_vae`); folders of .pt latents are read as they are."""
     (weight_dtype, tokenizers, text_encoders, unet, noise_scheduler, network, optimizer,
      lr_scheduler) = _setup(config, xl, True, device)
+    vae = None
+    if vae_source is not None:
+        vae = svae.load_vae(vae_source, svae.VAEConfig.sdxl() if xl else svae.VAEConfig.sd15(), device=device)
+    size = 512 if xl else 256                              # train_lora-scale-xl.py:220 / train_lora-scale.py:220
     synthetic = config.pretrained_model.name_or_path.startswith("synthetic")
     pairs = build_prompt_pairs(prompts, xl, device, weight_dtype, tokenizers=tokenizers, text_encoders=text_encoders,
                                embeds_file=embeds_file, synthetic=synthetic)
@@ -272,10 +318,22 @@ def train_image(config: RootConfig, prompts: Sequence[PromptSettings], device, x
         pair = pairs[_pick(len(pairs), device)]
         scale_to_look = abs(int(parallel.sync_draws([random.choice(list(scales))], device)[0]))   # :209
         low, high = folder_of[-scale_to_look], folder_of[scale_to_look]
-        names = list_pairs(folder_main, low, high)
-        name = names[int(parallel.sync_draws([random.randint(0, len(names) - 1)], device)[0])]
-        lat_low = load_latent(os.path.join(folder_main, low, name))
-        lat_high = load_latent(os.path.join(folder_main, high, name))
+        if vae is None or _has_latents(os.path.join(folder_main, low)):
+            names = list_pairs(folder_main, low, high)
+            name = names[int(parallel.sync_draws([random.randint(0, len(names) - 1)], device)[0])]
+            lat_low = load_latent(os.path.join(folder_main, low, name))
+            lat_high = load_latent(os.path.join(folder_main, high, name))
+        else:
+            names = list_image_pairs(folder_main, low, high)
+            name = names[int(parallel.sync_draws([random.randint(0, len(names) - 1)], device)[0])]
+            # latent_dist.sample(None) draws from the device's global generator; replicas of a sharded step must
+            # encode the same sample, so they share a seed drawn once
+            gen = None
+            if _dist_env()[0] > 1:
+                gen = torch.Generator(device=device).manual_seed(
+                    int(parallel.sync_draws([torch.randint(0, 2 ** 31 - 1, (1,)).item()], device)[0]))
+            lat_low = encode_image(vae, os.path.join(folder_main, low, name), size, gen)
+            lat_high = encode_image(vae, os.path.join(folder_main, high, name), size, gen)
         losses = step(unet, network, noise_scheduler, optimizer, lr_scheduler, pair, lat_low, lat_high,
                       float(scale_to_look), max_denoising_steps=config.train.max_denoising_steps, device=device,
                       weight_dtype=weight_dtype, seed=random.randint(0, 2 * 15))                   # :223 (SURVEY C.10)
@@ -305,6 +363,7 @@ def main(kind: str, argv: Optional[Sequence[str]] = None):
         if not image:
             return train_text(config, prompts, device, xl, args.embeds)
         folders, scales = split_csv(args.folders), [int(s) for s in split_csv(args.scales)]
+        vae_source = svae.resolve_vae_source(args.vae, config.pretrained_model.name_or_path)
         if len(scales) != len(folders):
             raise Exception("the number of folders need to match the number of scales")
         if args.stylecheck is not None:               # train_lora-scale-xl.py:452-463
@@ -315,9 +374,9 @@ def main(kind: str, argv: Optional[Sequence[str]] = None):
                 cfg = config.model_copy(deep=True)
                 cfg.save.name = f"{os.path.basename(folder_main)}_alpha{args.alpha}_rank{cfg.network.rank}"
                 cfg.save.path = f"models/{cfg.save.name}"
-                out = train_image(cfg, prompts, device, xl, folder_main, folders, scales, args.embeds)
+                out = train_image(cfg, prompts, device, xl, folder_main, folders, scales, args.embeds, vae_source)
             return out
-        return train_image(config, prompts, device, xl, args.folder_main, folders, scales, args.embeds)
+        return train_image(config, prompts, device, xl, args.folder_main, folders, scales, args.embeds, vae_source)
     finally:
         if world > 1 and dist.is_initialized():
             dist.destroy_process_group()

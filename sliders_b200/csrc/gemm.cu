@@ -82,7 +82,7 @@ struct GemmParams {
   int up_buf_bytes; // per-warp staging of one slab's lora_up rows: 32 * r * 4 (0 without LoRA)
   int n_fast;       // tile order: 1 = consecutive CTAs share the A row-tile and walk the N tiles (A is read from
                     // DRAM once, W stays L2-resident); 0 = M fastest (A re-streamed once per N tile when it exceeds L2)
-  int a_mode;       // 0 plain, 1 conv3x3 stride 1, 2 conv3x3 stride 2
+  int a_mode;       // 0 plain, 1 conv3x3 stride 1, 2 conv3x3 stride 2, 3 stride 2 padded at the bottom / right
   int kb_split;     // k-blocks (per tap) that come from source 0
   int cb_total;     // k-blocks per tap
   int B, H, W;      // conv OUTPUT dims
@@ -209,12 +209,16 @@ __device__ __forceinline__ void load_a(const GemmParams& p, const AOrigin& o, in
     if (a_mode == 1) {
       const int src = cb < kb_split ? 0 : 1;
       tma_load_4d(sA, &p.tmA[src], bar, (src ? cb - kb_split : cb) * kBK, o.w0 + kw - 1, o.h0 + kh - 1, o.b0);
-    } else {
+    } else if (a_mode == 2) {
       // input row 2*ho + kh - 1: kh=0 -> odd plane, row ho-1; kh=1 -> even plane, row ho; kh=2 -> odd plane, row ho
       const int ph = (kh == 1) ? 0 : 1;
       const int pwl = (kw == 1) ? 0 : 1;
       tma_load_4d(sA, &p.tmA[ph * 2 + pwl], bar, cb * kBK, o.w0 + ((kw == 0) ? -1 : 0), o.h0 + ((kh == 0) ? -1 : 0),
                   o.b0);
+    } else {
+      // SB200_CONV_PAD_BR: input row 2*ho + kh: kh=0 -> even plane, row ho; kh=1 -> odd plane, row ho; kh=2 -> even
+      // plane, row ho+1 (past the last row for ho = Ho-1: the TMA zero fill is the bottom / right pad)
+      tma_load_4d(sA, &p.tmA[(kh & 1) * 2 + (kw & 1)], bar, cb * kBK, o.w0 + (kw >> 1), o.h0 + (kh >> 1), o.b0);
     }
   }
 }
@@ -1380,6 +1384,9 @@ extern "C" int sb200_conv3x3(void* handle, void* stream, const void* x0, int ldx
   SB200_REQUIRE(Cout % 16 == 0, "conv3x3: Cout=%d must be a multiple of 16", Cout);
   SB200_REQUIRE(!(flags & SB200_EPI_GEGLU), "conv3x3: GEGLU unsupported");
   SB200_REQUIRE(stride == 1 || C1 == 0, "conv3x3: stride 2 takes a single source");
+  const bool pad_br = flags & SB200_CONV_PAD_BR;
+  SB200_REQUIRE(!pad_br || stride == 2, "conv3x3: CONV_PAD_BR needs stride 2");
+  flags &= ~SB200_CONV_PAD_BR;
   SB200_REQUIRE(ldx0 % 8 == 0 && ldo % 8 == 0 && (C1 == 0 || ldx1 % 8 == 0), "conv3x3: leading dims");
   const bool has_lora = flags & SB200_EPI_LORA;
   SB200_REQUIRE(!has_lora || lora, "conv3x3: LORA without sb200_lora");
@@ -1401,7 +1408,7 @@ extern "C" int sb200_conv3x3(void* handle, void* stream, const void* x0, int ldx
   p.Nout = Cout;
   p.cb_total = Cin / kBK;
   p.kblocks = 9 * p.cb_total;
-  p.a_mode = stride == 1 ? 1 : 2;
+  p.a_mode = stride == 1 ? 1 : (pad_br ? 3 : 2);
   p.kb_split = C0 / kBK;
   p.B = B;
   p.H = H;

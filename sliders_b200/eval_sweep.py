@@ -9,8 +9,10 @@ case starts from the same noise (:501), the scale list [-2, -1, 0, 1, 2] (:445) 
 `<save_path>/<slider file name>/<scale>/<case_number>_<sample>.*`.
 
 Outside the denoise path (SURVEY.md §2) and therefore pluggable: prompt encoding (`--embeds FILE` =
-`torch.save({prompt: (text_embeds, pooled_embeds)})`; synthetic models draw seeded embeddings) and VAE decoding (final
-latents are written as `<case>_<sample>.pt`; pass `decode=` to `sweep()` for PNGs when an AutoencoderKL is around).
+`torch.save({prompt: (text_embeds, pooled_embeds)})`; prompts it lacks are encoded by the model directory's text
+encoders when it has them; synthetic models draw seeded embeddings) and VAE decoding (final latents are written as
+`<case>_<sample>.pt`; with `--vae` (sliders_b200.vae) the decoded image is written beside each as `<case>_<sample>.png`,
+as the reference's `pipe(...).images` are at :508).
 The SDXL pipeline's scheduler is EulerDiscrete (our "euler"); `--scheduler ddim` selects BASELINE config 5's.
 """
 from __future__ import annotations
@@ -22,7 +24,8 @@ from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
-from . import generate, io as sio, lora, model_util
+from . import generate, io as sio, lora, model_util, train_util
+from . import vae as svae
 from .scheduler import create_noise_scheduler
 
 SCALES = (-2, -1, 0, 1, 2)
@@ -158,6 +161,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--unet", type=str, default="stabilityai/stable-diffusion-xl-base-1.0",
                    help="diffusers directory, UNet state-dict file, hub id in the local cache, or 'synthetic'")
     p.add_argument("--embeds", type=str, default=None, help="torch file {prompt: (text_embeds, pooled_embeds)}")
+    p.add_argument("--vae", type=str, default="auto", metavar="auto|none|PATH|synthetic[:seed]",
+                   help="VAE that decodes each result to <case>_<sample>.png: auto = the vae/ of a --unet diffusers "
+                        "directory or hub-cache entry (none otherwise), none = latents only, or a diffusers directory, "
+                        "VAE state-dict file, hub id or synthetic weights")
     p.add_argument("--scheduler", type=str, default="euler", help="euler (the SDXL pipeline's), ddim, lms, ddpm, euler_a")
     p.add_argument("--device", type=int, default=0)
     p.add_argument("--compose", type=parse_compose, action="append", default=[], metavar="PATH:SCALE",
@@ -202,6 +209,11 @@ def main(argv: Optional[Sequence[str]] = None, xl: bool = True) -> int:
         def one(p):
             if p in table:
                 return table[p]
+            if encs is not None:
+                with torch.no_grad():
+                    if xl:
+                        return train_util.encode_prompts_xl(toks, encs, [p])
+                    return train_util.encode_prompts(toks, encs, [p])
             if args.unet.startswith("synthetic"):
                 e = synthetic_embedding(p, xl, "cpu", torch.float32)
                 return (e.text_embeds, e.pooled_embeds) if xl else e
@@ -212,6 +224,14 @@ def main(argv: Optional[Sequence[str]] = None, xl: bool = True) -> int:
             return torch.cat([n[0], c[0]]), torch.cat([n[1], c[1]])
         return torch.cat([n, c]), None
 
+    decode = None
+    vae_source = svae.resolve_vae_source(args.vae, args.unet)
+    if vae_source is not None:
+        vae = svae.load_vae(vae_source, svae.VAEConfig.sdxl() if xl else svae.VAEConfig.sd15(), device=dev)
+
+        def decode(latents):
+            return svae.to_pil(vae.decode(latents))
+
     rows = read_prompts_csv(args.prompts_path, args.from_case, args.till_case)
     save_dir = os.path.join(args.save_path, os.path.basename(args.model_name))
     # the reference ignores --guidance_scale / --image_size / --ddim_steps in the XL script (pipeline defaults: 5.0, 1024, 50)
@@ -219,6 +239,6 @@ def main(argv: Optional[Sequence[str]] = None, xl: bool = True) -> int:
               num_samples=args.num_samples, num_inference_steps=50 if xl else args.ddim_steps,
               guidance_scale=5.0 if xl else args.guidance_scale, start_noise=args.start_noise,
               image_size=1024 if xl else args.image_size, xl=xl, dtype=dtype, fixed_scales=fixed,
-              scales_per_batch=args.scales_per_batch)
-    print(f"wrote {n} latents under {save_dir}")
+              scales_per_batch=args.scales_per_batch, decode=decode)
+    print(f"wrote {n} latents{' and images' if decode is not None else ''} under {save_dir}")
     return n

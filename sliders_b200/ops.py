@@ -11,7 +11,7 @@ from typing import Optional, Tuple
 import torch
 
 from . import _cabi
-from ._cabi import EPI_BIAS, EPI_GEGLU, EPI_LORA, EPI_RESID, EPI_ROWBIAS, LoraArgs
+from ._cabi import CONV_PAD_BR, EPI_BIAS, EPI_GEGLU, EPI_LORA, EPI_RESID, EPI_ROWBIAS, LoraArgs
 
 BF16 = torch.bfloat16
 
@@ -168,10 +168,11 @@ def gemm(x: torch.Tensor, w: torch.Tensor, *, bias=None, rowbias=None, rows_per_
 
 def conv3x3(x0: torch.Tensor, w_packed: torch.Tensor, *, x1: Optional[torch.Tensor] = None, stride: int = 1,
             bias=None, rowbias=None, resid=None, lora: Optional[Lora] = None, out: Optional[torch.Tensor] = None,
-            bn: int = 0) -> torch.Tensor:
+            bn: int = 0, pad_bottom_right: bool = False) -> torch.Tensor:
     """3x3 / pad 1 conv on NHWC bf16 ([B,H,W,C] tensors); w_packed is [Cout,3,3,Cin].  One `gemm_kernel`.
     `out`: [B, Ho, Wo, Cout] whose pixels are rows of one 2-D matrix with row stride out.stride(2) (e.g. a column
-    slice of a wider NHWC buffer)."""
+    slice of a wider NHWC buffer).  pad_bottom_right (stride 2 only): the conv of F.pad(x, (0, 1, 0, 1)) with
+    padding 0, as diffusers' Downsample2D in the VAE encoder (SB200_CONV_PAD_BR)."""
     B, H, W, C0 = x0.shape
     C1 = x1.shape[-1] if x1 is not None else 0
     Cout = w_packed.shape[0]
@@ -184,6 +185,8 @@ def conv3x3(x0: torch.Tensor, w_packed: torch.Tensor, *, x1: Optional[torch.Tens
         flags |= EPI_RESID
     if lora is not None:
         flags |= EPI_LORA
+    if pad_bottom_right:
+        flags |= CONV_PAD_BR
     Ho, Wo = H // stride, W // stride
     if out is None:
         out = torch.empty((B, Ho, Wo, Cout), device=x0.device, dtype=BF16)
@@ -322,6 +325,87 @@ def upsample2x(x: torch.Tensor) -> torch.Tensor:
     _cabi.check(lib.sb200_upsample2x(_ctx(x), _stream(), _p(x), _p(out), B, H, W, Cc))
     _count("upsample2x")
     return out
+
+
+def _image_shape(t: torch.Tensor, what: str, name: str, dtype, C: Optional[int] = None):
+    if t.dim() != 4 or t.dtype != dtype or not t.is_contiguous() or (C is not None and t.shape[-1] != C):
+        raise ValueError(f"{what}: {name} {tuple(t.shape)} {t.dtype} / strides {t.stride()} is not a contiguous "
+                         f"[B, H, W, {C if C is not None else 'C'}] {dtype} tensor")
+    return t.shape
+
+
+def vae_conv_in_u8(img: torch.Tensor, w_packed: torch.Tensor, bias) -> torch.Tensor:
+    """uint8 [B, H, W, 3] pixels -> NHWC bf16 [B, H, W, Cout]: preprocess (v / 255 * 2 - 1) + the VAE encoder's
+    conv_in.  One `vae_conv_in_u8_kernel`."""
+    B, H, W, _ = _image_shape(img, "vae_conv_in_u8", "img", torch.uint8, 3)
+    Cout = w_packed.shape[0]
+    out = torch.empty((B, H, W, Cout), device=img.device, dtype=BF16)
+    lib = _begin()
+    _cabi.check(lib.sb200_vae_conv_in_u8(_ctx(img), _stream(), _p(img), _p(w_packed), _p(bias), _p(out), B, H, W,
+                                         Cout))
+    _count("vae_conv_in_u8", 2.0 * B * H * W * Cout * 27)
+    return out
+
+
+def vae_conv_out_u8(x: torch.Tensor, w_packed: torch.Tensor, bias, return_float: bool = False):
+    """NHWC bf16 [B, H, W, Cin] (normalised + SiLU) -> uint8 [B, H, W, 3]: the VAE decoder's conv_out + postprocess
+    (rint(clamp(y / 2 + 0.5, 0, 1) * 255)).  return_float: (uint8, fp32 NCHW [B, 3, H, W] y).  One
+    `vae_conv_out_u8_kernel`."""
+    B, H, W, Cin = _image_shape(x, "vae_conv_out_u8", "x", BF16)
+    img = torch.empty((B, H, W, 3), device=x.device, dtype=torch.uint8)
+    y = torch.empty((B, 3, H, W), device=x.device, dtype=torch.float32) if return_float else None
+    lib = _begin()
+    _cabi.check(lib.sb200_vae_conv_out_u8(_ctx(x), _stream(), _p(x), _p(w_packed), _p(bias), _p(img), _p(y), B, H, W,
+                                          Cin))
+    _count("vae_conv_out_u8", 2.0 * B * H * W * 3 * 9 * Cin)
+    return (img, y) if return_float else img
+
+
+def vae_moments(x: torch.Tensor, w_packed: torch.Tensor, bias, quant_w: torch.Tensor, quant_b: torch.Tensor,
+                eps: Optional[torch.Tensor], scaling: float) -> torch.Tensor:
+    """NHWC bf16 [B, h, w, Cin] -> fp32 [B, 4, h, w] scaled latents: the VAE encoder's conv_out (Cin -> 8), quant_conv
+    (fp32 [8, 8] + [8]), logvar clamp, mean + exp(logvar / 2) * eps (eps None: the mean), times scaling.  One
+    `vae_moments_kernel`."""
+    B, H, W, Cin = _image_shape(x, "vae_moments", "x", BF16)
+    if tuple(quant_w.shape) != (8, 8) or quant_w.dtype != torch.float32 or quant_b.dtype != torch.float32:
+        raise ValueError("vae_moments: quant_w / quant_b must be fp32 [8, 8] / [8]")
+    if eps is not None and (tuple(eps.shape) != (B, 4, H, W) or eps.dtype != torch.float32 or not eps.is_contiguous()):
+        raise ValueError(f"vae_moments: eps {tuple(eps.shape)} {eps.dtype} is not a contiguous fp32 [{B}, 4, {H}, {W}]")
+    z = torch.empty((B, 4, H, W), device=x.device, dtype=torch.float32)
+    lib = _begin()
+    _cabi.check(lib.sb200_vae_moments(_ctx(x), _stream(), _p(x), _p(w_packed), _p(bias), _p(quant_w.contiguous()),
+                                      _p(quant_b.contiguous()), _p(eps), float(scaling), _p(z), B, H, W, Cin))
+    _count("vae_moments", 2.0 * B * H * W * 8 * 9 * Cin)
+    return z
+
+
+def vae_post_quant(z: torch.Tensor, post_w: torch.Tensor, post_b: torch.Tensor, scaling: float) -> torch.Tensor:
+    """fp32 NCHW [B, 4, h, w] -> post_quant_conv(z / scaling) (fp32 [4, 4] + [4]).  One `vae_post_quant_kernel`."""
+    if z.dim() != 4 or z.shape[1] != 4 or z.dtype != torch.float32 or not z.is_contiguous():
+        raise ValueError(f"vae_post_quant: z {tuple(z.shape)} {z.dtype} is not a contiguous fp32 [B, 4, h, w]")
+    if tuple(post_w.shape) != (4, 4) or post_w.dtype != torch.float32 or post_b.dtype != torch.float32:
+        raise ValueError("vae_post_quant: post_w / post_b must be fp32 [4, 4] / [4]")
+    out = torch.empty_like(z)
+    lib = _begin()
+    _cabi.check(lib.sb200_vae_post_quant(_ctx(z), _stream(), _p(z), _p(post_w.contiguous()), _p(post_b.contiguous()),
+                                         float(scaling), _p(out), z.shape[0], z.shape[2] * z.shape[3]))
+    _count("vae_post_quant")
+    return out
+
+
+def softmax_rows(s: torch.Tensor, scale: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp32 scores [rows, cols] (row-strided) -> bf16 softmax(scale * s) per row, max and sum in fp32.  One
+    `softmax_rows_kernel`."""
+    rows, cols = s.shape
+    _row_matrix(s, (rows, cols), "softmax_rows", "s", dtype=torch.float32)
+    p = _row_matrix_out(out, (rows, cols), "softmax_rows")
+    if p is None:
+        p = torch.empty((rows, cols), device=s.device, dtype=BF16)
+    lib = _begin()
+    _cabi.check(lib.sb200_softmax_rows(_ctx(s), _stream(), _p(s), s.stride(0), _p(p), p.stride(0), rows, cols,
+                                       float(scale)))
+    _count("softmax_rows")
+    return p
 
 
 def cfg_ddim(eps2: torch.Tensor, guidance: float, x: Optional[torch.Tensor] = None, a_t: float = 1.0,

@@ -29,7 +29,8 @@ def synthetic_tensor(key: str, shape, seed: int = 0, device="cpu") -> torch.Tens
     g = _gen(key, seed, device)
     shape = tuple(shape)
     leaf = key.rsplit(".", 1)[-1]
-    is_norm = ".norm" in key or key.startswith("conv_norm_out") or ".norm." in key
+    is_norm = (".norm" in key or key.startswith("conv_norm_out") or ".conv_norm_out." in key
+               or ".group_norm." in key)  # the last two: the VAE's encoder / decoder and mid-block attention
     if is_norm and len(shape) == 1:
         t = torch.randn(shape, generator=g, device=device) * 0.1
         if leaf == "weight":

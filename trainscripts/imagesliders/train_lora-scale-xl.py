@@ -4,7 +4,8 @@
         --config_file 'trainscripts/imagesliders/data/config-xl.yaml' --folder_main 'datasets/eyesize/' \
         --folders 'bigsize, smallsize' --scales '1, -1'
 
-`folder_main/<folder>/` holds VAE-encoded latents (`<name>.pt`), see sliders_b200/cli.py.  Needs an H100."""
+`folder_main/<folder>/` holds images (encoded each iteration by the VAE of `--vae`, default the model directory's) or
+VAE-encoded latents (`<name>.pt`), see sliders_b200/cli.py.  Needs an H100."""
 import os
 import sys
 
