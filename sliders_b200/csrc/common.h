@@ -82,7 +82,6 @@ inline int pdl_mode() {
   }();
   return m;
 }
-inline bool pdl_enabled() { return pdl_mode() != 0; }
 
 // Per-call hint set by the C-ABI entry points: PDL pays off for small launches (launch latency and prologue are a
 // visible share: +3 % at 2 passes per forward) and costs ~1 % on machine-filling ones (8 passes), so the big shapes
@@ -92,22 +91,33 @@ inline bool& pdl_hint() {
   return h;
 }
 
-// <<<grid, block, smem, stream>>> with the programmatic-stream-serialization attribute (the kernel must call
-// pdl_wait() before touching global memory)
+// <<<grid, block, smem, stream>>> in clusters of `cluster_x` CTAs along x (1: no cluster), with the
+// programmatic-stream-serialization attribute as pdl_mode() / pdl_hint() decide (the kernel must call pdl_wait() before
+// touching global memory)
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                              Args&&... args) {
+inline cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                             unsigned cluster_x, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
+  cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = (pdl_mode() == 2 || (pdl_mode() == 1 && pdl_hint())) ? 1 : 0;
+  attr[1].id = cudaLaunchAttributeClusterDimension;
+  attr[1].val.clusterDim.x = cluster_x;
+  attr[1].val.clusterDim.y = 1;
+  attr[1].val.clusterDim.z = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = 1;
+  cfg.numAttrs = cluster_x > 1 ? 2 : 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                              Args&&... args) {
+  return launch_ex(kernel, grid, block, smem, stream, 1u, static_cast<Args&&>(args)...);
 }
 
 inline Ctx* as_ctx(void* h) { return reinterpret_cast<Ctx*>(h); }

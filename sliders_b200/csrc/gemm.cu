@@ -18,6 +18,11 @@
 // either width.  Each CTA's ring is sized from its share of the SM's shared memory.
 // CTA pairs (kCtas = 2): a cluster of two CTAs on consecutive 128-row tiles of the same N tile.  Each CTA loads half
 // of the W (and LoRA-down) rows of a stage and multicasts them to both, which halves the weight traffic from L2.
+// The ring protocol is written once for this kernel and gemm_wide_kernel below: gemm_prologue (descriptor prefetch,
+// barrier init, sync), produce (the producer's k-block loop, CTA-pair multicast included) and consume (the consumers'
+// k-block loop and stage handback); tile_coords maps a tile index to its (mt, nt) and tile_out_row a tile row to its
+// output row.  On the host the three entry points fill in their A operand and hand over to plan_and_launch (epilogue
+// and LoRA checks, tile choice, W / LoRA-down maps), launch_gemm (ring sizing) and launch_checked (the launch).
 //
 // A-operand addressing modes:
 //   plain   2-D [M, K], optionally split along K over two sources (skip-connection concat, conv_shortcut)
@@ -166,8 +171,16 @@ template <int BN>
 __device__ __forceinline__ void wgmma_main(float* d, uint64_t a, uint64_t b) {
   if constexpr (BN == 64)
     wgmma_ss_n64(d, a, b, 1u);
-  else
+  else if constexpr (BN == 128)
     wgmma_ss_n128(d, a, b, 1u);
+  else
+    wgmma_ss_n256(d, a, b, 1u);
+}
+
+// Output tile t of the launch order -> its row tile mt and N tile nt
+__device__ __forceinline__ void tile_coords(const GemmParams& p, int t, int& mt, int& nt) {
+  mt = p.n_fast ? t / p.num_n_tiles : t % p.num_m_tiles;
+  nt = p.n_fast ? t % p.num_n_tiles : t / p.num_m_tiles;
 }
 
 // First output pixel (b0, h0, w0) of conv sub-tile `st` (w fastest, then h, then batch).
@@ -223,37 +236,48 @@ __device__ __forceinline__ void load_a(const GemmParams& p, const AOrigin& o, in
   }
 }
 
-template <int BN, int kCtas, int RT>
-__global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(const __grid_constant__ GemmParams p) {
+// Output row of row r of 128-row sub-tile st (the conv patch mapping of conv_origin), or -1 for a padding row (the
+// phantom sub-tile of an odd pair has only padding rows)
+__device__ __forceinline__ int tile_out_row(const GemmParams& p, int st, int r) {
+  if (p.a_mode == 0) {
+    const int m = st * kBM + r;
+    return m < p.M ? m : -1;
+  }
+  int b0, h0, w0;
+  conv_origin(p, st, b0, h0, w0);
+  const int iw = r % p.bw;
+  const int t2 = r / p.bw;
+  const int ih = t2 % p.bh;
+  const int ib = t2 / p.bh;
+  const int b = b0 + ib, h = h0 + ih, w = w0 + iw;
+  return (ib < p.bb && b < p.B && h < p.H && w < p.W) ? (b * p.H + h) * p.W + w : -1;
+}
+
+// The stage ring in shared memory: `stages` stages of stage_bytes from `tiles` on, each with a full barrier (its TMA
+// bytes have landed) and an empty barrier (every consumer warpgroup of every CTA the stage feeds is done reading it)
+struct Ring {
+  uint32_t full, empty, tiles, stage_bytes;
+  int stages;
+};
+
+// Prologue of both GEMM kernels: descriptor prefetch and barrier init, which overlap the previous kernel's tail, then
+// the block / cluster sync and pdl_wait; global memory is touched only after it
+template <int kCtas>
+__device__ __forceinline__ Ring gemm_prologue(const GemmParams& p, bool has_lora) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  const uint32_t base = (raw_addr + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024 B alignment
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t cta_rank = kCtas == 2 ? cluster_ctarank() : 0u;
-  const int S = p.stages;
-  const uint32_t bar_full = base;            // S barriers
-  const uint32_t bar_empty = base + 8u * S;  // S barriers
-  const uint32_t tiles = base + kBarRegion;
-  // launch_gemm runs every LoRA call on an RT > 0 instantiation, so the RT = 0 ones carry no LoRA code; GEGLU never
-  // comes with LoRA (sb200_gemm refuses it), so the RT > 0 ones carry no GEGLU code, whose gate registers would
-  // otherwise stay live across the LoRA update and spill the 96-register instantiations
-  const bool has_lora = RT != 0 && (p.flags & SB200_EPI_LORA) != 0;
-  const bool geglu = RT == 0 && (p.flags & SB200_EPI_GEGLU) != 0;
-  constexpr int rt = RT;  // LoRA-down rows of a stage (0 without LoRA)
-
-  if (warp == 0 && lane == 0) {
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024 B alignment
+  const Ring ring{base, base + 8u * p.stages, base + kBarRegion, static_cast<uint32_t>(p.stage_bytes), p.stages};
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmA[0]);
     tma_prefetch_desc(&p.tmB);
     if (has_lora) tma_prefetch_desc(&p.tmL);
   }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < S; ++i) {
-      mbar_init(bar_full + 8u * i, 1);
-      mbar_init(bar_empty + 8u * i, 2 * kCtas);  // one arrival per consumer warpgroup of every CTA the stage feeds
-    }
+  if (threadIdx.x == 32) {
+    // stage i's full barrier, then its empty one: one arrival per consumer warpgroup of every CTA the stage feeds
+    for (int i = 0; i < ring.stages; ++i)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) mbar_init((e ? ring.empty : ring.full) + 8u * i, e ? 2 * kCtas : 1);
     fence_barrier_init();
   }
   if constexpr (kCtas == 2) {
@@ -261,109 +285,145 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
   } else {
     __syncthreads();
   }
-  pdl_wait();  // everything above overlapped the previous kernel's tail; global memory is touched only below
+  pdl_wait();
+  return ring;
+}
 
-  const int t = blockIdx.x / kCtas;  // this CTA's (pair's) output tile
-  const int num_n_tiles = p.num_n_tiles, num_m_tiles = p.num_m_tiles;
-  const int mt = p.n_fast ? t / num_n_tiles : t % num_m_tiles;
-  const int nt = p.n_fast ? t % num_n_tiles : t / num_m_tiles;
+// TMA producer, one converged warp: k-blocks [kb_lo, kb_hi) of the tile at A origin `ao` and N tile nt into the ring;
+// `stage` and `phase` run on across calls.  A stage holds the A tile, the tile's kBRows W rows (GEGLU: its value rows,
+// then the matching gate rows from row N/2 on) and RT LoRA-down rows.  In a CTA pair each CTA loads half of the W and
+// LoRA-down rows (GEGLU: CTA 1 the gate rows) and multicasts them to both.
+template <int kBRows, int RT, int kCtas>
+__device__ __forceinline__ void produce(const GemmParams& p, const Ring& ring, const AOrigin& ao, int nt,
+                                        uint32_t cta_rank, bool geglu, bool has_lora, int kb_lo, int kb_hi,
+                                        int& stage, uint32_t& phase) {
+  constexpr uint32_t a_bytes = kBM * 128, b_bytes = kBRows * 128;
+  const uint32_t tx = static_cast<uint32_t>(p.a_tx) + b_bytes + static_cast<uint32_t>(RT) * 128u;
+  int brow;  // the first W row this CTA loads
+  if (geglu) {
+    const int half = kBRows >> 1;
+    brow = (kCtas == 2 && cta_rank == 1) ? (p.N >> 1) + nt * half : nt * half;
+  } else {
+    brow = nt * kBRows + static_cast<int>(cta_rank) * p.b_rows;
+  }
+  for (int kb = kb_lo; kb < kb_hi; ++kb) {
+    const uint32_t full_bar = ring.full + 8u * stage;
+    mbar_wait(ring.empty + 8u * stage, phase ^ 1u);
+    if (elect_one()) {
+      mbar_expect_tx(full_bar, tx);
+      const uint32_t sA = ring.tiles + static_cast<uint32_t>(stage) * ring.stage_bytes;
+      const uint32_t sB = sA + a_bytes;
+      load_a(p, ao, kb, sA, full_bar);
+      if constexpr (kCtas == 2) {
+        const uint32_t boff = cta_rank * static_cast<uint32_t>(p.b_rows) * 128u;
+        tma_load_2d_mc(sB + boff, &p.tmB, full_bar, kb * kBK, brow, 3);
+        if (has_lora)
+          tma_load_2d_mc(sB + b_bytes + cta_rank * static_cast<uint32_t>(p.l_rows) * 128u, &p.tmL, full_bar, kb * kBK,
+                         static_cast<int>(cta_rank) * p.l_rows, 3);
+      } else {
+        tma_load_2d(sB, &p.tmB, full_bar, kb * kBK, brow);
+        if (geglu) tma_load_2d(sB + (b_bytes >> 1), &p.tmB, full_bar, kb * kBK, (p.N >> 1) + nt * (kBRows >> 1));
+        if (has_lora) tma_load_2d(sB + b_bytes, &p.tmL, full_bar, kb * kBK, 0);
+      }
+    }
+    __syncwarp();
+    if (++stage == ring.stages) {
+      stage = 0;
+      phase ^= 1u;
+    }
+  }
+}
+
+// reg_fence over an accumulator array, once its wgmmas have completed
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) reg_fence(r[i]);
+}
+
+// Main loop of consumer warpgroup wg (rows wg * 64 ..) over k-blocks [kb_lo, kb_hi): zeroes acc (m64 x BN) and accl
+// (t = A.down^T, m64 x RT), issues each k-block's wgmmas with one k-block's group kept in flight, and hands each stage
+// back (to both CTAs of a pair) once the products reading it are done.  On return every product has completed; the
+// caller fences the registers (fence_regs).  Returns the stage of the last k-block, which it has not handed back.
+template <int BN, int RT, int kCtas, int NL>
+__device__ __forceinline__ int consume(float (&acc)[BN / 2], float (&accl)[NL], const Ring& ring, int wg,
+                                       uint32_t cta_rank, int kb_lo, int kb_hi, int& stage, uint32_t& phase) {
+  constexpr uint32_t a_bytes = kBM * 128, b_bytes = BN * 128;
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < NL; ++i) accl[i] = 0.f;
+  const bool signal = (threadIdx.x & 127) == 0;
+  const uint32_t peer_empty = kCtas == 2 ? mapa_u32(ring.empty, cta_rank ^ 1u) : 0u;
+  int prev = 0;
+  for (int kb = kb_lo; kb < kb_hi; ++kb) {
+    mbar_wait(ring.full + 8u * stage, phase);
+    const uint32_t stage_base = ring.tiles + static_cast<uint32_t>(stage) * ring.stage_bytes;
+    const uint32_t sA = stage_base + static_cast<uint32_t>(wg) * 64u * 128u;
+    const uint32_t sB = stage_base + a_bytes;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBK / 16; ++k) {
+      const uint64_t adesc = gmma_desc_sw128(sA + 32u * k);
+      wgmma_main<BN>(acc, adesc, gmma_desc_sw128(sB + 32u * k));
+      if constexpr (RT == 16)
+        wgmma_ss_n16(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
+      else if constexpr (RT == 32)
+        wgmma_ss_n32(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
+      else if constexpr (RT == 64)
+        wgmma_ss_n64(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();  // the previous k-block's products have read their stage: hand it back to the producer(s)
+    if (kb > kb_lo && signal) {
+      mbar_arrive(ring.empty + 8u * prev);
+      if (kCtas == 2) mbar_arrive_cluster(peer_empty + 8u * prev);
+    }
+    prev = stage;
+    if (++stage == ring.stages) {
+      stage = 0;
+      phase ^= 1u;
+    }
+  }
+  wgmma_wait<0>();
+  return prev;
+}
+
+template <int BN, int kCtas, int RT>
+__global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(const __grid_constant__ GemmParams p) {
+  // launch_gemm runs every LoRA call on an RT > 0 instantiation, so the RT = 0 ones carry no LoRA code; GEGLU never
+  // comes with LoRA (sb200_gemm refuses it), so the RT > 0 ones carry no GEGLU code, whose gate registers would
+  // otherwise stay live across the LoRA update and spill the 96-register instantiations
+  const bool has_lora = RT != 0 && (p.flags & SB200_EPI_LORA) != 0;
+  const bool geglu = RT == 0 && (p.flags & SB200_EPI_GEGLU) != 0;
+  constexpr int rt = RT;  // LoRA-down rows of a stage (0 without LoRA)
+  const Ring ring = gemm_prologue<kCtas>(p, has_lora);
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const uint32_t cta_rank = kCtas == 2 ? cluster_ctarank() : 0u;
+  int mt, nt;
+  tile_coords(p, blockIdx.x / kCtas, mt, nt);  // this CTA's (pair's) output tile
   const int st = mt * kCtas + static_cast<int>(cta_rank);  // this CTA's 128-row sub-tile
   const int kb_lo = p.sk_ws ? static_cast<int>(blockIdx.y) * p.sk_kb : 0;
   const int kb_hi = p.sk_ws ? min(p.kblocks, kb_lo + p.sk_kb) : p.kblocks;
-  const uint32_t stage_bytes = static_cast<uint32_t>(p.stage_bytes);
-  const uint32_t a_bytes = kBM * 128;
-  const uint32_t b_bytes = static_cast<uint32_t>(BN) * 128;  // W rows of a stage (both halves for a pair)
+  int stage = 0;
+  uint32_t phase = 0;
 
   if (warp == kProducerWarp) {
-    // ------------------------------------------------------------------ TMA producer, converged warp
-    const uint32_t tx = static_cast<uint32_t>(p.a_tx) + b_bytes + static_cast<uint32_t>(rt) * 128u;
-    const AOrigin ao = a_origin(p, st);
-    // W rows this CTA loads (a pair: half each, multicast to both)
-    int brow;
-    if (geglu) {
-      const int half = BN >> 1;
-      brow = (kCtas == 2 && cta_rank == 1) ? (p.N >> 1) + nt * half : nt * half;
-    } else {
-      brow = nt * BN + static_cast<int>(cta_rank) * p.b_rows;
-    }
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int kb = kb_lo; kb < kb_hi; ++kb) {
-      const uint32_t full_bar = bar_full + 8u * stage, empty_bar = bar_empty + 8u * stage;
-      mbar_wait(empty_bar, phase ^ 1u);
-      if (elect_one()) {
-        mbar_expect_tx(full_bar, tx);
-        const uint32_t sA = tiles + static_cast<uint32_t>(stage) * stage_bytes;
-        const uint32_t sB = sA + a_bytes;
-        load_a(p, ao, kb, sA, full_bar);
-        if constexpr (kCtas == 2) {
-          const uint32_t boff = cta_rank * static_cast<uint32_t>(p.b_rows) * 128u;
-          tma_load_2d_mc(sB + boff, &p.tmB, full_bar, kb * kBK, brow, 3);
-          if (has_lora)
-            tma_load_2d_mc(sB + b_bytes + cta_rank * static_cast<uint32_t>(p.l_rows) * 128u, &p.tmL, full_bar, kb * kBK,
-                           static_cast<int>(cta_rank) * p.l_rows, 3);
-        } else {
-          tma_load_2d(sB, &p.tmB, full_bar, kb * kBK, brow);
-          if (geglu) tma_load_2d(sB + (b_bytes >> 1), &p.tmB, full_bar, kb * kBK, (p.N >> 1) + nt * (BN >> 1));
-          if (has_lora) tma_load_2d(sB + b_bytes, &p.tmL, full_bar, kb * kBK, 0);
-        }
-      }
-      __syncwarp();
-      if (++stage == S) {
-        stage = 0;
-        phase ^= 1u;
-      }
-    }
+    produce<BN, RT, kCtas>(p, ring, a_origin(p, st), nt, cta_rank, geglu, has_lora, kb_lo, kb_hi, stage, phase);
   } else {
     // ------------------------------------------------------------------ consumers: main loop
     const int wg = warp >> 2;
     constexpr int kAccl = RT > 32 ? RT / 2 : 16;  // t = A.down^T fragment registers
     float acc[BN / 2];
     float accl[kAccl];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < kAccl; ++i) accl[i] = 0.f;
-    const bool signal = (threadIdx.x & 127) == 0;
-    const uint32_t peer_empty = kCtas == 2 ? mapa_u32(bar_empty, cta_rank ^ 1u) : 0u;
-    int stage = 0, prev = 0;
-    uint32_t phase = 0;
-    for (int kb = kb_lo; kb < kb_hi; ++kb) {
-      mbar_wait(bar_full + 8u * stage, phase);
-      const uint32_t sA = tiles + static_cast<uint32_t>(stage) * stage_bytes + static_cast<uint32_t>(wg) * 64u * 128u;
-      const uint32_t sB = tiles + static_cast<uint32_t>(stage) * stage_bytes + a_bytes;
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < kBK / 16; ++k) {
-        const uint64_t adesc = gmma_desc_sw128(sA + 32u * k);
-        wgmma_main<BN>(acc, adesc, gmma_desc_sw128(sB + 32u * k));
-        if constexpr (rt == 16)
-          wgmma_ss_n16(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
-        else if constexpr (rt == 32)
-          wgmma_ss_n32(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
-        else if constexpr (rt == 64)
-          wgmma_ss_n64(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();  // the previous k-block's products have read their stage: hand it back to the producer(s)
-      if (kb > kb_lo && signal) {
-        mbar_arrive(bar_empty + 8u * prev);
-        if (kCtas == 2) mbar_arrive_cluster(peer_empty + 8u * prev);
-      }
-      prev = stage;
-      if (++stage == S) {
-        stage = 0;
-        phase ^= 1u;
-      }
-    }
-    wgmma_wait<0>();
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
-#pragma unroll
-    for (int i = 0; i < kAccl; ++i) reg_fence(accl[i]);
+    consume<BN, RT, kCtas>(acc, accl, ring, wg, cta_rank, kb_lo, kb_hi, stage, phase);
+    fence_regs(acc);
+    fence_regs(accl);
 
     // ------------------------------------------------------------------ epilogue
-    const uint32_t accs = tiles;  // fp32 accumulator tile, over the stage ring
+    const uint32_t accs = ring.tiles;  // fp32 accumulator tile, over the stage ring
     constexpr int kStride = acc_stride(BN, RT);
     asm volatile("bar.sync %0, %1;" ::"n"(kConsumerBar), "n"(32 * kEpiWarps) : "memory");  // both warpgroups done reading
     store_frag<BN>(acc, accs, wg * 64, 0, kStride);
@@ -396,30 +456,11 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
     // writes; in between every thread touches only its own row.  The buffers sit in the ring behind the accumulator
     // tile: every k-block's loads have landed (this CTA waited on each full barrier, whose byte count includes the
     // peer's multicast) and both warpgroups have passed kConsumerBar, so nothing else writes or reads there.
-    const uint32_t epi = tiles + static_cast<uint32_t>(acc_tile_bytes(BN, RT));
+    const uint32_t epi = accs + static_cast<uint32_t>(acc_tile_bytes(BN, RT));
     const uint32_t ebuf = epi + static_cast<uint32_t>(warp) * (kEpiBufBytes + p.up_buf_bytes);
     const uint32_t ubuf = ebuf + kEpiBufBytes;  // p.up_buf_bytes of lora_up rows
     const uint32_t arow = accs + static_cast<uint32_t>((q * 32 + lane) * kStride) * 4u;
-    // output row of this thread's accumulator row (q * 32 + lane), or -1 (padding row of the tile)
-    int my_row = -1, my_batch = 0;
-    {
-      const int r = q * 32 + lane;
-      if (p.a_mode == 0) {
-        const int m = st * kBM + r;
-        if (m < p.M) my_row = m;
-        my_batch = (p.flags & SB200_EPI_ROWBIAS) ? m / p.rows_per_batch : 0;
-      } else if (st < p.num_sub) {
-        int b0, h0, w0;
-        conv_origin(p, st, b0, h0, w0);
-        const int iw = r % p.bw;
-        const int t2 = r / p.bw;
-        const int ih = t2 % p.bh;
-        const int ib = t2 / p.bh;
-        const int b = b0 + ib, h = h0 + ih, w = w0 + iw;
-        if (ib < p.bb && b < p.B && h < p.H && w < p.W) my_row = (b * p.H + h) * p.W + w;
-        my_batch = b;
-      }
-    }
+    const int my_row = tile_out_row(p, st, q * 32 + lane);  // output row of this thread's accumulator row, or -1
     const bool row_ok = my_row >= 0;
     float lscale = has_lora ? (p.lora_scale_dev ? p.lora_scale * __ldg(p.lora_scale_dev) : p.lora_scale) : 0.f;
     // this thread's row factor, read once per tile; without a vector nothing is loaded and lscale keeps its bits
@@ -458,7 +499,8 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
     const bool staged = has_resid || has_lora;
     if (staged && my_slabs > 0) prefetch_resid(hsel * kSlab, min(kSlab, ncols_valid - hsel * kSlab));
     const __nv_bfloat16* rb =
-        (p.flags & SB200_EPI_ROWBIAS) ? p.rowbias + static_cast<size_t>(row_ok ? my_batch : 0) * p.Nout : nullptr;
+        (p.flags & SB200_EPI_ROWBIAS) ? p.rowbias + static_cast<size_t>(row_ok ? my_row / p.rows_per_batch : 0) * p.Nout
+                                      : nullptr;
     float tl[8];
     int group_lo = 0, group_hi = 0;  // output-column range of the adaptor whose t = A.down^T is held in tl
     // tl = lscale * t, from the 8 t columns of this row starting at column j; rank 4 uses the first 4 (the row's 4
@@ -573,8 +615,9 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
 //   warpgroup 2    producer: gives its registers to the consumers (setmaxnreg 40); one elected thread of warp 8 issues
 //                  the TMA loads, running ahead into the next tile while the consumers finish the current epilogue
 //   warpgroups 0/1 consumers (setmaxnreg 232): rows 0..63 / 64..127, an m64 x 256 accumulator of 128 registers
-// The k-loop, its barrier protocol and the LoRA-down rows behind the W rows are those of gemm_kernel; the ring's phases
-// run on across tiles.  The epilogue works on the accumulator registers: per element it applies, in gemm_kernel's
+// The k-loop, its barrier protocol and the LoRA-down rows behind the W rows are gemm_kernel's (gemm_prologue, produce
+// and consume, called once per tile); the ring's stage and phase run on across tiles, and the consumers hand each
+// tile's last stage back once its wgmmas are done.  The epilogue works on the accumulator registers: per element it applies, in gemm_kernel's
 // order and with its expressions, the LoRA update, bias, row bias and GEGLU, rounds to bf16, adds the residual in bf16,
 // and leaves through a swizzled staging buffer (two per warpgroup, 64 rows x 64 columns each) with coalesced stores.
 // Only t = A.down^T and the tile's lora_up rows are staged in shared memory.  No split-K or CTA pairs: those stay on
@@ -597,84 +640,23 @@ __host__ __device__ constexpr int wide_epi_bytes(int rt, int r) {
   return 2 * kWideStgBytes + wide_t_bytes(rt) + (rt ? kWideBN * r * 4 : 0);
 }
 
-// Output row of row r of 128-row sub-tile st (the conv patch mapping of conv_origin), or -1 for a padding row
-__device__ __forceinline__ int tile_out_row(const GemmParams& p, int st, int r) {
-  if (p.a_mode == 0) {
-    const int m = st * kBM + r;
-    return m < p.M ? m : -1;
-  }
-  int b0, h0, w0;
-  conv_origin(p, st, b0, h0, w0);
-  const int iw = r % p.bw;
-  const int t2 = r / p.bw;
-  const int ih = t2 % p.bh;
-  const int ib = t2 / p.bh;
-  const int b = b0 + ib, h = h0 + ih, w = w0 + iw;
-  return (ib < p.bb && b < p.B && h < p.H && w < p.W) ? (b * p.H + h) * p.W + w : -1;
-}
-
 template <int RT, bool GEGLU>
 __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid_constant__ GemmParams p) {
-  pdl_trigger();
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024 B alignment
+  const Ring ring = gemm_prologue<1>(p, RT != 0);
   const int warp = threadIdx.x >> 5;
-  const int S = p.stages;
-  const uint32_t bar_full = base;            // S barriers
-  const uint32_t bar_empty = base + 8u * S;  // S barriers
-  const uint32_t tiles = base + kBarRegion;
-  const uint32_t stage_bytes = static_cast<uint32_t>(p.stage_bytes);
-  constexpr uint32_t a_bytes = kBM * 128;
-  constexpr uint32_t b_bytes = kWideBN * 128;
   constexpr bool geglu = GEGLU;
   const int num_tiles = p.num_m_tiles * p.num_n_tiles;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&p.tmA[0]);
-    tma_prefetch_desc(&p.tmB);
-    if (RT) tma_prefetch_desc(&p.tmL);
-  }
-  if (threadIdx.x == 32) {
-    for (int i = 0; i < S; ++i) {
-      mbar_init(bar_full + 8u * i, 1);
-      mbar_init(bar_empty + 8u * i, 2);  // one arrival per consumer warpgroup
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-  pdl_wait();  // everything above overlapped the previous kernel's tail; global memory is touched only below
+  int stage = 0;
+  uint32_t phase = 0;
 
   if (warp >= 8) {
     // ------------------------------------------------------------------ TMA producer
     setmaxnreg_dec<40>();
     if (warp != 8) return;
-    const uint32_t tx = static_cast<uint32_t>(p.a_tx) + b_bytes + static_cast<uint32_t>(RT) * 128u;
-    int stage = 0;
-    uint32_t phase = 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int mt = p.n_fast ? t / p.num_n_tiles : t % p.num_m_tiles;
-      const int nt = p.n_fast ? t % p.num_n_tiles : t / p.num_m_tiles;
-      const AOrigin ao = a_origin(p, mt);
-      // GEGLU: the tile's 128 value rows of W, then the 128 matching gate rows
-      const int brow = geglu ? nt * (kWideBN / 2) : nt * kWideBN;
-      for (int kb = 0; kb < p.kblocks; ++kb) {
-        const uint32_t full_bar = bar_full + 8u * stage, empty_bar = bar_empty + 8u * stage;
-        mbar_wait(empty_bar, phase ^ 1u);
-        if (elect_one()) {
-          mbar_expect_tx(full_bar, tx);
-          const uint32_t sA = tiles + static_cast<uint32_t>(stage) * stage_bytes;
-          const uint32_t sB = sA + a_bytes;
-          load_a(p, ao, kb, sA, full_bar);
-          tma_load_2d(sB, &p.tmB, full_bar, kb * kBK, brow);
-          if (geglu) tma_load_2d(sB + (b_bytes >> 1), &p.tmB, full_bar, kb * kBK, (p.N >> 1) + brow);
-          if (RT) tma_load_2d(sB + b_bytes, &p.tmL, full_bar, kb * kBK, 0);
-        }
-        __syncwarp();
-        if (++stage == S) {
-          stage = 0;
-          phase ^= 1u;
-        }
-      }
+      int mt, nt;
+      tile_coords(p, t, mt, nt);
+      produce<kWideBN, RT, 1>(p, ring, a_origin(p, mt), nt, 0u, geglu, RT != 0, 0, p.kblocks, stage, phase);
     }
     return;
   }
@@ -686,7 +668,6 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
   const int lane = threadIdx.x & 31;
   const int q = lane & 3;
   const int fr0 = (warp & 3) * 16 + (lane >> 2);  // accumulator rows of this thread: fr0 and fr0 + 8 (of 64)
-  const bool signal = tid == 0;
   const bool has_lora = RT != 0;
   const bool has_resid = (p.flags & SB200_EPI_RESID) != 0;
   const bool has_bias = (p.flags & SB200_EPI_BIAS) != 0;
@@ -694,7 +675,7 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
   const int r = has_lora ? p.lora_r : 0;
   const float lscale = has_lora ? (p.lora_scale_dev ? p.lora_scale * __ldg(p.lora_scale_dev) : p.lora_scale) : 0.f;
   constexpr int nchunks = (GEGLU ? kWideBN / 2 : kWideBN) / kWideChunk;  // p.ncols_out / kWideChunk
-  const uint32_t epi = tiles + static_cast<uint32_t>(S) * stage_bytes +
+  const uint32_t epi = ring.tiles + static_cast<uint32_t>(ring.stages) * ring.stage_bytes +
                        static_cast<uint32_t>(wg) * static_cast<uint32_t>(wide_epi_bytes(RT, r));
   const uint32_t tbuf = epi + 2 * kWideStgBytes;  // [64][RT + 4] fp32: t of this warpgroup's rows
   const uint32_t ubuf = tbuf + wide_t_bytes(RT);  // [256][r] fp32: the tile's lora_up rows
@@ -704,12 +685,9 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
   const uint32_t bar_id = kWideBarBase + wg;
   auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); };
 
-  int stage = 0;
-  uint32_t phase = 0;
   for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-    const int mt = p.n_fast ? t / p.num_n_tiles : t % p.num_m_tiles;
-    const int nt = p.n_fast ? t % p.num_n_tiles : t / p.num_m_tiles;
-    const int st = mt;
+    int st, nt;
+    tile_coords(p, t, st, nt);
     const int n_base = nt * p.ncols_out;
     int orow[4];  // output rows this thread copies
 #pragma unroll
@@ -736,40 +714,10 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
     if (has_resid) prefetch_resid(0, epi);
     float acc[kWideBN / 2];
     float accl[RT ? RT / 2 : 1];
-#pragma unroll
-    for (int i = 0; i < kWideBN / 2; ++i) acc[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < (RT ? RT / 2 : 1); ++i) accl[i] = 0.f;
-    int prev = 0;
-    for (int kb = 0; kb < p.kblocks; ++kb) {
-      mbar_wait(bar_full + 8u * stage, phase);
-      const uint32_t sA = tiles + static_cast<uint32_t>(stage) * stage_bytes + static_cast<uint32_t>(wg) * 64u * 128u;
-      const uint32_t sB = tiles + static_cast<uint32_t>(stage) * stage_bytes + a_bytes;
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < kBK / 16; ++k) {
-        const uint64_t adesc = gmma_desc_sw128(sA + 32u * k);
-        wgmma_ss_n256(acc, adesc, gmma_desc_sw128(sB + 32u * k), 1u);
-        if constexpr (RT == 16)
-          wgmma_ss_n16(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
-        else if constexpr (RT == 32)
-          wgmma_ss_n32(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();  // the previous k-block's products have read their stage: hand it back to the producer
-      if (kb > 0 && signal) mbar_arrive(bar_empty + 8u * prev);
-      prev = stage;
-      if (++stage == S) {
-        stage = 0;
-        phase ^= 1u;
-      }
-    }
-    wgmma_wait<0>();
-    if (signal) mbar_arrive(bar_empty + 8u * prev);  // the last stage of the tile, for the producer's next tile
-#pragma unroll
-    for (int i = 0; i < kWideBN / 2; ++i) reg_fence(acc[i]);
-#pragma unroll
-    for (int i = 0; i < (RT ? RT / 2 : 1); ++i) reg_fence(accl[i]);
+    const int last = consume<kWideBN, RT, 1>(acc, accl, ring, wg, 0u, 0, p.kblocks, stage, phase);
+    if (tid == 0) mbar_arrive(ring.empty + 8u * last);  // the last stage of the tile, for the producer's next tile
+    fence_regs(acc);
+    fence_regs(accl);
 
     // ------------------------------------------------------------------ epilogue
     if constexpr (RT != 0) {
@@ -1007,68 +955,38 @@ static int smem_budget(const Ctx* ctx, int slots) {
   return std::min(ctx->smem_optin, ctx->smem_per_sm / slots - ctx->smem_reserved);
 }
 
-template <int BN, int kCtas, int RT>
-static int launch_gemm_bn(Ctx* ctx, cudaStream_t stream, const GemmParams& p, int smem) {
-  static bool attr_set = false;  // one flag per instantiation
-  if (!attr_set) {
-    const auto kernel = gemm_kernel<BN, kCtas, RT>;
-    constexpr int slots = gemm_slots(BN, RT);
-    SB200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin));
+// Launches kKernel, kThreads threads per CTA and built for kSlots CTAs per SM, in clusters of `cluster` CTAs.  Its
+// first launch opts it in to the SM's shared memory and checks with the occupancy calculator that kSlots CTAs fit.
+template <void (*kKernel)(GemmParams), int kThreads, int kSlots>
+static int launch_checked(Ctx* ctx, cudaStream_t stream, const GemmParams& p, dim3 grid, int smem, int cluster) {
+  static bool checked = false;  // one flag per instantiation
+  if (!checked) {
+    SB200_CUDA_CHECK(cudaFuncSetAttribute(kKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin));
     SB200_CUDA_CHECK(
-        cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+        cudaFuncSetAttribute(kKernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     int resident = 0;
     SB200_CUDA_CHECK(
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kernel, kGemmThreads, smem_budget(ctx, slots)));
-    if (resident < slots)
-      return set_error(SB200_ERR_CUDA, "gemm_kernel<%d, %d, %d>: %d CTA(s) per SM fit, built for %d", BN, kCtas, RT,
-                       resident, slots);
-    attr_set = true;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kKernel, kThreads, smem_budget(ctx, kSlots)));
+    if (resident < kSlots)
+      return set_error(SB200_ERR_CUDA, "gemm: bn=%d, %d CTA(s) per cluster, rt=%d: %d CTA(s) per SM fit, built for %d",
+                       p.bn, cluster, p.lora_rt, resident, kSlots);
+    checked = true;
   }
-  const int total = p.num_m_tiles * p.num_n_tiles;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(total * kCtas, p.sk_ws ? p.sk_splits : 1);
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = (pdl_mode() == 2 || (pdl_mode() == 1 && pdl_hint())) ? 1 : 0;
-  attr[1].id = cudaLaunchAttributeClusterDimension;
-  attr[1].val.clusterDim.x = kCtas;
-  attr[1].val.clusterDim.y = 1;
-  attr[1].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = kCtas == 2 ? 2 : 1;
-  SB200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_kernel<BN, kCtas, RT>, p));
-  (void)ctx;
+  SB200_CUDA_CHECK(launch_ex(kKernel, grid, dim3(kThreads), smem, stream, cluster, p));
   return 0;
 }
 
-template <int RT, bool GEGLU>
-static int launch_gemm_wide(Ctx* ctx, cudaStream_t stream, const GemmParams& p, int smem) {
-  static bool attr_set = false;  // one flag per instantiation
-  const auto kernel = gemm_wide_kernel<RT, GEGLU>;
-  if (!attr_set) {
-    SB200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin));
-    SB200_CUDA_CHECK(
-        cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    int resident = 0;
-    SB200_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kernel, kWideThreads, smem));
-    if (resident < 1) return set_error(SB200_ERR_CUDA, "gemm_wide_kernel<%d, %d>: no CTA fits an SM", RT, GEGLU);
-    attr_set = true;
+// gemm_kernel<BN, kCtas, RT> for the call's RT
+template <int BN, int kCtas>
+static int launch_narrow(Ctx* ctx, cudaStream_t s, const GemmParams& p, int rt, int smem) {
+  const dim3 grid(p.num_m_tiles * p.num_n_tiles * kCtas, p.sk_ws ? p.sk_splits : 1);
+  constexpr int T = kGemmThreads;
+  switch (rt) {
+    case 0: return launch_checked<gemm_kernel<BN, kCtas, 0>, T, gemm_slots(BN, 0)>(ctx, s, p, grid, smem, kCtas);
+    case 16: return launch_checked<gemm_kernel<BN, kCtas, 16>, T, gemm_slots(BN, 16)>(ctx, s, p, grid, smem, kCtas);
+    case 32: return launch_checked<gemm_kernel<BN, kCtas, 32>, T, gemm_slots(BN, 32)>(ctx, s, p, grid, smem, kCtas);
+    default: return launch_checked<gemm_kernel<BN, kCtas, 64>, T, gemm_slots(BN, 64)>(ctx, s, p, grid, smem, kCtas);
   }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(std::min(p.num_m_tiles * p.num_n_tiles, ctx->num_sms));
-  cfg.blockDim = dim3(kWideThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = (pdl_mode() == 2 || (pdl_mode() == 1 && pdl_hint())) ? 1 : 0;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  SB200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, p));
-  return 0;
 }
 
 static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
@@ -1086,6 +1004,7 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
   p.stage_bytes = kBM * 128 + p.bn * 128 + (has_lora ? p.lora_rt * 128 : 0);
   p.up_buf_bytes = has_lora ? kSlab * p.lora_r * 4 : 0;
   const int rt = has_lora ? p.lora_rt : 0;
+  int st;
   if (p.bn == kWideBN) {
     // one CTA per SM: the ring gets what the two warpgroups' epilogue buffers leave of the SM's shared memory
     const int budget = smem_budget(ctx, 1);
@@ -1096,52 +1015,31 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
     p.ring_bytes = stages * p.stage_bytes + epi;
     const int smem = kBarRegion + kAlignSlack + p.ring_bytes;
     pdl_hint() = p.num_m_tiles * p.num_n_tiles <= 2 * ctx->num_sms;
-    SB200_REQUIRE(wide_lora_ok(p.lora_r, rt), "gemm: bn=256 takes LoRA of rank 4 or 8 in 16 or 32 rows (r=%d, rt=%d)",
-                  p.lora_r, rt);
-    int st;
-    switch (rt) {
-      case 0:
-        st = (p.flags & SB200_EPI_GEGLU) ? launch_gemm_wide<0, true>(ctx, stream, p, smem)
-                                         : launch_gemm_wide<0, false>(ctx, stream, p, smem);
-        break;
-      case 16: st = launch_gemm_wide<16, false>(ctx, stream, p, smem); break;
-      default: st = launch_gemm_wide<32, false>(ctx, stream, p, smem); break;
-    }
-    if (st) return st;
-    SB200_CUDA_CHECK(cudaGetLastError());
-    return 0;
-  }
-  const int grid_ctas = p.num_m_tiles * p.num_n_tiles * ctas * (p.sk_ws ? p.sk_splits : 1);
-  // A grid that gives each SM at most one CTA lets that CTA have the whole SM's shared memory (a deeper ring).
-  const int budget = smem_budget(ctx, grid_ctas > ctx->num_sms ? gemm_slots(p.bn, rt) : 1);
-  int stages = (budget - kBarRegion - kAlignSlack) / p.stage_bytes;
-  if (stages > kMaxStages) stages = kMaxStages;
-  if (stages < 2) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
-  p.stages = stages;
-  p.ring_bytes = std::max(stages * p.stage_bytes, acc_tile_bytes(p.bn, rt) + kEpiBytes + kEpiWarps * p.up_buf_bytes);
-  const int smem = kBarRegion + kAlignSlack + p.ring_bytes;
-  if (smem > budget) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
-  pdl_hint() = grid_ctas <= 2 * ctx->num_sms;
-  const int variant = (ctas == 2 ? 8 : 0) + (p.bn == 128 ? 4 : 0) + (rt == 16 ? 1 : rt == 32 ? 2 : rt == 64 ? 3 : 0);
-  cudaStream_t s = stream;
-  int st;
-  switch (variant) {
-    case 0: st = launch_gemm_bn<64, 1, 0>(ctx, s, p, smem); break;
-    case 1: st = launch_gemm_bn<64, 1, 16>(ctx, s, p, smem); break;
-    case 2: st = launch_gemm_bn<64, 1, 32>(ctx, s, p, smem); break;
-    case 3: st = launch_gemm_bn<64, 1, 64>(ctx, s, p, smem); break;
-    case 4: st = launch_gemm_bn<128, 1, 0>(ctx, s, p, smem); break;
-    case 5: st = launch_gemm_bn<128, 1, 16>(ctx, s, p, smem); break;
-    case 6: st = launch_gemm_bn<128, 1, 32>(ctx, s, p, smem); break;
-    case 7: st = launch_gemm_bn<128, 1, 64>(ctx, s, p, smem); break;
-    case 8: st = launch_gemm_bn<64, 2, 0>(ctx, s, p, smem); break;
-    case 9: st = launch_gemm_bn<64, 2, 16>(ctx, s, p, smem); break;
-    case 10: st = launch_gemm_bn<64, 2, 32>(ctx, s, p, smem); break;
-    case 11: st = launch_gemm_bn<64, 2, 64>(ctx, s, p, smem); break;
-    case 12: st = launch_gemm_bn<128, 2, 0>(ctx, s, p, smem); break;
-    case 13: st = launch_gemm_bn<128, 2, 16>(ctx, s, p, smem); break;
-    case 14: st = launch_gemm_bn<128, 2, 32>(ctx, s, p, smem); break;
-    default: st = launch_gemm_bn<128, 2, 64>(ctx, s, p, smem); break;
+    const dim3 grid(std::min(p.num_m_tiles * p.num_n_tiles, ctx->num_sms));
+    if (rt == 16)
+      st = launch_checked<gemm_wide_kernel<16, false>, kWideThreads, 1>(ctx, stream, p, grid, smem, 1);
+    else if (rt != 0)
+      st = launch_checked<gemm_wide_kernel<32, false>, kWideThreads, 1>(ctx, stream, p, grid, smem, 1);
+    else if (p.flags & SB200_EPI_GEGLU)
+      st = launch_checked<gemm_wide_kernel<0, true>, kWideThreads, 1>(ctx, stream, p, grid, smem, 1);
+    else
+      st = launch_checked<gemm_wide_kernel<0, false>, kWideThreads, 1>(ctx, stream, p, grid, smem, 1);
+  } else {
+    const int grid_ctas = p.num_m_tiles * p.num_n_tiles * ctas * (p.sk_ws ? p.sk_splits : 1);
+    // A grid that gives each SM at most one CTA lets that CTA have the whole SM's shared memory (a deeper ring).
+    const int budget = smem_budget(ctx, grid_ctas > ctx->num_sms ? gemm_slots(p.bn, rt) : 1);
+    int stages = (budget - kBarRegion - kAlignSlack) / p.stage_bytes;
+    if (stages > kMaxStages) stages = kMaxStages;
+    if (stages < 2) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
+    p.stages = stages;
+    p.ring_bytes = std::max(stages * p.stage_bytes, acc_tile_bytes(p.bn, rt) + kEpiBytes + kEpiWarps * p.up_buf_bytes);
+    const int smem = kBarRegion + kAlignSlack + p.ring_bytes;
+    if (smem > budget) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
+    pdl_hint() = grid_ctas <= 2 * ctx->num_sms;
+    if (p.bn == 128)
+      st = ctas == 2 ? launch_narrow<128, 2>(ctx, stream, p, rt, smem) : launch_narrow<128, 1>(ctx, stream, p, rt, smem);
+    else
+      st = ctas == 2 ? launch_narrow<64, 2>(ctx, stream, p, rt, smem) : launch_narrow<64, 1>(ctx, stream, p, rt, smem);
   }
   if (st) return st;
   SB200_CUDA_CHECK(cudaGetLastError());
@@ -1168,15 +1066,67 @@ static void decode_bn(int bn_arg, int* bn, int* force_ctas) {
   *bn = bn_arg > 0 ? (bn_arg & 0xFFF) : 0;
 }
 
-static void fill_lora(GemmParams& p, const sb200_lora* lora) {
-  p.lora_up = static_cast<const float*>(lora->up);
-  p.lora_r = lora->r;
-  p.lora_rt = lora->rt;
-  p.lora_group_n = lora->group_n;
-  p.lora_scale = lora->scale;
-  p.lora_scale_dev = lora->scale_dev;
-  p.lora_sample_scale = lora->sample_scale;
-  p.lora_rows_per_sample = lora->rows_per_sample;
+// 2-D bf16 tensor map of `rows` rows of k elements, row stride ld elements, in boxes of box_rows rows x 64 k
+static int tmap_2d(Ctx* ctx, CUtensorMap* out, const void* ptr, int ld, int k, int rows, int box_rows) {
+  const uint64_t dims[2] = {static_cast<uint64_t>(k), static_cast<uint64_t>(rows)};
+  const uint64_t strides[1] = {static_cast<uint64_t>(ld) * 2};
+  const uint32_t box[2] = {kBK, static_cast<uint32_t>(box_rows)};
+  return make_tmap_bf16(ctx, out, ptr, 2, dims, strides, box);
+}
+
+// The part of a GEMM / conv / split-K launch that does not depend on how A is addressed.  The entry point `who` has
+// filled in the problem (M, N, K, flags, kblocks, num_sub, split-K) and the A operand; this validates the epilogue
+// flags and the LoRA, picks the tile (bn_arg as decode_bn reads it), fills in the tile counts and the epilogue
+// pointers, builds the tensor maps of W ([N, K], row stride ldw) and of the LoRA down-projection, and launches.
+static int plan_and_launch(Ctx* ctx, cudaStream_t stream, GemmParams& p, const char* who, const void* w, int ldw,
+                           const void* bias, const void* rowbias, int rows_per_batch, const void* resid, int ldr,
+                           void* out, int ldo, const sb200_lora* lora, int bn_arg) {
+  const int flags = p.flags;
+  const bool geglu = flags & SB200_EPI_GEGLU;
+  const bool has_lora = flags & SB200_EPI_LORA;
+  SB200_REQUIRE(!(geglu && has_lora), "%s: GEGLU and LORA cannot be combined", who);
+  SB200_REQUIRE(!geglu || p.N % 32 == 0, "%s: GEGLU needs N %% 32 == 0", who);
+  SB200_REQUIRE(!(flags & SB200_EPI_BIAS) || bias, "%s: BIAS without bias", who);
+  SB200_REQUIRE(!(flags & SB200_EPI_ROWBIAS) || (rowbias && rows_per_batch > 0), "%s: ROWBIAS args", who);
+  SB200_REQUIRE(!(flags & SB200_EPI_RESID) || (resid && ldr % 8 == 0), "%s: RESID args", who);
+  SB200_REQUIRE(!has_lora || lora, "%s: LORA without sb200_lora", who);
+  if (has_lora) {
+    const int st = check_lora(lora, p.M, p.N);
+    if (st) return st;
+    p.lora_up = static_cast<const float*>(lora->up);
+    p.lora_r = lora->r;
+    p.lora_rt = lora->rt;
+    p.lora_group_n = lora->group_n;
+    p.lora_scale = lora->scale;
+    p.lora_scale_dev = lora->scale_dev;
+    p.lora_sample_scale = lora->sample_scale;
+    p.lora_rows_per_sample = lora->rows_per_sample;
+  }
+  int bn, force_ctas;
+  decode_bn(bn_arg, &bn, &force_ctas);
+  TileChoice tc = pick_tile(p.N, ctx->num_sms, p.kblocks, p.lora_r, p.lora_rt, force_ctas, p.num_sub, flags);
+  if (bn > 0) tc.bn = bn;
+  if (force_ctas) tc.ctas = force_ctas;
+  SB200_REQUIRE(bn_supported(tc.bn), "%s: bn=%d invalid (64, 128 or 256)", who, tc.bn);
+  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(p.N, tc.ctas, p.lora_r, p.lora_rt),
+                "%s: bn=256 needs N %% 256 == 0 and single CTAs, without LoRA of rank 16 or rt 64 (N=%d)", who, p.N);
+  p.Nout = geglu ? p.N / 2 : p.N;
+  p.bn = tc.bn;
+  p.ncols_out = geglu ? tc.bn / 2 : tc.bn;
+  p.num_m_tiles = (p.num_sub + tc.ctas - 1) / tc.ctas;
+  p.num_n_tiles = (p.Nout + p.ncols_out - 1) / p.ncols_out;
+  p.bias = static_cast<const __nv_bfloat16*>(bias);
+  p.rowbias = static_cast<const __nv_bfloat16*>(rowbias);
+  p.rows_per_batch = rows_per_batch;
+  p.resid = static_cast<const __nv_bfloat16*>(resid);
+  p.ldr = ldr;
+  p.out = static_cast<__nv_bfloat16*>(out);
+  p.ldo = ldo;
+  // a CTA's W rows per k-block: half of the tile's in a pair; with GEGLU one box of value rows and one of gate rows
+  int st;
+  if ((st = tmap_2d(ctx, &p.tmB, w, ldw, p.K, p.N, (geglu || tc.ctas == 2) ? tc.bn / 2 : tc.bn))) return st;
+  if (has_lora && (st = tmap_2d(ctx, &p.tmL, lora->down, p.K, p.K, lora->rt, lora->rt / tc.ctas))) return st;
+  return launch_gemm(ctx, stream, p, tc.ctas);
 }
 
 // out[m, n] = sum over s (in order) of ws[s][m][n]; four columns per thread
@@ -1220,34 +1170,22 @@ extern "C" int sb200_gemm_splitk_f32(void* handle, void* stream, const void* x, 
   p.M = M;
   p.N = N;
   p.K = K;
-  p.Nout = N;
   p.kblocks = (K + kBK - 1) / kBK;
   p.kb_split = p.kblocks;
   p.cb_total = p.kblocks;
   p.a_tx = kBM * 128;
   p.num_sub = (M + kBM - 1) / kBM;
-  p.bn = N % 128 == 0 ? 128 : 64;
-  p.ncols_out = p.bn;
-  p.num_m_tiles = p.num_sub;
-  p.num_n_tiles = (N + p.bn - 1) / p.bn;
   p.sk_ws = ws;
   p.sk_kb = SB200_GEMM_SPLITK_KB(M, N, K);
   p.sk_splits = SB200_GEMM_SPLITK_SPLITS(M, N, K);
   int st;
-  {
-    const uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(M)};
-    const uint64_t strides[1] = {static_cast<uint64_t>(ldx) * 2};
-    const uint32_t box[2] = {kBK, kBM};
-    if ((st = make_tmap_bf16(ctx, &p.tmA[0], x, 2, dims, strides, box))) return st;
-  }
-  {
-    const uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(N)};
-    const uint64_t strides[1] = {static_cast<uint64_t>(ldw) * 2};
-    const uint32_t box[2] = {kBK, static_cast<uint32_t>(p.bn)};
-    if ((st = make_tmap_bf16(ctx, &p.tmB, w, 2, dims, strides, box))) return st;
-  }
+  if ((st = tmap_2d(ctx, &p.tmA[0], x, ldx, K, M, kBM))) return st;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if ((st = launch_gemm(ctx, s, p, 1))) return st;
+  // single CTAs on tiles 128 wide where N allows, no epilogue
+  const int bn_arg = (N % 128 == 0 ? 128 : 64) | 0x2000;
+  if ((st = plan_and_launch(ctx, s, p, "gemm_splitk_f32", w, ldw, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr,
+                            bn_arg)))
+    return st;
   const size_t quads = static_cast<size_t>(M) * N / 4;
   SB200_CUDA_CHECK(launch_pdl(splitk_reduce_kernel, dim3(static_cast<unsigned>((quads + 255) / 256)), dim3(256), 0, s,
                               static_cast<const float*>(ws), p.sk_splits, M, N, out, ldo));
@@ -1269,14 +1207,6 @@ extern "C" int sb200_gemm(void* handle, void* stream, const void* x0, int ldx0, 
   if (!split) K0 = K;
   SB200_REQUIRE(!split || (K0 % 64 == 0 && K0 > 0 && K0 < K && ldx1 % 8 == 0),
                 "gemm: split K0=%d must be a multiple of 64 inside (0, K)", K0);
-  const bool geglu = flags & SB200_EPI_GEGLU;
-  const bool has_lora = flags & SB200_EPI_LORA;
-  SB200_REQUIRE(!(geglu && has_lora), "gemm: GEGLU and LORA cannot be combined");
-  SB200_REQUIRE(!geglu || N % 32 == 0, "gemm: GEGLU needs N %% 32 == 0");
-  SB200_REQUIRE(!(flags & SB200_EPI_BIAS) || bias, "gemm: BIAS without bias");
-  SB200_REQUIRE(!(flags & SB200_EPI_ROWBIAS) || (rowbias && rows_per_batch > 0), "gemm: ROWBIAS args");
-  SB200_REQUIRE(!(flags & SB200_EPI_RESID) || (resid && ldr % 8 == 0), "gemm: RESID args");
-  SB200_REQUIRE(!has_lora || lora, "gemm: LORA without sb200_lora");
 
   GemmParams p;
   memset(&p, 0, sizeof(p));
@@ -1284,65 +1214,17 @@ extern "C" int sb200_gemm(void* handle, void* stream, const void* x0, int ldx0, 
   p.N = N;
   p.K = K;
   p.flags = flags;
-  p.Nout = geglu ? N / 2 : N;
   p.kblocks = (K + kBK - 1) / kBK;
   p.a_mode = 0;
   p.kb_split = split ? K0 / kBK : p.kblocks;
   p.cb_total = p.kblocks;
   p.a_tx = kBM * 128;
   p.num_sub = (M + kBM - 1) / kBM;
-  if (has_lora) {
-    int st = check_lora(lora, M, N);
-    if (st) return st;
-    fill_lora(p, lora);
-  }
-  int bn, force_ctas;
-  decode_bn(bn_arg, &bn, &force_ctas);
-  TileChoice tc = pick_tile(N, ctx->num_sms, p.kblocks, p.lora_r, p.lora_rt, force_ctas, p.num_sub, flags);
-  if (bn > 0) tc.bn = bn;
-  if (force_ctas) tc.ctas = force_ctas;
-  SB200_REQUIRE(bn_supported(tc.bn), "gemm: bn=%d invalid (64, 128 or 256)", tc.bn);
-  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(N, tc.ctas, p.lora_r, p.lora_rt),
-                "gemm: bn=256 needs N %% 256 == 0 and single CTAs, without LoRA of rank 16 or rt 64 (N=%d)", N);
-  p.bn = tc.bn;
-  p.ncols_out = geglu ? tc.bn / 2 : tc.bn;
-  p.num_m_tiles = (p.num_sub + tc.ctas - 1) / tc.ctas;
-  p.num_n_tiles = (p.Nout + p.ncols_out - 1) / p.ncols_out;
-  p.bias = static_cast<const __nv_bfloat16*>(bias);
-  p.rowbias = static_cast<const __nv_bfloat16*>(rowbias);
-  p.rows_per_batch = rows_per_batch;
-  p.resid = static_cast<const __nv_bfloat16*>(resid);
-  p.ldr = ldr;
-  p.out = static_cast<__nv_bfloat16*>(out);
-  p.ldo = ldo;
-
   int st;
-  {
-    const uint64_t dims[2] = {static_cast<uint64_t>(K0), static_cast<uint64_t>(M)};
-    const uint64_t strides[1] = {static_cast<uint64_t>(ldx0) * 2};
-    const uint32_t box[2] = {kBK, kBM};
-    if ((st = make_tmap_bf16(ctx, &p.tmA[0], x0, 2, dims, strides, box))) return st;
-  }
-  if (split) {
-    const uint64_t dims[2] = {static_cast<uint64_t>(K - K0), static_cast<uint64_t>(M)};
-    const uint64_t strides[1] = {static_cast<uint64_t>(ldx1) * 2};
-    const uint32_t box[2] = {kBK, kBM};
-    if ((st = make_tmap_bf16(ctx, &p.tmA[1], x1, 2, dims, strides, box))) return st;
-  }
-  {
-    const uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(N)};
-    const uint64_t strides[1] = {static_cast<uint64_t>(ldw) * 2};
-    const int brows = (geglu || tc.ctas == 2) ? tc.bn / 2 : tc.bn;
-    const uint32_t box[2] = {kBK, static_cast<uint32_t>(brows)};
-    if ((st = make_tmap_bf16(ctx, &p.tmB, w, 2, dims, strides, box))) return st;
-  }
-  if (has_lora) {
-    const uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(lora->rt)};
-    const uint64_t strides[1] = {static_cast<uint64_t>(K) * 2};
-    const uint32_t box[2] = {kBK, static_cast<uint32_t>(lora->rt / tc.ctas)};
-    if ((st = make_tmap_bf16(ctx, &p.tmL, lora->down, 2, dims, strides, box))) return st;
-  }
-  return launch_gemm(ctx, static_cast<cudaStream_t>(stream), p, tc.ctas);
+  if ((st = tmap_2d(ctx, &p.tmA[0], x0, ldx0, K0, M, kBM))) return st;
+  if (split && (st = tmap_2d(ctx, &p.tmA[1], x1, ldx1, K - K0, M, kBM))) return st;
+  return plan_and_launch(ctx, static_cast<cudaStream_t>(stream), p, "gemm", w, ldw, bias, rowbias, rows_per_batch,
+                         resid, ldr, out, ldo, lora, bn_arg);
 }
 
 // Patch of output pixels one 128-row sub-tile covers: bw x bh x bb with bw * bh * bb <= 128, chosen to minimise the
@@ -1388,24 +1270,17 @@ extern "C" int sb200_conv3x3(void* handle, void* stream, const void* x0, int ldx
   SB200_REQUIRE(!pad_br || stride == 2, "conv3x3: CONV_PAD_BR needs stride 2");
   flags &= ~SB200_CONV_PAD_BR;
   SB200_REQUIRE(ldx0 % 8 == 0 && ldo % 8 == 0 && (C1 == 0 || ldx1 % 8 == 0), "conv3x3: leading dims");
-  const bool has_lora = flags & SB200_EPI_LORA;
-  SB200_REQUIRE(!has_lora || lora, "conv3x3: LORA without sb200_lora");
-  SB200_REQUIRE(!(flags & SB200_EPI_BIAS) || bias, "conv3x3: BIAS without bias");
-  SB200_REQUIRE(!(flags & SB200_EPI_ROWBIAS) || rowbias, "conv3x3: ROWBIAS without rowbias");
-  SB200_REQUIRE(!(flags & SB200_EPI_RESID) || (resid && ldr % 8 == 0), "conv3x3: RESID args");
   const int H = Hin / stride, W = Win / stride;
   int bw, bh, bb;
   pick_patch(B, H, W, &bw, &bh, &bb);
   const int Cin = C0 + C1;
-  const int M = B * H * W;
 
   GemmParams p;
   memset(&p, 0, sizeof(p));
-  p.M = M;
+  p.M = B * H * W;
   p.N = Cout;
   p.K = 9 * Cin;
   p.flags = flags;
-  p.Nout = Cout;
   p.cb_total = Cin / kBK;
   p.kblocks = 9 * p.cb_total;
   p.a_mode = stride == 1 ? 1 : (pad_br ? 3 : 2);
@@ -1420,31 +1295,6 @@ extern "C" int sb200_conv3x3(void* handle, void* stream, const void* x0, int ldx
   p.tiles_h = (H + bh - 1) / bh;
   p.num_sub = p.tiles_w * p.tiles_h * ((B + bb - 1) / bb);
   p.a_tx = bw * bh * bb * 128;
-  if (has_lora) {
-    int st = check_lora(lora, M, Cout);
-    if (st) return st;
-    fill_lora(p, lora);
-  }
-  int bn, force_ctas;
-  decode_bn(bn_arg, &bn, &force_ctas);
-  TileChoice tc = pick_tile(Cout, ctx->num_sms, p.kblocks, p.lora_r, p.lora_rt, force_ctas, p.num_sub, flags);
-  if (bn > 0) tc.bn = bn;
-  if (force_ctas) tc.ctas = force_ctas;
-  SB200_REQUIRE(bn_supported(tc.bn), "conv3x3: bn=%d invalid (64, 128 or 256)", tc.bn);
-  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(Cout, tc.ctas, p.lora_r, p.lora_rt),
-                "conv3x3: bn=256 needs Cout %% 256 == 0 and single CTAs, without LoRA of rank 16 or rt 64 (Cout=%d)",
-                Cout);
-  p.bn = tc.bn;
-  p.ncols_out = tc.bn;
-  p.num_m_tiles = (p.num_sub + tc.ctas - 1) / tc.ctas;
-  p.num_n_tiles = (Cout + tc.bn - 1) / tc.bn;
-  p.bias = static_cast<const __nv_bfloat16*>(bias);
-  p.rowbias = static_cast<const __nv_bfloat16*>(rowbias);
-  p.rows_per_batch = H * W;
-  p.resid = static_cast<const __nv_bfloat16*>(resid);
-  p.ldr = ldr;
-  p.out = static_cast<__nv_bfloat16*>(out);
-  p.ldo = ldo;
 
   int st;
   const uint32_t box[4] = {kBK, static_cast<uint32_t>(bw), static_cast<uint32_t>(bh),
@@ -1472,17 +1322,7 @@ extern "C" int sb200_conv3x3(void* handle, void* stream, const void* x0, int ldx
         if ((st = make_tmap_bf16(ctx, &p.tmA[ph * 2 + pw], basep, 4, dims, strides, box))) return st;
       }
   }
-  {
-    const uint64_t dims[2] = {static_cast<uint64_t>(p.K), static_cast<uint64_t>(Cout)};
-    const uint64_t strides[1] = {static_cast<uint64_t>(p.K) * 2};
-    const uint32_t wbox[2] = {kBK, static_cast<uint32_t>(tc.bn / tc.ctas)};
-    if ((st = make_tmap_bf16(ctx, &p.tmB, w, 2, dims, strides, wbox))) return st;
-  }
-  if (has_lora) {
-    const uint64_t dims[2] = {static_cast<uint64_t>(p.K), static_cast<uint64_t>(lora->rt)};
-    const uint64_t strides[1] = {static_cast<uint64_t>(p.K) * 2};
-    const uint32_t lbox[2] = {kBK, static_cast<uint32_t>(lora->rt / tc.ctas)};
-    if ((st = make_tmap_bf16(ctx, &p.tmL, lora->down, 2, dims, strides, lbox))) return st;
-  }
-  return launch_gemm(ctx, static_cast<cudaStream_t>(stream), p, tc.ctas);
+  // w: [Cout, 3, 3, Cin], a row of K = 9 * Cin per output channel
+  return plan_and_launch(ctx, static_cast<cudaStream_t>(stream), p, "conv3x3", w, p.K, bias, rowbias, H * W, resid,
+                         ldr, out, ldo, lora, bn_arg);
 }
