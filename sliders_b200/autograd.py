@@ -118,22 +118,22 @@ def _pad_rank(t: torch.Tensor, dim: int, rp: int) -> torch.Tensor:
     return out
 
 
-def _new_tape(unet) -> list:
-    """A tape for `unet._walk`, opened with the snapshot of the active adaptors that `_Grads` reads."""
-    if unet._stack_status() is not None:
+def _new_tape(snap) -> list:
+    """A tape for `unet._walk`, opened with the active adaptors of the forward's snapshot (lora_pack.scan), which
+    `_Grads` reads."""
+    if snap.stack_mults is not None:
         # the backward kernels read one adaptor per leaf; a SliderStack's composite hooks carry several
         raise NotImplementedError("sliders_b200: a gradient through an active SliderStack is not implemented "
                                   "(stacks are for inference)")
     scales = {}
-    for leaf, a in unet._adapted_leaves():
-        s = float(a.multiplier) * float(a.scale)
+    for key, (a, s, trainable) in snap.adaptors.items():
         if s != 0.0:
             if getattr(a, "sample_scales", None) is not None:
                 # the backward kernels (lora_wgrad, lora_rank_update and their conv forms) take one scale per launch
                 raise NotImplementedError("sliders_b200: a gradient through a forward with per-sample slider scales is "
                                           "not implemented (per-sample scales are for inference; set a scalar with "
                                           "set_lora_slider, or run under torch.no_grad())")
-            scales[id(leaf)] = (a, s, bool(a.lora_down.weight.requires_grad))
+            scales[key] = (a, s, trainable)
     return [("scales", scales)]
 
 
@@ -414,7 +414,7 @@ class _TrainCapture(_GraphInputs):
     of all adaptor weights are static buffers.  The forward reads the slider factor from the device scalar the
     inference graphs use; the backward bakes it in, so the factor is part of the cache key."""
 
-    def __init__(self, unet, sample, t, ehs, added, out_dtype, params, keys, need_ehs=False):
+    def __init__(self, unet, sample, t, ehs, added, out_dtype, params, keys, snap, need_ehs=False):
         super().__init__(sample, t, ehs, added)
         self.need_ehs = need_ehs
         self.keys = keys
@@ -424,20 +424,16 @@ class _TrainCapture(_GraphInputs):
         stream = torch.cuda.Stream(device=sample.device)
         stream.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(stream):  # warm-up: weight / LoRA packing caches, transposed weights, TMA descriptors
-            tape = _new_tape(unet)
-            out = unet._walk(self.x, self.t, self.ehs, self.added, out_dtype, tape)
+            tape = _new_tape(snap)
+            out = unet._walk(self.x, self.t, self.ehs, self.added, out_dtype, tape, snap)
             backward(unet, tape, torch.zeros_like(out), need_ehs)
             del tape
         torch.cuda.current_stream().wait_stream(stream)
         torch.cuda.synchronize()
         self.gf = torch.cuda.CUDAGraph()
-        self.tape = _new_tape(unet)
-        unet._capturing = True
-        try:
-            with torch.cuda.graph(self.gf):
-                self.out = unet._walk(self.x, self.t, self.ehs, self.added, out_dtype, self.tape)
-        finally:
-            unet._capturing = False
+        self.tape = _new_tape(snap)
+        with torch.cuda.graph(self.gf):
+            self.out = unet._walk(self.x, self.t, self.ehs, self.added, out_dtype, self.tape, snap, capture=True)
         self.d_out = torch.zeros_like(self.out)
         self.unet = unet
         self.bwd = {}  # dead leading samples -> (graph, flat fp32 gradient of every adaptor weight, d_ehs or None)
@@ -464,8 +460,8 @@ class _TrainCapture(_GraphInputs):
             flat = torch.cat(pieces) if pieces else None
         self.bwd[dead] = (graph, flat, by_param.get("ehs"))
 
-    def run_forward(self, unet, x, t, ehs, added):
-        self.load(unet, x, t, ehs, added)
+    def run_forward(self, unet, x, t, ehs, added, snap):
+        self.load(unet, x, t, ehs, added, snap)
         self.gf.replay()
         self.pending = True
         return self.out.clone()
@@ -495,12 +491,12 @@ class _TrainCapture(_GraphInputs):
         return grads, d_ehs
 
 
-def _capture_for(unet, sample, t, ehs, added, out_dtype, params, keys, need_ehs=False):
+def _capture_for(unet, sample, t, ehs, added, out_dtype, params, keys, snap, need_ehs=False):
     """Cached _TrainCapture for this call signature, or None when graphs are off / the signature cannot be captured
     (adaptors with different factors, or a second forward before the first one's backward)."""
     if not getattr(unet, "use_cuda_graph", False):
         return None
-    sig, common = unet._lora_signature()
+    sig, common = snap.signature, snap.common
     if common is None and any(sig[0]):
         return None
     key = (("train",) + _GraphInputs.key(sample, ehs, added, out_dtype)
@@ -510,7 +506,7 @@ def _capture_for(unet, sample, t, ehs, added, out_dtype, params, keys, need_ehs=
     if cap is None:
         while len(cache) >= getattr(unet, "train_graph_max", 2):  # each capture pins its activations (19 GB at SDXL)
             cache.pop(next(iter(cache)))
-        cap = _TrainCapture(unet, sample, t, ehs, added, out_dtype, params, keys, need_ehs)
+        cap = _TrainCapture(unet, sample, t, ehs, added, out_dtype, params, keys, snap, need_ehs)
         cache[key] = cap
     if cap.pending and cap.pending_token is not None and cap.pending_token() is None:
         # the autograd node of the forward that was never back-propagated is gone (exception, loss only logged, skipped
@@ -538,19 +534,19 @@ class _Token:
 class _UNetFunction(torch.autograd.Function):
     @staticmethod
     def forward(fctx, unet, call, ehs_in, *params):
-        sample, t, added, out_dtype, keys, need_ehs = call
+        sample, t, added, out_dtype, keys, need_ehs, snap = call
         ehs = ehs_in.detach().to(device=sample.device, dtype=BF16).contiguous()
         fctx.unet, fctx.keys, fctx.need_ehs = unet, keys, need_ehs
         fctx.ehs_meta = (tuple(ehs_in.shape), ehs_in.dtype, ehs_in.device)
         fctx.meta = [(tuple(p.shape), p.dtype) for p in params]
-        fctx.cap = _capture_for(unet, sample, t, ehs, added, out_dtype, params, keys, need_ehs)
+        fctx.cap = _capture_for(unet, sample, t, ehs, added, out_dtype, params, keys, snap, need_ehs)
         if fctx.cap is not None:
             fctx.tape = True
             fctx.token = _Token()
             fctx.cap.pending_token = weakref.ref(fctx.token)
-            return fctx.cap.run_forward(unet, sample, t, ehs, added)
-        fctx.tape = _new_tape(unet)
-        return unet._walk(sample, t, ehs, added, out_dtype, fctx.tape)
+            return fctx.cap.run_forward(unet, sample, t, ehs, added, snap)
+        fctx.tape = _new_tape(snap)
+        return unet._walk(sample, t, ehs, added, out_dtype, fctx.tape, snap)
 
     @staticmethod
     def backward(fctx, d_out):
@@ -592,19 +588,19 @@ def _ehs_grad(fctx, d_ctx: Optional[torch.Tensor], dead: int) -> Optional[torch.
 
 
 
-def trainable_lora_params(unet) -> List[torch.Tensor]:
+def trainable_lora_params(snap) -> List[torch.Tensor]:
     ps = []
-    for leaf, a in unet._adapted_leaves():
-        if float(a.multiplier) * float(a.scale) != 0.0 and a.lora_down.weight.requires_grad:
+    for a, s, trainable in snap.adaptors.values():
+        if s != 0.0 and trainable:
             ps += [a.lora_down.weight, a.lora_up.weight]
     return ps
 
 
-def apply(unet, sample, t, ehs, added, out_dtype, need_ehs: bool = False):
+def apply(unet, sample, t, ehs, added, out_dtype, snap, need_ehs: bool = False):
     """ehs: encoder_hidden_states as the caller passed it (any float dtype); with `need_ehs` it is an autograd input
-    and its gradient comes back in its own dtype, shape and device."""
-    params = trainable_lora_params(unet)
+    and its gradient comes back in its own dtype, shape and device.  `snap`: the forward's lora_pack.scan."""
+    params = trainable_lora_params(snap)
     keys = [id(p) for p in params]  # the backward files gradients under id(adaptor parameter)
     if not need_ehs:
         ehs = ehs.detach()
-    return _UNetFunction.apply(unet, (sample, t, added, out_dtype, keys, need_ehs), ehs, *params)
+    return _UNetFunction.apply(unet, (sample, t, added, out_dtype, keys, need_ehs, snap), ehs, *params)

@@ -17,11 +17,12 @@ from __future__ import annotations
 
 import math
 import os
-import weakref
 from typing import Dict, List, Literal, Optional, Sequence, Union
 
 import torch
 import torch.nn as nn
+
+from .lora_pack import adapted_leaves
 
 UNET_TARGET_REPLACE_MODULE_TRANSFORMER = ["Attention"]
 UNET_TARGET_REPLACE_MODULE_CONV = ["ResnetBlock2D", "Downsample2D", "Upsample2D", "DownBlock2D", "UpBlock2D"]
@@ -32,8 +33,6 @@ DEFAULT_TARGET_REPLACE = UNET_TARGET_REPLACE_MODULE_TRANSFORMER
 TRAINING_METHODS = Literal["noxattn", "innoxattn", "selfattn", "xattn", "full", "xattn-strict",
                            "noxattn-hspace", "noxattn-hspace-last"]
 _LEAF_CLASS_NAMES = ("Linear", "Conv2d", "LoRACompatibleLinear", "LoRACompatibleConv")
-# networks inside `with network:` with per-sample slider values: while it is empty the UNet skips looking for them
-PER_SAMPLE_NETWORKS: "weakref.WeakSet" = weakref.WeakSet()
 
 
 class LoRAModule(nn.Module):
@@ -195,18 +194,12 @@ class LoRANetwork(nn.Module):
             for lora in self.unet_loras:
                 lora.multiplier = 1.0 if on else 0.0
                 lora.sample_scales = self.lora_scale if on else None
-            if on:
-                PER_SAMPLE_NETWORKS.add(self)
-            else:
-                PER_SAMPLE_NETWORKS.discard(self)
             return
-        PER_SAMPLE_NETWORKS.discard(self)
         for lora in self.unet_loras:
             lora.multiplier = 1.0 * self.lora_scale
             lora.sample_scales = None
 
     def __exit__(self, exc_type, exc_value, tb):
-        PER_SAMPLE_NETWORKS.discard(self)
         for lora in self.unet_loras:
             lora.multiplier = 0
             lora.sample_scales = None
@@ -273,11 +266,6 @@ class SliderHook:
             "deltas are fused into the wgmma GEMM/conv kernels (UNet2DConditionModel.forward); there is no eager path.")
 
 
-def _has_adaptor(leaf: nn.Module) -> bool:
-    owner = getattr(leaf.__dict__.get("forward"), "__self__", None)
-    return owner is not None and (hasattr(owner, "lora_down") or hasattr(owner, "slider_entries"))
-
-
 class SliderStack(nn.Module):
     """Several sliders composed on one UNet, each at its own strength (an age slider at 2 and a smile slider at -1).
 
@@ -305,7 +293,7 @@ class SliderStack(nn.Module):
                                       "the fused kernels' LoRA slot")
         if unet.__dict__.get("_slider_stack") is not None:
             raise RuntimeError("sliders_b200: this UNet already carries a SliderStack; put every slider in one stack")
-        if any(_has_adaptor(m) for m in unet.modules()):
+        if adapted_leaves(unet):
             raise RuntimeError("sliders_b200: a SliderStack cannot be built on a UNet that already carries a "
                                "LoRANetwork; build every slider through the stack")
         sliders = []

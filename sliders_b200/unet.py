@@ -24,9 +24,11 @@ from typing import Dict, List, Optional, Tuple
 import torch
 import torch.nn as nn
 
-from . import lora as _lora_mod
+from . import lora_pack as lp
 from . import ops
-from .ops import BF16, Lora
+# re-exported for code that imports the LoRA discovery and composite-packing helpers from the UNet module
+from .lora_pack import _StackArena, _fill_composite, adaptor_of as _adaptor_of, hook_of as _hook_of  # noqa: F401
+from .ops import BF16
 
 
 # --------------------------------------------------------------------------------------------------
@@ -225,110 +227,6 @@ class UNet2DConditionOutput(SimpleNamespace):
     """`.sample` holder, like diffusers' BaseOutput (train_util.py:163)."""
 
 
-# --------------------------------------------------------------------------------------------------
-# LoRA discovery: both the reference lora.py and sliders_b200.lora replace `leaf.forward` by a bound method
-# of the adaptor module (lora.py:103-106), which is how the engine finds the adaptor of a leaf.
-# --------------------------------------------------------------------------------------------------
-def _adaptor_of(leaf: nn.Module):
-    fwd = leaf.__dict__.get("forward")
-    owner = getattr(fwd, "__self__", None)
-    if owner is not None and hasattr(owner, "lora_down") and hasattr(owner, "lora_up"):
-        inner = getattr(getattr(owner, "org_forward", None), "__self__", None)
-        if inner is not None and hasattr(inner, "slider_entries"):
-            raise RuntimeError(f"{getattr(owner, 'lora_name', 'leaf')}: a LoRANetwork was applied on top of a "
-                               "SliderStack; the stack's composite hook owns this leaf, so add the slider to the stack")
-        if inner is not None and hasattr(inner, "lora_down"):
-            # the reference chains `org_forward`, so two networks on one UNet both apply there; the fused kernels carry
-            # one adaptor per leaf — refuse loudly instead of silently dropping the first network
-            raise RuntimeError(f"{getattr(owner, 'lora_name', 'leaf')}: a second LoRANetwork was applied to a UNet that "
-                               "already carries one; merge the sliders' weights or build the second network on another "
-                               "UNet2DConditionModel (parameters can be shared with load_state_dict(assign=True))")
-        return owner
-    return None
-
-
-_UNSET = object()
-
-
-def _hook_of(leaf: nn.Module):
-    """The composite hook a SliderStack installed on `leaf` (sliders_b200.lora.SliderHook), or None."""
-    owner = getattr(leaf.__dict__.get("forward"), "__self__", None)
-    return owner if owner is not None and hasattr(owner, "slider_entries") else None
-
-
-def _fill_composite(down: torch.Tensor, raw: torch.Tensor, leaves, hooks, offsets, rp: int) -> None:
-    """Writes the sliders of one fused call into zeroed packs: leaf gi's slider i takes down rows
-    [gi * rp + o_i, + r) and raw up columns [o_i, o_i + r) of the leaf's output rows, with its alpha / r (the conv rank
-    clamp of lora.py:78 included) folded in; r is the adaptor's own rank, so a leaf a slider does not adapt, and the
-    columns past a clamped rank, keep zeros."""
-    n0 = 0
-    for gi, (leaf, h) in enumerate(zip(leaves, hooks)):
-        n1 = n0 + leaf.weight.shape[0]
-        for i, a in (h.slider_entries if h is not None else ()):
-            d = a.lora_down.weight.detach()
-            if d.dim() == 4:
-                d = d.permute(0, 2, 3, 1)
-            rr = d.shape[0]
-            c0 = offsets[i]
-            down[gi * rp + c0: gi * rp + c0 + rr].copy_(d.reshape(rr, -1))
-            u = a.lora_up.weight.detach().reshape(leaf.weight.shape[0], -1)
-            raw[n0:n1, c0:c0 + rr].copy_(u.float() * float(a.scale))
-        n0 = n1
-
-
-class _LoraPack:
-    """Packed (down [rt,K], up [N,r]) buffers of one fused call site; repacked only when a parameter changes.  A
-    composite pack (SliderStack) also keeps `raw`: the sliders' up columns with alpha / r folded in, before the runtime
-    multipliers; `up` is then the effective pack sb200_lora_compose writes."""
-
-    def __init__(self):
-        self.key = None
-        self.down = None
-        self.up = None
-        self.raw = None
-
-
-class _StackArena:
-    """Device state of a UNet's SliderStack.  Every composite pack's raw and effective up columns are row slices of one
-    fp32 arena each, so a single sb200_lora_compose launch per forward applies the per-column multipliers `mult` (one
-    fp32 value per slot column: slider i's multiplier on its columns [o_i, o_i + r_i), 0 on padding)."""
-
-    def __init__(self, stack, device):
-        self.stack = stack
-        self.rp = ops.lora_slots(stack.total_rank)[0]
-        self.mult = torch.zeros(self.rp, device=device, dtype=torch.float32)
-        self.packs: List[_LoraPack] = []
-        self.raw = None
-        self.eff = None
-        self.dirty = False
-
-    def load(self, mults) -> None:
-        """Writes the multipliers into `mult` with one fill per slider: kernel launches with the value as an argument, so
-        the host never waits for the stream (a copy from pageable host memory would)."""
-        for o, r, m in zip(self.stack.offsets, self.stack.ranks, mults):
-            self.mult[o:o + r].fill_(float(m))
-
-    def settle(self) -> bool:
-        """Moves packs built since the last call into a new arena; True when packs that a captured graph may read
-        moved (there was an arena before)."""
-        if not self.dirty:
-            return False
-        moved = self.raw is not None
-        rows = sum(p.raw.shape[0] for p in self.packs)
-        dev = self.packs[0].raw.device
-        raw = torch.empty((rows, self.rp), device=dev, dtype=torch.float32)
-        eff = torch.empty((rows, self.rp), device=dev, dtype=torch.float32)
-        n0 = 0
-        for p in self.packs:
-            n1 = n0 + p.raw.shape[0]
-            raw[n0:n1].copy_(p.raw)
-            eff[n0:n1].copy_(p.up)
-            p.raw, p.up = raw[n0:n1], eff[n0:n1]
-            n0 = n1
-        self.raw, self.eff, self.dirty = raw, eff, False
-        return moved
-
-
 class UNet2DConditionModel(nn.Module):
     """Drop-in for the diffusers model at the reference call sites (see module docstring)."""
 
@@ -378,16 +276,8 @@ class UNet2DConditionModel(nn.Module):
         self.conv_out = nn.Conv2d(boc[0], c.out_channels, 3, padding=1)
         # engine state (not part of the state dict)
         self._packed: Dict[int, torch.Tensor] = {}
-        self._lora_packs: Dict[tuple, _LoraPack] = {}
+        self._packer = lp.LoraPacker(self._drop_graphs)
         self._graphs: Dict[tuple, "_CapturedForward"] = {}
-        self._slider_scale_dev: Optional[torch.Tensor] = None
-        # per-sample slider values (LoRANetwork.set_lora_slider with a sequence): one fp32 device vector per (batch
-        # size, adaptor factor), entry b = value[b % n] * factor; `_sample_values` holds the walk's values
-        self._sample_vecs: Dict[tuple, torch.Tensor] = {}
-        self._sample_values: Optional[tuple] = None
-        self._sample_filled: set = set()
-        self._stack_arena: Optional[_StackArena] = None
-        self._stack_mults: Optional[List[float]] = None  # per-slider multipliers of the current walk; None: stack off
         self.use_cuda_graph = False
 
     # ---- diffusers-API shims used by the reference trainers (train_lora_xl.py:78-82) ----------------
@@ -405,22 +295,21 @@ class UNet2DConditionModel(nn.Module):
     def _apply(self, fn, *a, **k):
         out = super()._apply(fn, *a, **k)
         self.__dict__.pop("_adapted_cache", None)
-        self.__dict__.pop("_leaf_by_id", None)
         self._packed.clear()
-        self._lora_packs.clear()
-        self._graphs.clear()
-        self.__dict__.pop("_train_graphs", None)
-        self._slider_scale_dev = None
-        self._sample_vecs.clear()
-        self._stack_arena = None
+        self._packer.reset()
+        self._drop_graphs()
         return out
 
     def load_state_dict(self, *a, **k):
         out = super().load_state_dict(*a, **k)
         self._packed.clear()
+        self._drop_graphs()
+        return out
+
+    def _drop_graphs(self) -> None:
+        """Forgets every captured CUDA graph, inference and training: they read buffers that are being replaced."""
         self._graphs.clear()
         self.__dict__.pop("_train_graphs", None)
-        return out
 
     # ---- frozen-weight packing -----------------------------------------------------------------------
     def _w(self, leaf: nn.Module) -> torch.Tensor:
@@ -455,202 +344,9 @@ class UNet2DConditionModel(nn.Module):
             self._packed[key] = w
         return w
 
-    # ---- LoRA packing --------------------------------------------------------------------------------
-    def _lora(self, leaves: List[nn.Module]) -> Optional[Lora]:
-        """sb200_lora for one fused call over `leaves` (all sharing the same input), or None when no leaf is
-        adapted or every multiplier is 0 (lora.py:256-258: outside `with network:` the delta is exactly 0)."""
-        if "_slider_stack" in self.__dict__:
-            return self._lora_composite(leaves)
-        adaptors = [_adaptor_of(l) for l in leaves]
-        if all(a is None for a in adaptors):
-            return None
-        scales = [float(a.multiplier) * float(a.scale) if a is not None else 0.0 for a in adaptors]
-        if all(s == 0.0 for s in scales):
-            return None
-        r, rt = ops.lora_slots(max(int(a.lora_dim) for a in adaptors if a is not None), len(leaves))
-        nz = [s for s in scales if s != 0.0]
-        common = nz[0] if all(abs(s - nz[0]) < 1e-12 for s in nz) else None
-        if self._bake_scales:
-            # graph mode with adaptor factors that differ BETWEEN call sites (per-module multipliers, a conv rank clamp
-            # changing alpha / r): the replayed graph has one device-side factor, so here every factor is folded into
-            # the packed up-weights instead and the kernels run with scale 1
-            common = None
-        key_leaves = tuple(id(l) for l in leaves)
-        pack = self._lora_packs.setdefault(key_leaves, _LoraPack())
-        ver = tuple((a.lora_down.weight.data_ptr(), a.lora_down.weight._version, a.lora_up.weight.data_ptr(),
-                     a.lora_up.weight._version) if a is not None else None for a in adaptors)
-        ver = (ver, None if common is not None else tuple(scales))
-        group_n = leaves[0].weight.shape[0]
-        if pack.key != ver:
-            dev = leaves[0].weight.device
-            K = leaves[0].weight[0].numel()
-            N = sum(l.weight.shape[0] for l in leaves)
-            if pack.down is None or pack.down.shape != (rt, K) or pack.up.shape != (N, r):
-                # adaptor gi takes down rows [gi * r, +r) and up columns [0, r) with r the slot width (ops.lora_slots);
-                # the rows and columns beyond its own rank stay zero
-                if pack.down is not None:  # another slot width: captured graphs hold the old buffers
-                    if self._capturing:
-                        raise RuntimeError("sliders_b200: the LoRA slot width changed while a CUDA graph was captured")
-                    self._graphs.clear()
-                    self.__dict__.pop("_train_graphs", None)
-                pack.down = torch.zeros((rt, K), device=dev, dtype=BF16)
-                pack.up = torch.zeros((N, r), device=dev, dtype=torch.float32)  # sb200_lora.up is fp32
-            else:
-                pack.down.zero_()
-                pack.up.zero_()
-            n0 = 0
-            for gi, (leaf, a) in enumerate(zip(leaves, adaptors)):
-                n1 = n0 + leaf.weight.shape[0]
-                if a is not None:
-                    d = a.lora_down.weight.detach()
-                    if d.dim() == 4:
-                        d = d.permute(0, 2, 3, 1)
-                    rr = d.shape[0]
-                    pack.down[gi * r: gi * r + rr].copy_(d.reshape(rr, -1))
-                    u = a.lora_up.weight.detach().reshape(leaf.weight.shape[0], -1)
-                    if common is None:
-                        u = u.float() * scales[gi]
-                    pack.up[n0:n1, :rr].copy_(u)
-                n0 = n1
-            pack.key = ver
-        if self._sample_values is not None:
-            # per-sample values: the factor common to the call site (1 when folded into `up`) goes into the vector, so
-            # a constant vector reproduces the scalar path's fp32 scale exactly
-            vec = self._sample_vec(common if common is not None else 1.0)
-            return Lora(pack.down, pack.up, r, group_n, 1.0, sample_scale=vec)
-        if self._slider_scale_dev is None:
-            self._slider_scale_dev = torch.ones(1, device=leaves[0].weight.device, dtype=torch.float32)
-        if self._capturing and common is not None:
-            # graph mode: the common scale is read from device memory at replay time
-            return Lora(pack.down, pack.up, r, group_n, 1.0, self._slider_scale_dev)
-        return Lora(pack.down, pack.up, r, group_n, common if common is not None else 1.0)
-
-    _capturing = False
-    _bake_scales = False
-
-    # ---- per-sample slider values ------------------------------------------------------------------------------------
-    def _sample_scan(self, B: int) -> Optional[tuple]:
-        """The per-sample slider values the active adaptors carry (`LoRANetwork.set_lora_slider` with a sequence), or
-        None.  B, the batch of the call, must be a multiple of their count."""
-        values = None
-        if not _lora_mod.PER_SAMPLE_NETWORKS:
-            return None
-        for _, a in self._adapted_leaves():
-            v = getattr(a, "sample_scales", None)
-            if v is None or float(a.multiplier) * float(a.scale) == 0.0:
-                continue
-            if values is not None and v != values:
-                raise ValueError("sliders_b200: active adaptors carry different per-sample slider values")
-            values = v
-        if values is not None and B % len(values) != 0:
-            raise ValueError(f"sliders_b200: a batch of {B} is not a multiple of the {len(values)} per-sample slider "
-                             "values")
-        return values
-
-    def _sample_vec(self, factor: float) -> torch.Tensor:
-        """The device vector of the current walk's batch for adaptor factor `factor`, filled once per walk (a captured
-        graph gets its values from _GraphInputs.load instead)."""
-        B = self.__dict__["_sample_batch"]
-        key = (B, factor)
-        vec = self._sample_vecs.get(key)
-        if vec is None:
-            if self._capturing:
-                raise RuntimeError("sliders_b200: a per-sample scale vector was first needed while a CUDA graph was "
-                                   "captured")
-            vec = torch.empty(B, device=self.conv_in.weight.device, dtype=torch.float32)
-            self._sample_vecs[key] = vec
-        if not self._capturing and key not in self._sample_filled:
-            self._fill_sample_vec(vec, factor, self._sample_values)
-            self._sample_filled.add(key)
-        return vec
-
-    @staticmethod
-    def _fill_sample_vec(vec: torch.Tensor, factor: float, values: tuple) -> None:
-        """vec[b] = fp32(values[b % n] * factor), with one fill per run of equal entries: kernel launches with the value
-        as an argument, so the host never waits for the stream (a copy from pageable host memory would)."""
-        n = len(values)
-        entries = [values[b % n] * factor for b in range(vec.numel())]
-        b0 = 0
-        for b in range(1, len(entries) + 1):
-            if b == len(entries) or entries[b] != entries[b0]:
-                vec[b0:b].fill_(entries[b0])
-                b0 = b
-
-    # ---- SliderStack: composite LoRA packs -------------------------------------------------------------------------
-    def _stack_status(self) -> Optional[List[float]]:
-        """The stack's per-slider multipliers, or None when the UNet has no stack or every slider is at 0.  Read once
-        per `forward` (the snapshot below); outside a forward each call reads the sliders again."""
-        snap = self.__dict__.get("_stack_snapshot", _UNSET)
-        return self._stack_scan() if snap is _UNSET else snap
-
-    def _stack_scan(self) -> Optional[List[float]]:
-        stack = self.__dict__.get("_slider_stack")
-        if stack is None:
-            return None
-        if self._adapted_leaves():
-            raise RuntimeError("sliders_b200: a LoRANetwork was applied to a UNet that carries a SliderStack; add the "
-                               "slider to the stack instead")
-        mults = stack.slider_multipliers()
-        if all(m == 0.0 for m in mults):
-            return None
-        if self._stack_arena is None:
-            self._stack_arena = _StackArena(stack, self.conv_in.weight.device)
-        return mults
-
-    def _stack_begin(self, compose: bool = True) -> None:
-        """Start of a walk (or of a graph replay, compose=False): the current multipliers go to the device vector and,
-        once the packs are in their arena, one sb200_lora_compose writes every effective up pack."""
-        mults = self._stack_status()
-        self._stack_mults = mults
-        if mults is None:
-            return
-        arena = self._stack_arena
-        if not self._capturing:  # replays get the vector from _GraphInputs.load
-            arena.load(mults)
-        if compose and arena.raw is not None:
-            ops.lora_compose(arena.raw, arena.mult, out=arena.eff)
-
-    def _stack_end(self) -> None:
-        arena = self._stack_arena
-        if arena is not None and not self._capturing and arena.settle():
-            # graphs captured before hold the packs' old buffers
-            self._graphs.clear()
-
-    def _lora_composite(self, leaves: List[nn.Module]) -> Optional[Lora]:
-        """sb200_lora of one fused call on a UNet with a SliderStack: slider i's rows / columns [o_i, o_i + r_i) of every
-        leaf's slot, alpha / r folded into the raw up pack, the runtime multipliers applied by sb200_lora_compose; the
-        kernels run with scale 1.  None when no leaf is hooked or every slider is at 0."""
-        hooks = [_hook_of(l) for l in leaves]
-        if self._stack_mults is None or all(h is None for h in hooks):
-            return None
-        arena = self._stack_arena
-        rp = arena.rp
-        _, rt = ops.lora_slots(rp, len(leaves))
-        pack = self._lora_packs.setdefault(tuple(id(l) for l in leaves), _LoraPack())
-        ver = tuple(tuple((i, a.lora_down.weight.data_ptr(), a.lora_down.weight._version, a.lora_up.weight.data_ptr(),
-                           a.lora_up.weight._version) for i, a in h.slider_entries) if h is not None else None
-                    for h in hooks)
-        if pack.key != ver:
-            if pack.raw is None:
-                if self._capturing:
-                    raise RuntimeError("sliders_b200: a SliderStack call site was first met while a CUDA graph was "
-                                       "captured")
-                dev = leaves[0].weight.device
-                K = leaves[0].weight[0].numel()
-                N = sum(l.weight.shape[0] for l in leaves)
-                pack.down = torch.zeros((rt, K), device=dev, dtype=BF16)
-                pack.raw = torch.zeros((N, rp), device=dev, dtype=torch.float32)
-                pack.up = torch.empty((N, rp), device=dev, dtype=torch.float32)
-                arena.packs.append(pack)
-                arena.dirty = True
-            else:
-                pack.down.zero_()
-                pack.raw.zero_()
-            _fill_composite(pack.down, pack.raw, leaves, hooks, arena.stack.offsets, rp)
-            pack.key = ver
-            # the walk's compose has run already: compose this pack now
-            ops.lora_compose(pack.raw, arena.mult, out=pack.up)
-        return Lora(pack.down, pack.up, rp, leaves[0].weight.shape[0], 1.0)
+    def _lora(self, leaves: List[nn.Module]) -> Optional[ops.Lora]:
+        """The `ops.Lora` of one fused call over `leaves`, or None when it runs none (lora_pack.LoraPacker.lora)."""
+        return self._packer.lora(leaves)
 
     # ---- forward pieces ------------------------------------------------------------------------------
     # One walk serves inference and training.  `tape` is None for inference; for training it is a list to which every
@@ -709,23 +405,16 @@ class UNet2DConditionModel(nn.Module):
             self._packed["kvplan"] = plan
         return plan
 
-    def _cross_kv_adapted(self) -> bool:
-        """True when an active adaptor sits on a to_k / to_v of attn2 (train methods xattn / full)."""
-        stack_on = self._stack_status() is not None
-        for _, _, mods in self._kv_plan().values():
-            for a in mods:
-                for leaf in (a.to_k, a.to_v):
-                    if stack_on and _hook_of(leaf) is not None:
-                        return True  # every hooked leaf runs its composite pack while any slider is on
-                    ad = _adaptor_of(leaf)
-                    if ad is not None and float(ad.multiplier) * float(ad.scale) != 0.0:
-                        return True
-        return False
+    def _cross_kv_adapted(self, snap: Optional[lp.Snapshot] = None) -> bool:
+        """True when an active adaptor of `snap` (or of a fresh scan) sits on attn2's to_k / to_v (xattn / full)."""
+        snap = snap if snap is not None else lp.scan(self, None)
+        return any(snap.active(leaf) for _, _, mods in self._kv_plan().values() for a in mods
+                   for leaf in (a.to_k, a.to_v))
 
-    def _cross_kv(self, ctx):
+    def _cross_kv(self, ctx, snap: lp.Snapshot):
         """{C: (kv_all [B*77, n_blocks*2C], offsets)} or None when attn2's to_k / to_v carry active adaptors: those
         blocks keep the per-block fused path with its own LoRA stack."""
-        if self._cross_kv_adapted():
+        if self._cross_kv_adapted(snap):
             return None
         return {C_: (ops.gemm(ctx, w), offs) for C_, (w, offs, _) in self._kv_plan().items()}
 
@@ -815,31 +504,26 @@ class UNet2DConditionModel(nn.Module):
             emb = ops.small_linear(a, self._w(ae.linear_2), self._b(ae.linear_2), resid=emb, act_out=2)
         return emb
 
-    def _walk(self, sample, timesteps_f32, ehs, added_cond_kwargs, out_dtype, tape=None):
-        """The UNet forward.  With a `tape` (a list) it also records, in order, what the backward reads: ("ctx", tokens
-        of encoder_hidden_states), then one ("res" | "tr" | "skip" | "down" | "up" | "out", record) per block."""
+    def _walk(self, sample, timesteps_f32, ehs, added_cond_kwargs, out_dtype, tape=None, snap=None, capture=False,
+              bake=False):
+        """The UNet forward with the adaptors of `snap` (lora_pack.scan, taken here when None) and the LoRA packer's
+        graph modes `capture` / `bake`.  With a `tape` (a list) it also records, in order, what the backward reads:
+        ("ctx", tokens of encoder_hidden_states), then one ("res" | "tr" | "skip" | "down" | "up" | "out", record) per
+        block."""
         def record(kind, rec):
             if tape is not None:
                 tape.append((kind, rec))
 
         B = sample.shape[0]
-        self._sample_values = self._sample_scan(B)
-        self.__dict__["_sample_batch"] = B
-        self._sample_filled = set()
-        try:
-            return self._walk_body(sample, timesteps_f32, ehs, added_cond_kwargs, out_dtype, tape, record, B)
-        finally:
-            self._sample_values = None
-
-    def _walk_body(self, sample, timesteps_f32, ehs, added_cond_kwargs, out_dtype, tape, record, B):
-        if "_slider_stack" in self.__dict__:
-            if tape is not None and self._stack_status() is not None:
-                raise NotImplementedError("sliders_b200: a gradient through an active SliderStack is not implemented "
-                                          "(stacks are for inference)")
-            self._stack_begin()
+        if snap is None:
+            snap = lp.scan(self, B)
+        if tape is not None and snap.stack_mults is not None:
+            raise NotImplementedError("sliders_b200: a gradient through an active SliderStack is not implemented "
+                                      "(stacks are for inference)")
+        self._packer.begin(snap, self.conv_in.weight.device, capture, bake)
         Sctx = ehs.shape[1]
         ctx = ehs.reshape(B * Sctx, ehs.shape[-1])
-        kv_all = self._cross_kv(ctx)
+        kv_all = self._cross_kv(ctx, snap)
         emb = self._embeddings(timesteps_f32, B, added_cond_kwargs)
         h = ops.conv_in(sample, self._w(self.conv_in), self._b(self.conv_in))
         record("ctx", Sctx)
@@ -878,38 +562,29 @@ class UNet2DConditionModel(nn.Module):
         if tape is not None:
             tape.append(("out", (h, ops.gn_stats(ws, B, gn.num_groups))))
         out = ops.conv_out(hn, self._w(self.conv_out), self._b(self.conv_out), out_dtype=out_dtype)
-        if "_slider_stack" in self.__dict__:
-            self._stack_end()
+        self._packer.end()
         return out
 
     # ---- public forward --------------------------------------------------------------------------------
     def forward(self, sample, timestep, encoder_hidden_states=None, added_cond_kwargs=None,
                 cross_attention_kwargs=None, return_dict: bool = True, **unused):
-        if "_slider_stack" not in self.__dict__:
-            return self._forward(sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict)
-        # the sliders' multipliers are read once per forward: the graph signature, the graph inputs, the walk and the
+        # the adaptors are read once per forward: the graph signature, the graph inputs, the walk and the
         # cross-attention K / V decision all see this snapshot
-        self.__dict__["_stack_snapshot"] = self._stack_scan()
-        try:
-            return self._forward(sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict)
-        finally:
-            self.__dict__.pop("_stack_snapshot", None)
-
-    def _forward(self, sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict):
+        snap = lp.scan(self, sample.shape[0])
         ehs_grad = (torch.is_grad_enabled() and torch.is_tensor(encoder_hidden_states)
                     and encoder_hidden_states.requires_grad)
-        if torch.is_grad_enabled() and (self._needs_grad() or ehs_grad):
-            if self._stack_status() is not None:
+        if torch.is_grad_enabled() and (snap.needs_grad() or ehs_grad):
+            if snap.stack_mults is not None:
                 raise NotImplementedError("sliders_b200: training or a gradient w.r.t. encoder_hidden_states while a "
                                           "SliderStack slider is active is not implemented (stacks are for inference; "
                                           "run under torch.no_grad())")
             # training: keep activations and hand torch.autograd a node whose backward runs the sb200 backward kernels
-            return self._forward_nograd(sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict,
+            return self._forward_nograd(sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict, snap,
                                         train=True, ehs_grad=ehs_grad)
         with torch.no_grad():
-            return self._forward_nograd(sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict)
+            return self._forward_nograd(sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict, snap)
 
-    def _check_ehs_grad(self, sample, added_cond_kwargs):
+    def _check_ehs_grad(self, sample, added_cond_kwargs, snap: lp.Snapshot):
         """The encoder_hidden_states gradient covers the batched cross-attention K / V path with frozen or trainable
         adaptors elsewhere; the cases below are not implemented and say so instead of returning a silent None."""
         if sample.requires_grad:
@@ -917,13 +592,13 @@ class UNet2DConditionModel(nn.Module):
         for k, v in (added_cond_kwargs or {}).items():
             if torch.is_tensor(v) and v.requires_grad:
                 raise NotImplementedError(f"sliders_b200: a gradient w.r.t. added_cond_kwargs['{k}'] is not implemented")
-        if self._cross_kv_adapted():
+        if self._cross_kv_adapted(snap):
             raise NotImplementedError(
                 "sliders_b200: a gradient w.r.t. encoder_hidden_states while adaptors on the cross-attention "
                 "attn2.to_k / to_v are active (train methods xattn / full with multiplier != 0) is not implemented")
 
-    def _forward_nograd(self, sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict, train=False,
-                        ehs_grad=False):
+    def _forward_nograd(self, sample, timestep, encoder_hidden_states, added_cond_kwargs, return_dict, snap,
+                        train=False, ehs_grad=False):
         if not sample.is_cuda:
             raise RuntimeError("sliders_b200.UNet2DConditionModel runs only on a CUDA (sm_90) device; "
                                "there is no CPU path (the CPU oracle lives under oracle/ for tests)")
@@ -943,70 +618,29 @@ class UNet2DConditionModel(nn.Module):
             from . import autograd as sb_autograd
 
             if ehs_grad:
-                self._check_ehs_grad(sample, added_cond_kwargs)
+                self._check_ehs_grad(sample, added_cond_kwargs, snap)
             # the autograd node converts encoder_hidden_states to bf16 itself, so that its gradient can come back in
             # the caller's dtype (fp32 for an optimised embedding)
-            out = sb_autograd.apply(self, x.detach(), t, encoder_hidden_states, added_cond_kwargs, out_dtype, ehs_grad)
+            out = sb_autograd.apply(self, x.detach(), t, encoder_hidden_states, added_cond_kwargs, out_dtype, snap,
+                                    ehs_grad)
         elif self.use_cuda_graph:
             ehs = encoder_hidden_states.to(device=dev, dtype=BF16).contiguous()
-            out = self._graphed(x, t, ehs, added_cond_kwargs, out_dtype)
+            out = self._graphed(x, t, ehs, added_cond_kwargs, out_dtype, snap)
         else:
             ehs = encoder_hidden_states.to(device=dev, dtype=BF16).contiguous()
-            out = self._walk(x, t, ehs, added_cond_kwargs, out_dtype)
+            out = self._walk(x, t, ehs, added_cond_kwargs, out_dtype, snap=snap)
         if not return_dict:
             return (out,)
         return UNet2DConditionOutput(sample=out)
 
     # ---- CUDA-graph replay -----------------------------------------------------------------------------
-    def _adapted_leaves(self):
-        cache = self.__dict__.get("_adapted_cache")
-        if cache is None:
-            cache = [m for m in self.modules() if isinstance(m, (nn.Linear, nn.Conv2d))]
-            self.__dict__["_adapted_cache"] = cache
-        return [(m, a) for m in cache for a in (_adaptor_of(m),) if a is not None]
-
-    def _lora_signature(self):
-        """(signature, common slider factor).  Which adaptors contribute is baked into a captured graph; when
-        every active adaptor has the same multiplier*alpha/rank (the only thing `with network:` /
-        `set_lora_slider` can produce, lora.py:249-258) that factor is a device-side scalar and the
-        signature does not depend on it; otherwise the individual factors are part of the signature.  The adaptors'
-        ranks are part of it too: they set the sizes of the packed buffers a graph reads."""
-        adapted = self._adapted_leaves()
-        scales = [float(a.multiplier) * float(a.scale) for _, a in adapted]
-        # per-sample values are device-side too, but a graph captured with them reads a vector the scalar graph does not
-        ranks = (tuple(int(a.lora_dim) for _, a in adapted),
-                 bool(_lora_mod.PER_SAMPLE_NETWORKS) and
-                 any(getattr(a, "sample_scales", None) is not None for _, a in adapted))
-        nz = [s for s in scales if s != 0.0]
-        if "_slider_stack" in self.__dict__ and self._stack_status() is not None:
-            # the stack's layout, not its multipliers (device-side): one graph serves every combination of scales
-            return (tuple(s != 0.0 for s in scales), ranks, None, self.__dict__["_slider_stack"].structure), None
-        if not nz:
-            return (tuple(False for _ in scales), ranks, None), None
-        if all(abs(s - nz[0]) < 1e-12 for s in nz):
-            return (tuple(s != 0.0 for s in scales), ranks, None), nz[0]
-        return (tuple(s != 0.0 for s in scales), ranks, tuple(scales)), None
-
-    def _needs_grad(self) -> bool:
-        """True when an active adaptor (multiplier != 0, i.e. inside `with network:`) has trainable weights."""
-        for _, a in self._adapted_leaves():
-            if float(a.multiplier) * float(a.scale) != 0.0 and a.lora_down.weight.requires_grad:
-                return True
-        stack = self.__dict__.get("_slider_stack")
-        if stack is not None:
-            for net, m in zip(stack.sliders, self._stack_status() or ()):
-                if m != 0.0 and any(p.requires_grad for p in net.parameters()):
-                    return True
-        return False
-
-    def _graphed(self, x, t, ehs, added, out_dtype):
-        sig, _ = self._lora_signature()
-        key = _GraphInputs.key(x, ehs, added, out_dtype) + (sig,)
+    def _graphed(self, x, t, ehs, added, out_dtype, snap: lp.Snapshot):
+        key = _GraphInputs.key(x, ehs, added, out_dtype) + (snap.signature,)
         cap = self._graphs.get(key)
         if cap is None:
-            cap = _CapturedForward(self, x, t, ehs, added, out_dtype)
+            cap = _CapturedForward(self, x, t, ehs, added, out_dtype, snap)
             self._graphs[key] = cap
-        return cap.replay(self, x, t, ehs, added)
+        return cap.replay(self, x, t, ehs, added, snap)
 
 
 class _GraphInputs:
@@ -1029,30 +663,16 @@ class _GraphInputs:
             addk = (tuple(added["text_embeds"].shape), tuple(added["time_ids"].shape))
         return (tuple(x.shape), x.dtype, tuple(ehs.shape), addk, out_dtype)
 
-    def load(self, unet: UNet2DConditionModel, x, t, ehs, added, bake: bool = False) -> None:
-        """Copies the call's inputs in, sets the device-side slider factor and refreshes the packed LoRA weights if the
-        optimiser changed them (same storage, so the graph sees them)."""
+    def load(self, unet: UNet2DConditionModel, x, t, ehs, added, snap: lp.Snapshot, bake: bool = False) -> None:
+        """Copies the call's inputs in, sets the device-side slider factors and refreshes the packed LoRA weights if
+        the optimiser changed them (same storage, so the graph sees them)."""
         self.x.copy_(x)
         self.t.copy_(t)
         self.ehs.copy_(ehs)
         if added is not None:
             self.added["text_embeds"].copy_(added["text_embeds"])
             self.added["time_ids"].copy_(added["time_ids"])
-        _, common = unet._lora_signature()
-        if unet._slider_scale_dev is not None:
-            unet._slider_scale_dev.fill_(1.0 if common is None else common)
-        if "_slider_stack" in unet.__dict__:
-            unet._stack_begin(compose=False)  # per-slider multipliers; the graph's own compose applies them
-        values = unet._sample_scan(x.shape[0])
-        if values is not None:
-            for (B, factor), vec in unet._sample_vecs.items():
-                if B == x.shape[0]:
-                    unet._fill_sample_vec(vec, factor, values)
-        unet._bake_scales = bake
-        try:
-            unet._refresh_lora_packs()
-        finally:
-            unet._bake_scales = False
+        unet._packer.refresh(snap, bake)
 
 
 class _CapturedForward(_GraphInputs):
@@ -1060,42 +680,24 @@ class _CapturedForward(_GraphInputs):
     buffers; the LoRA slider factor and the timestep are device-side values, so one graph serves every
     denoise step and every slider scale)."""
 
-    def __init__(self, unet: UNet2DConditionModel, x, t, ehs, added, out_dtype):
+    def __init__(self, unet: UNet2DConditionModel, x, t, ehs, added, out_dtype, snap: lp.Snapshot):
         super().__init__(x, t, ehs, added)
         # one decision for the whole graph: a factor common to ALL active adaptors is a device-side scalar (one graph
         # serves every slider scale); otherwise the factors are baked into the packed weights (and are part of the key)
-        self.bake = unet._lora_signature()[1] is None
-        unet._bake_scales = self.bake
+        self.bake = snap.common is None
         stream = torch.cuda.Stream(device=x.device)
         stream.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(stream):
             for _ in range(2):  # warm-up: fills weight / LoRA packing caches and the TMA descriptor cache
-                unet._walk(self.x, self.t, self.ehs, self.added, out_dtype)
+                unet._walk(self.x, self.t, self.ehs, self.added, out_dtype, snap=snap, bake=self.bake)
         torch.cuda.current_stream().wait_stream(stream)
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()
-        unet._capturing = True
-        try:
-            with torch.cuda.graph(self.graph):
-                self.out = unet._walk(self.x, self.t, self.ehs, self.added, out_dtype)
-        finally:
-            unet._capturing = False
-            unet._bake_scales = False
+        with torch.cuda.graph(self.graph):
+            self.out = unet._walk(self.x, self.t, self.ehs, self.added, out_dtype, snap=snap, capture=True,
+                                  bake=self.bake)
 
-    def replay(self, unet: UNet2DConditionModel, x, t, ehs, added):
-        self.load(unet, x, t, ehs, added, self.bake)
+    def replay(self, unet: UNet2DConditionModel, x, t, ehs, added, snap: lp.Snapshot):
+        self.load(unet, x, t, ehs, added, snap, self.bake)
         self.graph.replay()
         return self.out.clone()
-
-
-def _refresh(self: UNet2DConditionModel):
-    leaves_by_id = getattr(self, "_leaf_by_id", None)
-    if leaves_by_id is None:
-        leaves_by_id = {id(m): m for m in self.modules() if isinstance(m, (nn.Linear, nn.Conv2d))}
-        self._leaf_by_id = leaves_by_id
-    for key in list(self._lora_packs.keys()):
-        leaves = [leaves_by_id[i] for i in key]
-        self._lora(leaves)
-
-
-UNet2DConditionModel._refresh_lora_packs = _refresh

@@ -10,6 +10,7 @@ import torch.nn as nn
 from oracle import reference_bridge as rb
 from oracle import unet as ounet
 from sliders_b200 import lora as plora
+from sliders_b200 import lora_pack as lp
 from sliders_b200 import ops
 from sliders_b200.unet import UNet2DConditionModel, UNetConfig, _StackArena, _adaptor_of, _fill_composite, _hook_of
 
@@ -229,7 +230,7 @@ def test_slider_with_mixed_multipliers_is_refused():
     with pytest.raises(ValueError, match="smile_rank8.pt has modules with different multipliers"):
         stack.slider_multipliers()
     with pytest.raises(ValueError, match="smile_rank8.pt"):
-        pm._lora_signature()
+        lp.scan(pm, 1)
 
 
 def test_autograd_paths_with_an_active_stack_are_refused():
@@ -248,9 +249,10 @@ def test_autograd_paths_with_an_active_stack_are_refused():
         with pytest.raises(NotImplementedError, match="SliderStack slider is active"):
             pm(x, 1, encoder_hidden_states=ehs.requires_grad_(True), added_cond_kwargs=added)
         with pytest.raises(NotImplementedError, match="active SliderStack"):
-            sb_autograd._new_tape(pm)
+            sb_autograd._new_tape(lp.scan(pm, 1))
     # every slider off: nothing of the stack is active, so the engine would take the plain path
-    assert pm._stack_status() is None and not pm._needs_grad()
+    snap = lp.scan(pm, 1)
+    assert snap.stack_mults is None and not snap.needs_grad()
 
 
 def test_composite_hook_raises_when_called_through_pytorch():
@@ -276,16 +278,21 @@ def test_stack_scales_and_context_manager():
         stack.set_lora_slider([1.0, 2.0, 3.0])
 
 
+def _signature(pm):
+    snap = lp.scan(pm, 1)
+    return snap.signature, snap.common
+
+
 def test_graph_signature_holds_structure_not_scales():
     pm, stack = _stack()
-    plain_off = _unet()._lora_signature()
+    plain_off = _signature(_unet())
     stack.__exit__(None, None, None)
-    assert pm._lora_signature() == plain_off            # every slider at 0: the no-adaptor graph
+    assert _signature(pm) == plain_off            # every slider at 0: the no-adaptor graph
     sigs = set()
     for scales in ([1.0, 0.0], [0.0, -2.0], [2.0, -1.0], [0.5, 0.5]):
         stack.set_lora_slider(scales)
         with stack:
-            sig, common = pm._lora_signature()
+            sig, common = _signature(pm)
             assert common is None
             sigs.add(sig)
     assert len(sigs) == 1 and sig != plain_off[0]
@@ -311,10 +318,12 @@ def test_shape_trace_stand_in_sees_the_composite_slot():
     st = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(st)
     pm, stack = _stack()
+    pm._packer.begin(lp.scan(pm, 1), "cpu")
+    lora = st._slot_plan(pm._packer)
     attn1 = pm.mid_block.attentions[0].transformer_blocks[0].attn1
-    got = st._lora_slots([attn1.to_q, attn1.to_k, attn1.to_v])
+    got = lora([attn1.to_q, attn1.to_k, attn1.to_v])
     assert (got.r, got.rt) == ops.lora_slots(12, 3)
-    assert st._lora_slots([pm.conv_in]) is None
+    assert lora([pm.conv_in]) is None
 
 
 # ------------------------------------------------------------------------------------------------ --compose

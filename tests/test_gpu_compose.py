@@ -163,21 +163,22 @@ def _plain(dev, fx, rank, alpha, method, conv, state):
 
 def _plain_eps(pu, net, f, dev, scale, folded):
     """eps of the plain network at `scale`; `folded`: multiplier * alpha / r folded into the packed up weights (the
-    path `_lora` takes under graph capture when the factors differ) instead of applied in the GEMM epilogue."""
+    walk's `bake` mode, taken under graph capture when the factors differ) instead of applied in the GEMM epilogue."""
     net.set_lora_slider(scale)
-    pu._bake_scales = folded
-    try:
-        with net:
+    with net:
+        if not folded:
             return _eps(pu, f, dev)
-    finally:
-        pu._bake_scales = False
+        lat, ehs, added = _inputs(f, dev)
+        t = torch.full((lat.shape[0],), float(f["timestep"]), device=dev)
+        with torch.no_grad():
+            return pu._walk(lat.contiguous(), t, ehs.to(BF).contiguous(), added, lat.dtype, bake=True).float().cpu()
 
 
 def test_one_slider_on_matches_plain_network(dev):
     """One slider on, the other at 0, against that slider as a plain LoRANetwork on an identical UNet.
 
     A plain network has two paths for its scale multiplier * alpha / r: eager, with one factor common to every adaptor,
-    it is applied in the GEMM epilogue; under graph capture with differing factors (`_bake_scales`) it is folded into
+    it is applied in the GEMM epilogue; under graph capture with differing factors (the `bake` mode) it is folded into
     the packed up weights.  The stack always folds (per-slider scales cannot be one epilogue scalar), so it must equal
     the plain network's folded path bit for bit, both for the slider `alone` and for a `matched` network adapting
     exactly the stack's leaves (the slider's weights, lora_up = 0 elsewhere): the zero columns of the sliders at 0 and

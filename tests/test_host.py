@@ -723,14 +723,15 @@ def test_second_network_on_one_unet_is_refused():
     """ADVICE r1: the reference chains `org_forward`, so two LoRANetworks on one UNet both apply; the fused kernels carry
     one adaptor per leaf, so the engine must refuse instead of silently dropping the first network."""
     from sliders_b200 import lora as plora
+    from sliders_b200 import lora_pack as lp
     from sliders_b200.unet import UNet2DConditionModel, UNetConfig
 
     from oracle import unet as ounet
 
     pm = UNet2DConditionModel(UNetConfig.from_dict(ounet.UNetConfig.tiny_xl().__dict__))
     plora.LoRANetwork(pm, rank=4, alpha=1.0, train_method="noxattn")
-    assert len(pm._adapted_leaves()) > 0
+    assert len(lp.adapted_leaves(pm)) > 0
     plora.LoRANetwork(pm, rank=4, alpha=1.0, train_method="noxattn")
     pm.__dict__.pop("_adapted_cache", None)
     with pytest.raises(RuntimeError, match="second LoRANetwork"):
-        pm._adapted_leaves()
+        lp.adapted_leaves(pm)

@@ -63,7 +63,7 @@ def main():
             ms = bench.timed(call, 10, 3)
             fwd[name].append(8 / ms * 1e3)
             print(f"round {rnd} {name}: {fwd[name][-1]:.1f} passes/s", flush=True)
-            arena = unet._stack_arena
+            arena = unet._packer.arena
             if rnd == 0 and arena is not None:
                 rows, rp = arena.raw.shape
                 cms = bench.timed(lambda: ops.lora_compose(arena.raw, arena.mult, out=arena.eff), 200, 20)
@@ -71,7 +71,7 @@ def main():
                 compose[name] = {"packs": len(arena.packs), "rows": rows, "rp": rp, "us": round(cms * 1e3, 2),
                                  "bytes": nbytes, "GB_per_s": round(nbytes / (cms * 1e-3) / 1e9, 0)}
                 print(f"lora_compose {name}: {compose[name]}", flush=True)
-            unet._graphs.clear()  # one forward graph resident at a time
+            unet._drop_graphs()  # one forward graph resident at a time
     res = {"card": card(),
            "sdxl_1024px_8pass_graph_passes_per_s": {k: [round(v, 1) for v in vs] for k, vs in fwd.items()},
            "lora_compose": compose}

@@ -68,7 +68,7 @@ def main():
             ms = bench.timed(call, 10, 3)
             fwd[r].append(8 / ms * 1e3)
             print(f"round {rnd} rank {r}: {fwd[r][-1]:.1f} passes/s", flush=True)
-            unet._graphs.clear()  # one forward graph resident at a time
+            unet._drop_graphs()  # one forward graph resident at a time
     train = {}
     for r in (4, 16):
         unet, net = products[r]
@@ -93,8 +93,7 @@ def main():
         train[r] = bench.timed(text_it, 3, 1)
         print(f"text-slider iteration rank {r}: {train[r]:.1f} ms", flush=True)
         net.requires_grad_(False)
-        unet._graphs.clear()
-        unet.__dict__.pop("_train_graphs", None)
+        unet._drop_graphs()
     res = {"card": card(),
            "sdxl_1024px_8pass_graph_passes_per_s": {str(r): [round(v, 1) for v in fwd[r]] for r in ranks},
            "text_slider_iteration_ms": {str(r): round(v, 1) for r, v in train.items()},

@@ -26,17 +26,14 @@ def _note_lora(lora):
         lora_rts[len(calls) - 1] = lora.rt
 
 
-def _lora_slots(leaves):
-    """Stand-in for UNet2DConditionModel._lora: the (slot width r, rt) that ops.lora_slots gives the call's adaptors.
-    A leaf of a SliderStack takes the stack's composite slot, as wide as its total rank."""
-    from sliders_b200.unet import _adaptor_of, _hook_of
+def _slot_plan(packer):
+    """Stand-in for `packer.lora` that packs nothing: the (slot width r, rt) of each call from the packer's own slot
+    rule (LoraPacker.slots), which reads the walk's snapshot."""
+    def lora(leaves):
+        slots = packer.slots(leaves)
+        return None if slots is None else types.SimpleNamespace(r=slots[0], rt=slots[1])
 
-    ranks = [int(a.lora_dim) for a in map(_adaptor_of, leaves) if a is not None]
-    ranks += [h.stack.total_rank for h in map(_hook_of, leaves) if h is not None]
-    if not ranks:
-        return None
-    r, rt = ops.lora_slots(max(ranks), len(leaves))
-    return types.SimpleNamespace(r=r, rt=rt)
+    return lora
 
 
 def _meta(*shape):
@@ -138,7 +135,7 @@ def trace(batch, with_lora=True, train=False, extra_targets=(), rank=4):
             plora.DEFAULT_TARGET_REPLACE += plora.UNET_TARGET_REPLACE_MODULE_CONV + list(extra_targets)
             net = plora.LoRANetwork(unet, rank=rank, multiplier=1.0, alpha=1.0, train_method="noxattn")
             del plora.DEFAULT_TARGET_REPLACE[len(saved):]
-        unet._lora = _lora_slots
+        unet._packer.lora = _slot_plan(unet._packer)
         x = torch.empty(batch, 4, 128, 128, dtype=torch.float32)
         t = torch.empty(batch, dtype=torch.float32)
         ehs = torch.empty(batch, 77, 2048, dtype=torch.bfloat16)
