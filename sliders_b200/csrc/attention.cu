@@ -144,9 +144,9 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
       const uint32_t qoff = static_cast<uint32_t>(k >> 2) * kQTileBytes + static_cast<uint32_t>(k & 3) * 32;
       const uint32_t koff = static_cast<uint32_t>(k >> 2) * kKVChunk + static_cast<uint32_t>(k & 3) * 32;
       if constexpr (kKV == 128)
-        wgmma_ss_n128(sc, gmma_desc_sw128(sQw + qoff), gmma_desc_sw128(sK + s * kKVBytes + koff), k != 0);
+        wgmma_ss<128>(sc, gmma_desc_sw128(sQw + qoff), gmma_desc_sw128(sK + s * kKVBytes + koff), k != 0);
       else
-        wgmma_ss_n64(sc, gmma_desc_sw128(sQw + qoff), gmma_desc_sw128(sK + s * kKVBytes + koff), k != 0);
+        wgmma_ss<64>(sc, gmma_desc_sw128(sQw + qoff), gmma_desc_sw128(sK + s * kKVBytes + koff), k != 0);
     }
     wgmma_commit();
     wgmma_wait<0>();

@@ -66,9 +66,9 @@ __device__ __forceinline__ float bwd_exp2(float x) {
 template <int kN>
 __device__ __forceinline__ void wgmma_ss_t(float* d, uint64_t a, uint64_t b, uint32_t acc) {
   if constexpr (kN == 64)
-    wgmma_ss_n64(d, a, b, acc);
+    wgmma_ss<64>(d, a, b, acc);
   else
-    wgmma_ss_n32(d, a, b, acc);
+    wgmma_ss<32>(d, a, b, acc);
 }
 
 template <int ND>

@@ -7,7 +7,7 @@
 //   warps 0..7  two consumer warpgroups, rows 0..63 and 64..127 of the tile: wgmma m64 x BN x 16 from shared memory
 //               into registers; then the epilogue
 // The LoRA down-projection rides in the same k-block loop: its rows are staged right behind the W rows of the stage and
-// one more wgmma (N = rt) per k-step accumulates t = A . down^T.
+// the same wgmma (N = BN + rt) accumulates t = A . down^T in the tail of the fragment (lora_folded).
 // Epilogue: both warpgroups park their accumulators in shared memory as an fp32 [128 x (BN + rt)] tile (over the stage
 // ring, which is free once the main loop has ended).  Each thread then owns one row: rank-r LoRA up-projection,
 // bias / time-embedding row bias / GEGLU / residual; residual tiles come in by cp.async and results leave through a
@@ -167,15 +167,12 @@ __device__ __forceinline__ void store_frag(const float* d, uint32_t tile, int ro
   }
 }
 
-template <int BN>
-__device__ __forceinline__ void wgmma_main(float* d, uint64_t a, uint64_t b) {
-  if constexpr (BN == 64)
-    wgmma_ss_n64(d, a, b, 1u);
-  else if constexpr (BN == 128)
-    wgmma_ss_n128(d, a, b, 1u);
-  else
-    wgmma_ss_n256(d, a, b, 1u);
-}
+// The RT LoRA-down rows of a stage sit right behind its BN W rows, so [BN + RT, 64] is one K-major SW128 operand:
+// wherever one wgmma can take it (N <= 256) each k-step issues a single m64 x (BN + RT) product and t = A.down^T is the
+// tail of the accumulator fragment (registers BN/2 ..).  BN = 256 keeps a second product (N = RT) into its own fragment.
+__host__ __device__ constexpr bool lora_folded(int bn, int rt) { return rt != 0 && bn + rt <= 256; }
+__host__ __device__ constexpr int acc_regs(int bn, int rt) { return (lora_folded(bn, rt) ? bn + rt : bn) / 2; }
+__host__ __device__ constexpr int accl_regs(int bn, int rt) { return (rt == 0 || lora_folded(bn, rt)) ? 1 : rt / 2; }
 
 // Output tile t of the launch order -> its row tile mt and N tile nt
 __device__ __forceinline__ void tile_coords(const GemmParams& p, int t, int& mt, int& nt) {
@@ -341,18 +338,21 @@ __device__ __forceinline__ void fence_regs(float (&r)[N]) {
   for (int i = 0; i < N; ++i) reg_fence(r[i]);
 }
 
-// Main loop of consumer warpgroup wg (rows wg * 64 ..) over k-blocks [kb_lo, kb_hi): zeroes acc (m64 x BN) and accl
-// (t = A.down^T, m64 x RT), issues each k-block's wgmmas with one k-block's group kept in flight, and hands each stage
-// back (to both CTAs of a pair) once the products reading it are done.  On return every product has completed; the
-// caller fences the registers (fence_regs).  Returns the stage of the last k-block, which it has not handed back.
-template <int BN, int RT, int kCtas, int NL>
-__device__ __forceinline__ int consume(float (&acc)[BN / 2], float (&accl)[NL], const Ring& ring, int wg,
-                                       uint32_t cta_rank, int kb_lo, int kb_hi, int& stage, uint32_t& phase) {
+// Main loop of consumer warpgroup wg (rows wg * 64 ..) over k-blocks [kb_lo, kb_hi): zeroes acc (m64 x BN, with t =
+// A.down^T in its tail where lora_folded) and accl (t otherwise, m64 x RT), issues each k-block's wgmmas with one
+// k-block's group kept in flight, and hands each stage back (to both CTAs of a pair) once the products reading it are
+// done.  On return every product has completed; the caller fences the registers (fence_regs).  Returns the stage of
+// the last k-block, which it has not handed back.
+template <int BN, int RT, int kCtas>
+__device__ __forceinline__ int consume(float (&acc)[acc_regs(BN, RT)], float (&accl)[accl_regs(BN, RT)],
+                                       const Ring& ring, int wg, uint32_t cta_rank, int kb_lo, int kb_hi, int& stage,
+                                       uint32_t& phase) {
   constexpr uint32_t a_bytes = kBM * 128, b_bytes = BN * 128;
+  constexpr bool folded = lora_folded(BN, RT);
 #pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  for (int i = 0; i < acc_regs(BN, RT); ++i) acc[i] = 0.f;
 #pragma unroll
-  for (int i = 0; i < NL; ++i) accl[i] = 0.f;
+  for (int i = 0; i < accl_regs(BN, RT); ++i) accl[i] = 0.f;
   const bool signal = (threadIdx.x & 127) == 0;
   const uint32_t peer_empty = kCtas == 2 ? mapa_u32(ring.empty, cta_rank ^ 1u) : 0u;
   int prev = 0;
@@ -365,13 +365,12 @@ __device__ __forceinline__ int consume(float (&acc)[BN / 2], float (&accl)[NL], 
 #pragma unroll
     for (int k = 0; k < kBK / 16; ++k) {
       const uint64_t adesc = gmma_desc_sw128(sA + 32u * k);
-      wgmma_main<BN>(acc, adesc, gmma_desc_sw128(sB + 32u * k));
-      if constexpr (RT == 16)
-        wgmma_ss_n16(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
-      else if constexpr (RT == 32)
-        wgmma_ss_n32(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
-      else if constexpr (RT == 64)
-        wgmma_ss_n64(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
+      if constexpr (folded) {
+        wgmma_ss<BN + RT>(acc, adesc, gmma_desc_sw128(sB + 32u * k), 1u);
+      } else {
+        wgmma_ss<BN>(acc, adesc, gmma_desc_sw128(sB + 32u * k), 1u);
+        if constexpr (RT != 0) wgmma_ss<RT>(accl, adesc, gmma_desc_sw128(sB + b_bytes + 32u * k), 1u);
+      }
     }
     wgmma_commit();
     wgmma_wait<1>();  // the previous k-block's products have read their stage: hand it back to the producer(s)
@@ -396,7 +395,6 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
   // otherwise stay live across the LoRA update and spill the 96-register instantiations
   const bool has_lora = RT != 0 && (p.flags & SB200_EPI_LORA) != 0;
   const bool geglu = RT == 0 && (p.flags & SB200_EPI_GEGLU) != 0;
-  constexpr int rt = RT;  // LoRA-down rows of a stage (0 without LoRA)
   const Ring ring = gemm_prologue<kCtas>(p, has_lora);
 
   const int warp = threadIdx.x >> 5;
@@ -415,9 +413,9 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
   } else {
     // ------------------------------------------------------------------ consumers: main loop
     const int wg = warp >> 2;
-    constexpr int kAccl = RT > 32 ? RT / 2 : 16;  // t = A.down^T fragment registers
-    float acc[BN / 2];
-    float accl[kAccl];
+    static_assert(RT == 0 || lora_folded(BN, RT), "gemm_kernel keeps t = A.down^T in the accumulator's tail");
+    float acc[acc_regs(BN, RT)];
+    float accl[accl_regs(BN, RT)];
     consume<BN, RT, kCtas>(acc, accl, ring, wg, cta_rank, kb_lo, kb_hi, stage, phase);
     fence_regs(acc);
     fence_regs(accl);
@@ -426,13 +424,7 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
     const uint32_t accs = ring.tiles;  // fp32 accumulator tile, over the stage ring
     constexpr int kStride = acc_stride(BN, RT);
     asm volatile("bar.sync %0, %1;" ::"n"(kConsumerBar), "n"(32 * kEpiWarps) : "memory");  // both warpgroups done reading
-    store_frag<BN>(acc, accs, wg * 64, 0, kStride);
-    if constexpr (rt == 16)
-      store_frag<16>(accl, accs, wg * 64, BN, kStride);
-    else if constexpr (rt == 32)
-      store_frag<32>(accl, accs, wg * 64, BN, kStride);
-    else if constexpr (rt == 64)
-      store_frag<64>(accl, accs, wg * 64, BN, kStride);
+    store_frag<BN + RT>(acc, accs, wg * 64, 0, kStride);  // t = A.down^T lands in columns BN ..
     asm volatile("bar.sync %0, %1;" ::"n"(kConsumerBar), "n"(32 * kEpiWarps) : "memory");
     if (p.sk_ws != nullptr) {
       // split-K: this split's raw fp32 tile, row-coalesced; sb200_gemm_splitk_f32's reduction sums the splits
@@ -608,18 +600,21 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
 }
 
 // -------------------------------------------------------------------------------------------------
-// Wide tiles: a persistent kernel for layers whose W has a multiple of 256 rows
+// Wide tiles: a persistent kernel for layers whose W has a multiple of 160 or 256 rows
 // -------------------------------------------------------------------------------------------------
-// gemm_wide_kernel<RT, GEGLU>: 128 x 256 tiles (GEGLU: 256 W rows, 128 output columns), 384 threads, one CTA per SM,
+// gemm_wide_kernel<BN, RT, GEGLU>: 128 x BN tiles, BN = 256 (GEGLU: 256 W rows, 128 output columns) or 160 (every
+// width the SD / SDXL UNets run is a multiple of 320, so 160 tiles their 320- and 640-wide layers with no ragged
+// tile, and 160 + 32 LoRA rows still fit one wgmma), 384 threads, one CTA per SM,
 // each CTA walking the tiles blockIdx.x, blockIdx.x + gridDim.x, ... in launch_gemm's order:
 //   warpgroup 2    producer: gives its registers to the consumers (setmaxnreg 40); one elected thread of warp 8 issues
 //                  the TMA loads, running ahead into the next tile while the consumers finish the current epilogue
-//   warpgroups 0/1 consumers (setmaxnreg 232): rows 0..63 / 64..127, an m64 x 256 accumulator of 128 registers
+//   warpgroups 0/1 consumers (setmaxnreg 232): rows 0..63 / 64..127, an m64 x BN accumulator of BN / 2 registers
 // The k-loop, its barrier protocol and the LoRA-down rows behind the W rows are gemm_kernel's (gemm_prologue, produce
 // and consume, called once per tile); the ring's stage and phase run on across tiles, and the consumers hand each
 // tile's last stage back once its wgmmas are done.  The epilogue works on the accumulator registers: per element it applies, in gemm_kernel's
 // order and with its expressions, the LoRA update, bias, row bias and GEGLU, rounds to bf16, adds the residual in bf16,
-// and leaves through a swizzled staging buffer (two per warpgroup, 64 rows x 64 columns each) with coalesced stores.
+// and leaves through a swizzled staging buffer (two per warpgroup, 64 rows x wide_chunk columns each) with coalesced
+// stores.
 // Only t = A.down^T and the tile's lora_up rows are staged in shared memory.  No split-K or CTA pairs: those stay on
 // gemm_kernel.  GEGLU is a template parameter (only with RT = 0: GEGLU never comes with LoRA) rather than a flag: with
 // a runtime flag every element's gate code sat between the plain path's instructions and the chunk loop spanned
@@ -627,21 +622,35 @@ __global__ void __launch_bounds__(kGemmThreads, gemm_slots(BN, RT)) gemm_kernel(
 // stamps per phase on an H100 SXM at 700 W), far above its instruction count and in line with instruction fetch from
 // a loop that does not stay in the instruction cache.  Split, and with 16-byte output stores, a plain tile's epilogue
 // takes half the cycles (DESIGN §8 item 1).
-constexpr int kWideBN = 256;
 constexpr int kWideThreads = 384;
-constexpr int kWideChunk = 64;                        // output columns per staging buffer
-constexpr int kWideStgBytes = 64 * kWideChunk * 2;    // [64 rows x 64 cols] bf16, 128 B rows
-constexpr int kWideBarBase = 1;                       // named barriers 1, 2: one per consumer warpgroup
+constexpr int kWideBarBase = 1;  // named barriers 1, 2: one per consumer warpgroup
+
+// Output columns per staging buffer: 64 where they divide the tile (128 B rows, 16-byte chunks XOR-swizzled by row & 7),
+// else 32 (BN = 160: 64 B rows swizzled by (row >> 1) & 3, gemm_kernel's layout).  Either way the 8 rows a warp stores
+// to at once, and the 2 or 1 rows a quarter-warp copies out, fall into distinct banks.
+__host__ __device__ constexpr int wide_chunk(int bn) { return bn % 64 == 0 ? 64 : 32; }
+__host__ __device__ constexpr int wide_stg_bytes(int bn) { return 64 * wide_chunk(bn) * 2; }  // [64 rows x chunk] bf16
 
 // Shared memory of one consumer warpgroup's epilogue: two staging buffers, then with LoRA its 64 rows of t
-// (row stride rt + 4 floats) and the tile's 256 lora_up rows.
+// (row stride rt + 4 floats) and the tile's bn lora_up rows.
 __host__ __device__ constexpr int wide_t_bytes(int rt) { return rt ? 64 * (rt + 4) * 4 : 0; }
-__host__ __device__ constexpr int wide_epi_bytes(int rt, int r) {
-  return 2 * kWideStgBytes + wide_t_bytes(rt) + (rt ? kWideBN * r * 4 : 0);
+__host__ __device__ constexpr int wide_epi_bytes(int bn, int rt, int r) {
+  return 2 * wide_stg_bytes(bn) + wide_t_bytes(rt) + (rt ? bn * r * 4 : 0);
 }
 
-template <int RT, bool GEGLU>
+// t = A.down^T of a consumer warpgroup's rows: the accumulator's tail where the LoRA rows ride in the main wgmma
+template <int BN, int RT>
+__device__ __forceinline__ const float* t_frag(const float (&acc)[acc_regs(BN, RT)],
+                                               const float (&accl)[accl_regs(BN, RT)]) {
+  if constexpr (lora_folded(BN, RT))
+    return acc + BN / 2;
+  else
+    return accl;
+}
+
+template <int BN, int RT, bool GEGLU>
 __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid_constant__ GemmParams p) {
+  static_assert(!GEGLU || (BN % 256 == 0 && RT == 0), "GEGLU runs on 256-wide tiles without LoRA");
   const Ring ring = gemm_prologue<1>(p, RT != 0);
   const int warp = threadIdx.x >> 5;
   constexpr bool geglu = GEGLU;
@@ -656,7 +665,7 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       int mt, nt;
       tile_coords(p, t, mt, nt);
-      produce<kWideBN, RT, 1>(p, ring, a_origin(p, mt), nt, 0u, geglu, RT != 0, 0, p.kblocks, stage, phase);
+      produce<BN, RT, 1>(p, ring, a_origin(p, mt), nt, 0u, geglu, RT != 0, 0, p.kblocks, stage, phase);
     }
     return;
   }
@@ -674,14 +683,20 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
   const bool has_rb = (p.flags & SB200_EPI_ROWBIAS) != 0;
   const int r = has_lora ? p.lora_r : 0;
   const float lscale = has_lora ? (p.lora_scale_dev ? p.lora_scale * __ldg(p.lora_scale_dev) : p.lora_scale) : 0.f;
-  constexpr int nchunks = (GEGLU ? kWideBN / 2 : kWideBN) / kWideChunk;  // p.ncols_out / kWideChunk
+  constexpr int kChunk = wide_chunk(BN);
+  constexpr int kCpr = kChunk / 8;          // 16-byte chunks per staging row = 8-column accumulator blocks per chunk
+  constexpr int kPitch = kChunk * 2;        // bytes per staging row
+  constexpr int kCopyRows = 128 / kCpr;     // staging rows the warpgroup moves per pass
+  constexpr int kPasses = 64 / kCopyRows;
+  constexpr int nchunks = (GEGLU ? BN / 2 : BN) / kChunk;  // p.ncols_out / kChunk
+  auto swz = [](int row) { return kChunk == 64 ? (row & 7) : ((row >> 1) & 3); };
   const uint32_t epi = ring.tiles + static_cast<uint32_t>(ring.stages) * ring.stage_bytes +
-                       static_cast<uint32_t>(wg) * static_cast<uint32_t>(wide_epi_bytes(RT, r));
-  const uint32_t tbuf = epi + 2 * kWideStgBytes;  // [64][RT + 4] fp32: t of this warpgroup's rows
-  const uint32_t ubuf = tbuf + wide_t_bytes(RT);  // [256][r] fp32: the tile's lora_up rows
+                       static_cast<uint32_t>(wg) * static_cast<uint32_t>(wide_epi_bytes(BN, RT, r));
+  const uint32_t tbuf = epi + 2 * wide_stg_bytes(BN);  // [64][RT + 4] fp32: t of this warpgroup's rows
+  const uint32_t ubuf = tbuf + wide_t_bytes(RT);        // [BN][r] fp32: the tile's lora_up rows
   constexpr int kTStride = RT + 4;
-  // rows / 16-byte chunk this thread moves between a staging buffer and global memory: rows crow + 16 i, chunk cch
-  const int crow = tid >> 3, cch = tid & 7;
+  // rows / 16-byte chunk this thread moves between a staging buffer and global memory: rows crow + kCopyRows i, chunk cch
+  const int crow = tid / kCpr, cch = tid % kCpr;
   const uint32_t bar_id = kWideBarBase + wg;
   auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); };
 
@@ -689,16 +704,16 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
     int st, nt;
     tile_coords(p, t, st, nt);
     const int n_base = nt * p.ncols_out;
-    int orow[4];  // output rows this thread copies
+    int orow[kPasses];  // output rows this thread copies
 #pragma unroll
-    for (int i = 0; i < 4; ++i) orow[i] = tile_out_row(p, st, wg * 64 + crow + 16 * i);
+    for (int i = 0; i < kPasses; ++i) orow[i] = tile_out_row(p, st, wg * 64 + crow + kCopyRows * i);
     auto prefetch_resid = [&](int c, uint32_t buf) {
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int row = crow + 16 * i;
+      for (int i = 0; i < kPasses; ++i) {
+        const int row = crow + kCopyRows * i;
         if (orow[i] >= 0)
-          cp_async_16(buf + row * 128 + ((cch ^ (row & 7)) << 4),
-                      p.resid + static_cast<size_t>(orow[i]) * p.ldr + n_base + c * kWideChunk + cch * 8);
+          cp_async_16(buf + row * kPitch + ((cch ^ swz(row)) << 4),
+                      p.resid + static_cast<size_t>(orow[i]) * p.ldr + n_base + c * kChunk + cch * 8);
       }
       cp_async_commit();
     };
@@ -708,13 +723,13 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
     wg_sync();
     if constexpr (RT != 0) {
       const float* up_src = p.lora_up + static_cast<size_t>(n_base) * r;
-      for (int i = tid; i < kWideBN * r / 4; i += 128) cp_async_16(ubuf + i * 16, up_src + i * 4);
+      for (int i = tid; i < BN * r / 4; i += 128) cp_async_16(ubuf + i * 16, up_src + i * 4);
       cp_async_commit();
     }
     if (has_resid) prefetch_resid(0, epi);
-    float acc[kWideBN / 2];
-    float accl[RT ? RT / 2 : 1];
-    const int last = consume<kWideBN, RT, 1>(acc, accl, ring, wg, 0u, 0, p.kblocks, stage, phase);
+    float acc[acc_regs(BN, RT)];
+    float accl[accl_regs(BN, RT)];
+    const int last = consume<BN, RT, 1>(acc, accl, ring, wg, 0u, 0, p.kblocks, stage, phase);
     if (tid == 0) mbar_arrive(ring.empty + 8u * last);  // the last stage of the tile, for the producer's next tile
     fence_regs(acc);
     fence_regs(accl);
@@ -722,12 +737,13 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
     // ------------------------------------------------------------------ epilogue
     if constexpr (RT != 0) {
       // t = A.down^T of this warpgroup's rows (fragment layout as in wgmma.cuh)
+      const float* tf = t_frag<BN, RT>(acc, accl);
 #pragma unroll
       for (int i = 0; i < RT / 2; i += 2) {
         const int row = fr0 + 8 * ((i >> 1) & 1);
         const int col = 8 * (i >> 2) + 2 * q;
-        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(tbuf + (row * kTStride + col) * 4), "f"(accl[i]),
-                     "f"(accl[i + 1])
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(tbuf + (row * kTStride + col) * 4), "f"(tf[i]),
+                     "f"(tf[i + 1])
                      : "memory");
       }
     }
@@ -755,22 +771,28 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
     float tl[2][8];  // lsc * t of the current adaptor, rows fr0 and fr0 + 8
     int cur_grp = -1;
     // A runtime loop over the chunks keeps one copy of the epilogue code (unrolled it outgrows the instruction cache);
-    // each pass first selects its chunk's 32 accumulator registers (and with GEGLU its 32 gate registers).
+    // each pass first selects its chunk's accumulator registers (and with GEGLU its gate registers).
 #pragma unroll 1
     for (int c = 0; c < nchunks; ++c) {
       {
-        constexpr int kChunkRegs = kWideChunk / 2;  // accumulator registers per thread and chunk
+        constexpr int kChunkRegs = kChunk / 2;  // accumulator registers per thread and chunk
         float v[kChunkRegs], gv[kChunkRegs];
 #pragma unroll
         for (int k = 0; k < kChunkRegs; ++k) {
-          v[k] = c == 0 ? acc[k] : c == 1 ? acc[kChunkRegs + k] : c == 2 ? acc[2 * kChunkRegs + k] : acc[3 * kChunkRegs + k];
-          gv[k] = c == 0 ? acc[2 * kChunkRegs + k] : acc[3 * kChunkRegs + k];  // GEGLU: column + 128, the gate half
-        }
-        const uint32_t buf = epi + static_cast<uint32_t>(c & 1) * kWideStgBytes;
-        uint32_t o[8][2];
+          v[k] = acc[k];
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-          const int j = c * 8 + jj;  // 8-column block of the accumulator
+          for (int cc = 1; cc < nchunks; ++cc) v[k] = c == cc ? acc[cc * kChunkRegs + k] : v[k];
+          if constexpr (GEGLU) {  // column + BN / 2, the gate half
+            gv[k] = acc[nchunks * kChunkRegs + k];
+#pragma unroll
+            for (int cc = 1; cc < nchunks; ++cc) gv[k] = c == cc ? acc[(nchunks + cc) * kChunkRegs + k] : gv[k];
+          }
+        }
+        const uint32_t buf = epi + static_cast<uint32_t>(c & 1) * wide_stg_bytes(BN);
+        uint32_t o[kCpr][2];
+#pragma unroll
+        for (int jj = 0; jj < kCpr; ++jj) {
+          const int j = c * kCpr + jj;  // 8-column block of the accumulator
           const int n = n_base + 8 * j + 2 * q;
           float up[2][8];
           if constexpr (RT != 0) {
@@ -828,24 +850,25 @@ __global__ void __launch_bounds__(kWideThreads, 1) gemm_wide_kernel(const __grid
           cp_async_wait<0>();
           wg_sync();  // chunk c's residual has landed; chunk c - 1's copy-out from the other buffer is done
         }
-        if (has_resid && c + 1 < nchunks) prefetch_resid(c + 1, epi + static_cast<uint32_t>((c + 1) & 1) * kWideStgBytes);
+        if (has_resid && c + 1 < nchunks)
+          prefetch_resid(c + 1, epi + static_cast<uint32_t>((c + 1) & 1) * wide_stg_bytes(BN));
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
+        for (int jj = 0; jj < kCpr; ++jj) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int row = fr0 + 8 * h;
-            const uint32_t a = buf + row * 128 + ((jj ^ (row & 7)) << 4) + q * 4;
+            const uint32_t a = buf + row * kPitch + ((jj ^ swz(row)) << 4) + q * 4;
             // the residual is added to the ROUNDED projection, in bf16, as in gemm_kernel
             st_shared_u32(a, has_resid ? add_bf16x2(o[jj][h], ld_shared_u32(a)) : o[jj][h]);
           }
         }
         wg_sync();
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int row = crow + 16 * i;
-          const uint4 v = ld_shared_v4(buf + row * 128 + ((cch ^ (row & 7)) << 4));
+        for (int i = 0; i < kPasses; ++i) {
+          const int row = crow + kCopyRows * i;
+          const uint4 v = ld_shared_v4(buf + row * kPitch + ((cch ^ swz(row)) << 4));
           if (orow[i] >= 0)
-            st_global_v4(p.out + static_cast<size_t>(orow[i]) * p.ldo + n_base + c * kWideChunk + cch * 8, v);
+            st_global_v4(p.out + static_cast<size_t>(orow[i]) * p.ldo + n_base + c * kChunk + cch * 8, v);
         }
       }
     }
@@ -874,15 +897,16 @@ static bool pairs_always() {
   return v;
 }
 
-// Tile widths: 64 and 128 run gemm_kernel, 256 runs gemm_wide_kernel (a 256-wide accumulator needs the registers a
-// producer warpgroup gives up, which 288 threads do not have).
-static bool bn_supported(int bn) { return bn == 64 || bn == 128 || bn == kWideBN; }
+// Tile widths: 64 and 128 run gemm_kernel, 160 and 256 run gemm_wide_kernel (a 160- or 256-wide accumulator needs the
+// registers a producer warpgroup gives up, which 288 threads do not have).
+static bool is_wide(int bn) { return bn == 160 || bn == 256; }
+static bool bn_supported(int bn) { return bn == 64 || bn == 128 || is_wide(bn); }
 
-// gemm_wide_kernel takes W with a multiple of 256 rows (with GEGLU: 128 rows per half, so a tile writes 128 output
-// columns), single CTAs, and LoRA of rank 4 or 8 in at most 32 rows.
+// gemm_wide_kernel takes W with a multiple of bn rows (with GEGLU, only at bn = 256: 128 rows per half, so a tile
+// writes 128 output columns), single CTAs, and LoRA of rank 4 or 8 in at most 32 rows.
 static bool wide_lora_ok(int lora_r, int lora_rt) { return lora_rt == 0 || (lora_rt <= 32 && lora_r <= 8); }
-static bool wide_eligible(int N, int ctas, int lora_r, int lora_rt) {
-  return N % kWideBN == 0 && ctas == 1 && wide_lora_ok(lora_r, lora_rt);
+static bool wide_eligible(int bn, int N, int ctas, int lora_r, int lora_rt, bool geglu) {
+  return N % bn == 0 && ctas == 1 && wide_lora_ok(lora_r, lora_rt) && (bn == 256 || !geglu);
 }
 
 // Tile width from a cost model in SM cycles.  A 128 x bn tile's 64-deep k-block takes 4 bn cycles of tensor work (m64
@@ -896,23 +920,31 @@ static bool wide_eligible(int N, int ctas, int lora_r, int lora_rt) {
 // 8192 x 1280 x 5120 + residual 293 / 245, 8192 x 3840 x 1280 LoRA 299 / 241, 32768 x 5120 x 640 GEGLU 833 / 625,
 // 32768 x 1920 x 640 LoRA 361 / 315, 32768 x 640 x 640 LoRA + residual 137 / 131, 616 x 153600 x 2048 1225 / 949,
 // LoRA convs 32x32 1280 -> 1280 850 / 620, 64x64 640 -> 640 831 / 630, 128x128 320 -> 320 881 / 832 (B = 8).
-// gemm_wide_kernel in the same units: 4 (256 + rt) cycles per k-block, kWideLoraPerKb more with LoRA, and kWideTile per
-// tile (epilogue and pipeline refill; the wide epilogue does not overlap the tensor cores).  Fitted to the same shapes
-// timed with each width forced on an H100 80GB HBM3 SXM at 700 W, each wide time scaled by the BN = 128 model's cycles
-// over the BN = 128 time of the same shape so that the choice compares like with like (us, BN 64 / 128 / 256): 8192 x
-// 10240 x 1280 GEGLU 583 / 437 / 389, 8192 x 1280 x 5120 + residual 274 / 214 / 169, 32768 x 5120 x 640 GEGLU 742 / 525
-// / 476, 616 x 153600 x 2048 1104 / 734 / 587, 8192 x 1280 x 1280 bias 72.7 / 61.7 / 54.7, the same + residual 79.3 /
-// 69.7 / 57.9, 8192 x 3840 x 1280 LoRA 239 / 202 / 183, 8192 x 1280 x 1280 LoRA + residual 91.5 / 82.0 / 71.8, LoRA
-// convs 32x32 1280 -> 1280 + residual 677 / 456 / 462, 2560 -> 1280 1515 / 937 / 1121, 8192 x 1280 x 2560 LoRA (two
-// sources) - / 123 / 131 (B = 8); SD-1.5 at B = 1 (CFG pair): 512 x 1280 x 1280 + residual 10.9 / 13.3 / 18.6, 512 x
-// 3840 x 1280 LoRA 19.8 / 15.1 / 23.8, 512 x 10240 x 1280 GEGLU 46.2 / 42.4 / 39.3, 2048 x 5120 x 640 GEGLU 51.0 / 40.4
-// / 40.2, convs 16x16 and 8x8 1280 -> 1280 + residual 73 / 83 / 111 and 73 / 82 / 110.  A LoRA k-block costs the wide
-// tile more than its 16 extra columns (there the LoRA ring has three stages, gemm_kernel's six; the cause was not
-// measured), so LoRA wins on the wide tile only where it saves waves at moderate K: the q|k|v and attention-out
-// projections, not the deep-K LoRA convs or the 2.4-wave K = 2560 shortcut. The fit reproduces every choice but the 512
-// x 10240 GEGLU, which stays at 128 (8 % slower than 256).
+// gemm_wide_kernel in the same units: 4 (bn + rt) cycles per k-block, a LoRA term more with LoRA, and a per-tile term
+// (epilogue and pipeline refill; the wide epilogue does not overlap the tensor cores): kWideLoraPerKb / kWideTile at
+// bn = 256, kW160LoraPerKb / kW160Tile at bn = 160, where the LoRA-down rows ride in the main wgmma (lora_folded) and a
+// LoRA k-block costs less than half as much.  The 256 constants were fitted earlier (its LoRA k-block costs more than
+// its 16 extra columns); the 160 ones are the grid-search optimum over the times below, with each width forced, on an
+// H100 80GB HBM3 SXM at 700 W (us, BN 64 / 128 / 160 / 256, "-" where the width does not divide N), B = 8 SDXL:
+// 8192 x 10240 x 1280 GEGLU 585 / 442 / - / 387, 8192 x 1280 x 5120 + residual 277 / 217 / 155 / 170, 32768 x 5120 x
+// 640 GEGLU 752 / 531 / - / 457, 616 x 153600 x 2048 1115 / 744 / 666 / 607, 8192 x 1280 x 1280 bias 72.1 / 61.7 / 50.0
+// / 54.8, the same + residual 79.5 / 70.4 / 57.2 / 57.9, 8192 x 3840 x 1280 LoRA 223 / 199 / 180 / 182, 8192 x 1280 x
+// 1280 LoRA + residual 84.7 / 79.1 / 63.4 / 72.3, 32768 x 1920 x 640 LoRA 274 / 262 / 231 / -, 32768 x 640 x 640 bias +
+// residual 104 / 81.8 / 79.3 / -, the same with LoRA 111 / 116 / 90.7 / -, 32768 x 640 x 2560 + residual 277 / 208 /
+// 175 / -, LoRA convs 32x32 1280 -> 1280 + residual 693 / 451 / 372 / 464, 2560 -> 1280 1540 / 959 / 795 / 1184, 64x64
+// 640 -> 640 + residual 689 / 476 / 394 / -, 128x128 320 -> 320 + residual 732 / 757 / 450 / -, 640 -> 320 1438 / 1368
+// / 779 / -; SD-1.5 at B = 1 (CFG pair): 512 x 1280 x 1280 + residual 10.1 / 13.2 / 13.0 / 18.3, 512 x 3840 x 1280
+// LoRA 16.8 / 14.5 / 17.1 / 23.5, 512 x 10240 x 1280 GEGLU 46.4 / 42.4 / - / 38.3, 2048 x 5120 x 640 GEGLU 50.9 / 40.7
+// / - / 39.1, convs 16x16 and 8x8 1280 -> 1280 + residual 73 / 82 / 85 / 112 and 74 / 82 / 84 / 112, 8192 x 320 x 320
+// LoRA + residual 16.1 / 17.9 / 10.8 / -, 8192 x 960 x 320 LoRA 29.0 / 30.2 / 26.0 / -, 2048 x 640 x 640 LoRA +
+// residual 11.8 / 11.3 / 12.0 / -, LoRA convs + residual 64x64 320 -> 320 54.2 / 55.0 / 28.9 / - and 32x32 640 -> 640
+// 61.2 / 47.4 / 48.8 / -.  Single-wave grids (SD-1.5 at B = 1) stay on the narrow tiles, whose smaller tiles finish
+// sooner.  The model picks the fastest width for every shape but the 512 x 10240 GEGLU, which stays at 128 (10 %
+// slower than 256).
 constexpr double kWideTile = 5400.0;
 constexpr double kWideLoraPerKb = 370.0;
+constexpr double kW160Tile = 5600.0;
+constexpr double kW160LoraPerKb = 160.0;
 static TileChoice pick_tile(int ncols, int num_sms, int kblocks, int lora_r, int lora_rt, int force_ctas, int sub_tiles,
                             int flags) {
   double best = -1;
@@ -920,15 +952,16 @@ static TileChoice pick_tile(int ncols, int num_sms, int kblocks, int lora_r, int
   const int ctas = force_ctas ? force_ctas : (pairs_always() ? 2 : 1);
   const bool geglu = (flags & SB200_EPI_GEGLU) != 0;
   const double epi_per_col = 21.0 + ((flags & SB200_EPI_RESID) ? 7.5 : 0.0) + (lora_rt ? 9.0 : 0.0) + (geglu ? 15.0 : 0.0);
-  const int max_bn = wide_eligible(ncols, ctas, lora_r, lora_rt) ? kWideBN : 128;
-  for (int bn = 64; bn <= max_bn; bn *= 2) {
+  for (const int bn : {64, 128, 160, 256}) {
+    if (is_wide(bn) && !wide_eligible(bn, ncols, ctas, lora_r, lora_rt, geglu)) continue;
     const long tiles = static_cast<long>(sub_tiles) * ((ncols + bn - 1) / bn);
     const long load = (tiles + num_sms - 1) / num_sms;
     const int cols_out = geglu ? bn / 2 : bn;
     double cost;
-    if (bn == kWideBN) {
+    if (is_wide(bn)) {
       // persistent, one CTA per SM
-      cost = load * (kblocks * (4.0 * (bn + lora_rt) + (lora_rt ? kWideLoraPerKb : 0.0)) + kWideTile);
+      const double lora_kb = lora_rt ? (bn == 256 ? kWideLoraPerKb : kW160LoraPerKb) : 0.0;
+      cost = load * (kblocks * (4.0 * (bn + lora_rt) + lora_kb) + (bn == 256 ? kWideTile : kW160Tile));
     } else {
       const int slots = gemm_slots(bn, lora_rt);
       const double perkb = 4.0 * (bn + lora_rt) + 208.0;
@@ -989,6 +1022,17 @@ static int launch_narrow(Ctx* ctx, cudaStream_t s, const GemmParams& p, int rt, 
   }
 }
 
+// gemm_wide_kernel<BN, RT, GEGLU> for the call's RT and epilogue
+template <int BN>
+static int launch_wide(Ctx* ctx, cudaStream_t s, const GemmParams& p, int rt, dim3 grid, int smem) {
+  constexpr int T = kWideThreads;
+  if (rt == 16) return launch_checked<gemm_wide_kernel<BN, 16, false>, T, 1>(ctx, s, p, grid, smem, 1);
+  if (rt != 0) return launch_checked<gemm_wide_kernel<BN, 32, false>, T, 1>(ctx, s, p, grid, smem, 1);
+  if constexpr (BN == 256)
+    if (p.flags & SB200_EPI_GEGLU) return launch_checked<gemm_wide_kernel<BN, 0, true>, T, 1>(ctx, s, p, grid, smem, 1);
+  return launch_checked<gemm_wide_kernel<BN, 0, false>, T, 1>(ctx, s, p, grid, smem, 1);
+}
+
 static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
   // Tile order: N fastest reads each A row-tile from DRAM once and re-reads W once per row-tile, which is free while W
   // stays in L2.  When W is the big operand and does not fit (the batched cross-attention K/V projection: 616 x 2048
@@ -1005,10 +1049,10 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
   p.up_buf_bytes = has_lora ? kSlab * p.lora_r * 4 : 0;
   const int rt = has_lora ? p.lora_rt : 0;
   int st;
-  if (p.bn == kWideBN) {
+  if (is_wide(p.bn)) {
     // one CTA per SM: the ring gets what the two warpgroups' epilogue buffers leave of the SM's shared memory
     const int budget = smem_budget(ctx, 1);
-    const int epi = 2 * wide_epi_bytes(rt, has_lora ? p.lora_r : 0);
+    const int epi = 2 * wide_epi_bytes(p.bn, rt, has_lora ? p.lora_r : 0);
     const int stages = std::min(kMaxStages, (budget - kBarRegion - kAlignSlack - epi) / p.stage_bytes);
     if (stages < 2) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
     p.stages = stages;
@@ -1016,14 +1060,7 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
     const int smem = kBarRegion + kAlignSlack + p.ring_bytes;
     pdl_hint() = p.num_m_tiles * p.num_n_tiles <= 2 * ctx->num_sms;
     const dim3 grid(std::min(p.num_m_tiles * p.num_n_tiles, ctx->num_sms));
-    if (rt == 16)
-      st = launch_checked<gemm_wide_kernel<16, false>, kWideThreads, 1>(ctx, stream, p, grid, smem, 1);
-    else if (rt != 0)
-      st = launch_checked<gemm_wide_kernel<32, false>, kWideThreads, 1>(ctx, stream, p, grid, smem, 1);
-    else if (p.flags & SB200_EPI_GEGLU)
-      st = launch_checked<gemm_wide_kernel<0, true>, kWideThreads, 1>(ctx, stream, p, grid, smem, 1);
-    else
-      st = launch_checked<gemm_wide_kernel<0, false>, kWideThreads, 1>(ctx, stream, p, grid, smem, 1);
+    st = p.bn == 160 ? launch_wide<160>(ctx, stream, p, rt, grid, smem) : launch_wide<256>(ctx, stream, p, rt, grid, smem);
   } else {
     const int grid_ctas = p.num_m_tiles * p.num_n_tiles * ctas * (p.sk_ws ? p.sk_splits : 1);
     // A grid that gives each SM at most one CTA lets that CTA have the whole SM's shared memory (a deeper ring).
@@ -1107,9 +1144,10 @@ static int plan_and_launch(Ctx* ctx, cudaStream_t stream, GemmParams& p, const c
   TileChoice tc = pick_tile(p.N, ctx->num_sms, p.kblocks, p.lora_r, p.lora_rt, force_ctas, p.num_sub, flags);
   if (bn > 0) tc.bn = bn;
   if (force_ctas) tc.ctas = force_ctas;
-  SB200_REQUIRE(bn_supported(tc.bn), "%s: bn=%d invalid (64, 128 or 256)", who, tc.bn);
-  SB200_REQUIRE(tc.bn != kWideBN || wide_eligible(p.N, tc.ctas, p.lora_r, p.lora_rt),
-                "%s: bn=256 needs N %% 256 == 0 and single CTAs, without LoRA of rank 16 or rt 64 (N=%d)", who, p.N);
+  SB200_REQUIRE(bn_supported(tc.bn), "%s: bn=%d invalid (64, 128, 160 or 256)", who, tc.bn);
+  SB200_REQUIRE(!is_wide(tc.bn) || wide_eligible(tc.bn, p.N, tc.ctas, p.lora_r, p.lora_rt, geglu),
+                "%s: bn=%d needs N %% %d == 0 and single CTAs, without LoRA of rank 16 or rt 64%s (N=%d)", who, tc.bn,
+                tc.bn, tc.bn == 160 ? " or GEGLU" : "", p.N);
   p.Nout = geglu ? p.N / 2 : p.N;
   p.bn = tc.bn;
   p.ncols_out = geglu ? tc.bn / 2 : tc.bn;

@@ -1,5 +1,6 @@
-"""The shapes of pick_tile's fit (sliders_b200/csrc/gemm.cu) timed with the tile width forced to 64, 128 and 256
+"""The shapes of pick_tile's fit (sliders_b200/csrc/gemm.cu) timed with the tile width forced to 64, 128, 160 and 256
 (single CTAs) and with the width pick_tile chooses, in us per launch: the data its cost-model constants are fitted to.
+A width the shape cannot take (160 or 256 on an N that is not a multiple of it) shows as "-".
 
     python tools/gpu_time_gemm_widths.py [--json PATH]
 """
@@ -59,12 +60,23 @@ def main():
         ("32768x1920x640 LoRA", gemm(32768, 1920, 640, la=lora(640, 1920, 4, 640))),
         ("conv 8x32x32 1280->1280 LoRA + residual", conv(8, 32, 1280, 1280, resid=True, la=lora(9 * 1280, 1280, 4, 1280))),
         ("conv 8x32x32 2560->1280 LoRA", conv(8, 32, 2560, 1280, la=lora(9 * 2560, 1280, 4, 1280))),
+        ("32768x640x640 bias + residual", gemm(32768, 640, 640, bias=True, resid=True)),
+        ("32768x640x640 LoRA + residual", gemm(32768, 640, 640, bias=True, resid=True, la=lora(640, 640, 4, 640))),
+        ("32768x640x2560 + residual", gemm(32768, 640, 2560, bias=True, resid=True)),
+        ("conv 8x64x64 640->640 LoRA + residual", conv(8, 64, 640, 640, resid=True, la=lora(9 * 640, 640, 4, 640))),
+        ("conv 8x128x128 320->320 LoRA + residual", conv(8, 128, 320, 320, resid=True, la=lora(9 * 320, 320, 4, 320))),
+        ("conv 8x128x128 640->320 LoRA", conv(8, 128, 640, 320, la=lora(9 * 640, 320, 4, 320))),
         ("SD-1.5 512x1280x1280 + residual", gemm(512, 1280, 1280, bias=True, resid=True)),
         ("SD-1.5 512x3840x1280 LoRA", gemm(512, 3840, 1280, la=lora(1280, 3840, 4, 1280))),
         ("SD-1.5 512x10240x1280 GEGLU", gemm(512, 10240, 1280, bias=True, geglu=True)),
         ("SD-1.5 2048x5120x640 GEGLU", gemm(2048, 5120, 640, bias=True, geglu=True)),
         ("SD-1.5 conv 2x16x16 1280->1280 + residual", conv(2, 16, 1280, 1280, resid=True)),
         ("SD-1.5 conv 2x8x8 1280->1280 + residual", conv(2, 8, 1280, 1280, resid=True)),
+        ("SD-1.5 8192x320x320 LoRA + residual", gemm(8192, 320, 320, bias=True, resid=True, la=lora(320, 320, 4, 320))),
+        ("SD-1.5 8192x960x320 LoRA", gemm(8192, 960, 320, la=lora(320, 960, 4, 320))),
+        ("SD-1.5 2048x640x640 LoRA + residual", gemm(2048, 640, 640, bias=True, resid=True, la=lora(640, 640, 4, 640))),
+        ("SD-1.5 conv 2x64x64 320->320 LoRA + residual", conv(2, 64, 320, 320, resid=True, la=lora(9 * 320, 320, 4, 320))),
+        ("SD-1.5 conv 2x32x32 640->640 LoRA + residual", conv(2, 32, 640, 640, resid=True, la=lora(9 * 640, 640, 4, 640))),
     ]
 
     def time_us(fn, bn, iters=20, repeats=5):
@@ -85,20 +97,21 @@ def main():
 
     gpu = torch.cuda.get_device_name(dev)
     print(f"{gpu}: us per launch, median of 5 x 20 launches")
-    print("| shape | bn 64 | bn 128 | bn 256 | picked |")
-    print("|---|---|---|---|---|")
+    widths = (64, 128, 160, 256)
+    print("| shape | " + " | ".join(f"bn {bn}" for bn in widths) + " | picked |")
+    print("|---" * (len(widths) + 2) + "|")
     rows = []
     with torch.no_grad():
         for name, fn in cases:
             row = {"shape": name}
-            for bn in (64, 128, 256):
+            for bn in widths:
                 try:
                     row[str(bn)] = time_us(fn, bn)
-                except _cabi.Sb200Error:  # bn = 256 on a width that is not a multiple of 256
+                except _cabi.Sb200Error:  # a width the shape cannot take
                     row[str(bn)] = None
             row["picked"] = time_us(fn, 0)
             rows.append(row)
-            cells = " | ".join(f"{row[str(bn)]:.1f}" if row[str(bn)] else "-" for bn in (64, 128, 256))
+            cells = " | ".join(f"{row[str(bn)]:.1f}" if row[str(bn)] else "-" for bn in widths)
             print(f"| {name} | {cells} | {row['picked']:.1f} |", flush=True)
     if args.json:
         with open(args.json, "w") as f:
