@@ -230,14 +230,14 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
 }
 
 template <int ND>
-static int launch_attention(cudaStream_t stream, const AttnParams& p, dim3 grid) {
+static int launch_attention(cudaStream_t stream, const AttnParams& p, dim3 grid, bool pdl) {
   static bool attr_set = false;
   if (!attr_set) {
     SB200_CUDA_CHECK(
         cudaFuncSetAttribute(attention_kernel<ND>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnCfg<ND>::kSmem));
     attr_set = true;
   }
-  SB200_CUDA_CHECK(launch_pdl(attention_kernel<ND>, grid, dim3(kAttnThreads), AttnCfg<ND>::kSmem, stream, p));
+  SB200_CUDA_CHECK(launch_pdl(attention_kernel<ND>, grid, dim3(kAttnThreads), AttnCfg<ND>::kSmem, stream, pdl, p));
   SB200_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -290,8 +290,8 @@ extern "C" int sb200_attention(void* handle, void* stream, const void* q, int ld
   p.scale_log2 = scale * 1.4426950408889634f;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   dim3 grid((Sq + 127) / 128, heads, B);
-  pdl_hint() = static_cast<long long>(grid.x) * grid.y * grid.z <= 2LL * ctx->num_sms;
-  if (head_dim <= 64) return launch_attention<1>(s, p, grid);
-  if (head_dim <= 128) return launch_attention<2>(s, p, grid);
-  return launch_attention<3>(s, p, grid);
+  const bool pdl = pdl_small_grid(ctx, static_cast<long long>(grid.x) * grid.y * grid.z);
+  if (head_dim <= 64) return launch_attention<1>(s, p, grid, pdl);
+  if (head_dim <= 128) return launch_attention<2>(s, p, grid, pdl);
+  return launch_attention<3>(s, p, grid, pdl);
 }

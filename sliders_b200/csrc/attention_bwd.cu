@@ -341,7 +341,7 @@ static int launch_attention_bwd(cudaStream_t stream, const AttnBwdParams& p, dim
                                           AttnBwdCfg<ND>::kSmem));
     attr_set = true;
   }
-  SB200_CUDA_CHECK(launch_pdl(attention_bwd_kernel<ND>, grid, dim3(kBwdThreads), AttnBwdCfg<ND>::kSmem, stream, p));
+  SB200_CUDA_CHECK(launch_pdl(attention_bwd_kernel<ND>, grid, dim3(kBwdThreads), AttnBwdCfg<ND>::kSmem, stream, true, p));
   SB200_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -384,7 +384,6 @@ static int attention_bwd_impl(void* handle, void* stream, const void* q, int ldq
                               const float* lse, float* dsum, void* dq, int lddq, void* dk, int lddk, void* dv,
                               int lddv, int B, int heads, int Sq, int Skv, int head_dim, float scale, float* ws,
                               size_t ws_floats) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx, "attention_bwd: NULL handle");
   SB200_REQUIRE(B > 0 && heads > 0 && Sq > 0 && Skv > 0, "attention_bwd: bad dims");
@@ -403,7 +402,7 @@ static int attention_bwd_impl(void* handle, void* stream, const void* q, int ldq
   {
     const size_t total = static_cast<size_t>(B) * Sq * heads;
     SB200_CUDA_CHECK(launch_pdl(attn_bwd_prep_kernel, dim3(static_cast<unsigned>((total + 255) / 256)), dim3(256), 0, s,
-                                static_cast<const __nv_bfloat16*>(o), ldo, static_cast<const __nv_bfloat16*>(dout), lddo,
+                                true, static_cast<const __nv_bfloat16*>(o), ldo, static_cast<const __nv_bfloat16*>(dout), lddo,
                                 dsum, B, heads, Sq, head_dim));
     SB200_CUDA_CHECK(cudaGetLastError());
   }
@@ -449,7 +448,7 @@ static int attention_bwd_impl(void* handle, void* stream, const void* q, int ldq
     if ((st = launch_attention_bwd_d(s, p, gs))) return st;
     const size_t quads = static_cast<size_t>(B) * Skv * heads * head_dim / 4;
     SB200_CUDA_CHECK(launch_pdl(attn_bwd_reduce_kernel, dim3(static_cast<unsigned>((quads + 255) / 256), 2), dim3(256),
-                                0, s, static_cast<const float*>(ws), nsplit, B * Skv, heads * head_dim,
+                                0, s, true, static_cast<const float*>(ws), nsplit, B * Skv, heads * head_dim,
                                 static_cast<__nv_bfloat16*>(dv), lddv, static_cast<__nv_bfloat16*>(dk), lddk));
     SB200_CUDA_CHECK(cudaGetLastError());
     return 0;

@@ -53,8 +53,6 @@ struct GnBwdArgs {
   int silu;
 };
 
-constexpr int kGnBwdMaxChunks = 128;
-
 __device__ __forceinline__ void gn_bwd_load(const GnBwdArgs& a, int b, int c, const float*& st,
                                             const __nv_bfloat16*& src, int& ld, int& cc, float* gm, float* bt,
                                             float* mean, float* rstd) {
@@ -857,12 +855,6 @@ __global__ void adam_f32_kernel(const AdamTensorF32* __restrict__ table, float w
   }
 }
 
-static inline int grid_for(size_t work, int threads, int sms) {
-  size_t b = (work + threads - 1) / threads;
-  const size_t cap = static_cast<size_t>(sms) * 16;
-  return static_cast<int>(b < 1 ? 1 : (b > cap ? cap : b));
-}
-
 }  // namespace sb200
 
 using namespace sb200;
@@ -872,7 +864,6 @@ extern "C" int sb200_groupnorm_bwd(void* handle, void* stream, const void* x0, i
                                    int ldx1, int C1, const void* gamma, const void* beta, const void* dy, int lddy,
                                    const void* add, int ldadd, void* dx, int lddx, int B, int HW, int groups,
                                    int silu, const float* fwd_stats, float* ws) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx, "groupnorm_bwd: NULL handle");
   if (!x1) C1 = 0;
@@ -899,10 +890,7 @@ extern "C" int sb200_groupnorm_bwd(void* handle, void* stream, const void* x0, i
   a.lddx = lddx;
   a.stats = fwd_stats;
   a.silu = silu;
-  const int nvec = C / 8;
-  int rows_par = 512 / nvec;
-  if (rows_par < 1) rows_par = 1;
-  const int threads = nvec * rows_par;
+  const GnShape g = gn_shape(ctx, B, HW, C);
   // above C = 4096 a block has C/8 > 512 threads; the stats / apply kernels' register use caps the block size
   int max_threads = 1024;
   for (const void* fn : {reinterpret_cast<const void*>(gn_bwd_stats_kernel), reinterpret_cast<const void*>(gn_bwd_apply_kernel)}) {
@@ -910,32 +898,25 @@ extern "C" int sb200_groupnorm_bwd(void* handle, void* stream, const void* x0, i
     SB200_CUDA_CHECK(cudaFuncGetAttributes(&attr, fn));
     if (attr.maxThreadsPerBlock < max_threads) max_threads = attr.maxThreadsPerBlock;
   }
-  SB200_REQUIRE(threads <= max_threads, "groupnorm_bwd: C=%d too large (%d threads per block, at most %d)", C, threads,
+  SB200_REQUIRE(g.threads <= max_threads, "groupnorm_bwd: C=%d too large (%d threads per block, at most %d)", C, g.threads,
                 max_threads);
-  int chunks = (ctx->num_sms * 4 + B - 1) / B;
-  if (chunks > kGnBwdMaxChunks) chunks = kGnBwdMaxChunks;
-  int rows_per_block = (HW + chunks - 1) / chunks;
-  if (rows_per_block < rows_par * 8) rows_per_block = rows_par * 8;
-  chunks = (HW + rows_per_block - 1) / rows_per_block;
-  a.rows_per_block = rows_per_block;
-  float* final_m = ws + static_cast<size_t>(B) * kGnBwdMaxChunks * groups * 2;
-  SB200_CUDA_CHECK(launch_pdl(gn_bwd_stats_kernel, dim3(dim3(chunks, B)), dim3(threads), sizeof(float) * 2 * C * rows_par, s, a, ws));
-  SB200_CUDA_CHECK(launch_pdl(gn_bwd_finalize_kernel, dim3(B), dim3(1024), 0, s, ws, final_m, chunks, groups, 1.f / (static_cast<float>(HW) * a.cpg)));
-  SB200_CUDA_CHECK(launch_pdl(gn_bwd_apply_kernel, dim3(dim3(chunks, B)), dim3(threads), 0, s, a, final_m));
+  a.rows_per_block = g.rows_per_block;
+  float* final_m = ws + SB200_GN_STATS_OFFSET(B, groups);
+  SB200_CUDA_CHECK(launch_pdl(gn_bwd_stats_kernel, dim3(g.chunks, B), dim3(g.threads), sizeof(float) * 2 * C * g.rows_par, s, true, a, ws));
+  SB200_CUDA_CHECK(launch_pdl(gn_bwd_finalize_kernel, dim3(B), dim3(1024), 0, s, true, ws, final_m, g.chunks, groups, 1.f / (static_cast<float>(HW) * a.cpg)));
+  SB200_CUDA_CHECK(launch_pdl(gn_bwd_apply_kernel, dim3(g.chunks, B), dim3(g.threads), 0, s, true, a, final_m));
   return 0;
 }
 
 extern "C" int sb200_layernorm_bwd(void* handle, void* stream, const void* x, int ldx, const void* gamma,
                                    const void* dy, int lddy, const void* add, int ldadd, void* dx, int lddx, int M,
                                    int C, float eps) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx, "layernorm_bwd: NULL handle");
   SB200_REQUIRE(M > 0 && C > 0 && C % 8 == 0 && C <= 2048, "layernorm_bwd: C=%d unsupported", C);
   SB200_REQUIRE(ldx % 8 == 0 && lddy % 8 == 0 && lddx % 8 == 0 && (!add || ldadd % 8 == 0), "layernorm_bwd: leading dims");
   const int warps = 8;
-  int blocks = (M + warps - 1) / warps;
-  if (blocks > ctx->num_sms * 16) blocks = ctx->num_sms * 16;
+  const int blocks = grid_cap(ctx, M, warps, 16);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define SB200_LNB(NV)                                                                                           \
   layernorm_bwd_kernel<NV><<<blocks, warps * 32, 0, st>>>(static_cast<const bf*>(x), ldx,                        \
@@ -956,22 +937,20 @@ extern "C" int sb200_layernorm_bwd(void* handle, void* stream, const void* x, in
 }
 
 extern "C" int sb200_geglu(void* handle, void* stream, const void* pre, int ldp, void* out, int ldo, int M, int F) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && M > 0 && F > 0 && F % 8 == 0 && ldp % 8 == 0 && ldo % 8 == 0, "geglu: arguments");
-  SB200_CUDA_CHECK(launch_pdl(geglu_kernel, dim3(grid_for(static_cast<size_t>(M) * F / 8, 256, ctx->num_sms)), dim3(256), 0,
-                              static_cast<cudaStream_t>(stream), static_cast<const bf*>(pre), ldp, static_cast<bf*>(out), ldo, M, F));
+  SB200_CUDA_CHECK(launch_pdl(geglu_kernel, dim3(grid_cap(ctx, static_cast<size_t>(M) * F / 8, 256, 16, true)), dim3(256), 0,
+                              static_cast<cudaStream_t>(stream), true, static_cast<const bf*>(pre), ldp, static_cast<bf*>(out), ldo, M, F));
   return 0;
 }
 
 extern "C" int sb200_geglu_bwd(void* handle, void* stream, const void* pre, int ldp, const void* dout, int lddo,
                                void* dpre, int lddp, int M, int F) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && M > 0 && F > 0 && F % 8 == 0 && ldp % 8 == 0 && lddo % 8 == 0 && lddp % 8 == 0,
                 "geglu_bwd: arguments");
-  SB200_CUDA_CHECK(launch_pdl(geglu_bwd_kernel, dim3(grid_for(static_cast<size_t>(M) * F / 8, 256, ctx->num_sms)), dim3(256), 0,
-                              static_cast<cudaStream_t>(stream), static_cast<const bf*>(pre), ldp,
+  SB200_CUDA_CHECK(launch_pdl(geglu_bwd_kernel, dim3(grid_cap(ctx, static_cast<size_t>(M) * F / 8, 256, 16, true)), dim3(256), 0,
+                              static_cast<cudaStream_t>(stream), true, static_cast<const bf*>(pre), ldp,
                                                           static_cast<const bf*>(dout), lddo, static_cast<bf*>(dpre),
                                                           lddp, M, F));
   return 0;
@@ -979,73 +958,65 @@ extern "C" int sb200_geglu_bwd(void* handle, void* stream, const void* pre, int 
 
 extern "C" int sb200_add(void* handle, void* stream, const void* a, int lda, const void* b, int ldb, const void* c,
                          int ldc, void* out, int ldo, int M, int C) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && a && b && out && M > 0 && C > 0 && C % 8 == 0 && lda % 8 == 0 && ldb % 8 == 0 &&
                     ldo % 8 == 0 && (!c || ldc % 8 == 0),
                 "add: arguments");
-  SB200_CUDA_CHECK(launch_pdl(add_kernel, dim3(grid_for(static_cast<size_t>(M) * C / 8, 256, ctx->num_sms)), dim3(256), 0,
-                              static_cast<cudaStream_t>(stream), static_cast<const bf*>(a), lda, static_cast<const bf*>(b), ldb,
+  SB200_CUDA_CHECK(launch_pdl(add_kernel, dim3(grid_cap(ctx, static_cast<size_t>(M) * C / 8, 256, 16, true)), dim3(256), 0,
+                              static_cast<cudaStream_t>(stream), true, static_cast<const bf*>(a), lda, static_cast<const bf*>(b), ldb,
                                                     static_cast<const bf*>(c), ldc, static_cast<bf*>(out), ldo, M, C));
   return 0;
 }
 
 extern "C" int sb200_upsample2x_bwd(void* handle, void* stream, const void* dy, void* dx, int B, int H, int W, int C) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && dy && dx && B > 0 && H > 0 && W > 0 && C % 8 == 0, "upsample2x_bwd: arguments");
-  SB200_CUDA_CHECK(launch_pdl(upsample2x_bwd_kernel, dim3(grid_for(static_cast<size_t>(B) * H * W * C / 8, 256, ctx->num_sms)), dim3(256), 0,
-                              static_cast<cudaStream_t>(stream), static_cast<const bf*>(dy), static_cast<bf*>(dx), B, H, W, C));
+  SB200_CUDA_CHECK(launch_pdl(upsample2x_bwd_kernel, dim3(grid_cap(ctx, static_cast<size_t>(B) * H * W * C / 8, 256, 16, true)), dim3(256), 0,
+                              static_cast<cudaStream_t>(stream), true, static_cast<const bf*>(dy), static_cast<bf*>(dx), B, H, W, C));
   return 0;
 }
 
 extern "C" int sb200_zero_stuff(void* handle, void* stream, const void* dy, void* z, int B, int Ho, int Wo, int C) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && dy && z && B > 0 && Ho > 0 && Wo > 0 && C % 8 == 0, "zero_stuff: arguments");
-  SB200_CUDA_CHECK(launch_pdl(zero_stuff_kernel, dim3(grid_for(static_cast<size_t>(B) * 4 * Ho * Wo * C / 8, 256, ctx->num_sms)), dim3(256), 0,
-                              static_cast<cudaStream_t>(stream), static_cast<const bf*>(dy), static_cast<bf*>(z), B, Ho, Wo, C));
+  SB200_CUDA_CHECK(launch_pdl(zero_stuff_kernel, dim3(grid_cap(ctx, static_cast<size_t>(B) * 4 * Ho * Wo * C / 8, 256, 16, true)), dim3(256), 0,
+                              static_cast<cudaStream_t>(stream), true, static_cast<const bf*>(dy), static_cast<bf*>(z), B, Ho, Wo, C));
   return 0;
 }
 
 extern "C" int sb200_conv_out_bwd(void* handle, void* stream, const void* deps, int deps_f32, const void* w, void* dx,
                                   int B, int H, int W, int C) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && deps && w && dx && B > 0 && H > 0 && W > 0 && C % 8 == 0, "conv_out_bwd: arguments");
-  SB200_CUDA_CHECK(launch_pdl(conv_out_bwd_kernel, dim3(grid_for(static_cast<size_t>(B) * H * W * C / 8, 256, ctx->num_sms)), dim3(256), 0,
-                              static_cast<cudaStream_t>(stream), deps, deps_f32, static_cast<const bf*>(w),
+  SB200_CUDA_CHECK(launch_pdl(conv_out_bwd_kernel, dim3(grid_cap(ctx, static_cast<size_t>(B) * H * W * C / 8, 256, 16, true)), dim3(256), 0,
+                              static_cast<cudaStream_t>(stream), true, deps, deps_f32, static_cast<const bf*>(w),
                                                              static_cast<bf*>(dx), B, H, W, C));
   return 0;
 }
 
 extern "C" int sb200_colsum(void* handle, void* stream, const void* dy, int ld, float* out, int B, int HW, int C) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && dy && out && B > 0 && HW > 0 && C % 8 == 0 && ld % 8 == 0, "colsum: arguments");
   const int vpb = 8, rows_par = 64;  // 64 channels per block: many blocks, each streams 128-byte row pieces
   dim3 grid((C / 8 + vpb - 1) / vpb, B), block(vpb, rows_par);
-  SB200_CUDA_CHECK(launch_pdl(colsum_kernel, dim3(grid), dim3(block), sizeof(float) * rows_par * vpb * 8, static_cast<cudaStream_t>(stream), 
+  SB200_CUDA_CHECK(launch_pdl(colsum_kernel, dim3(grid), dim3(block), sizeof(float) * rows_par * vpb * 8, static_cast<cudaStream_t>(stream), true, 
       static_cast<const bf*>(dy), ld, out, HW, C));
   return 0;
 }
 
 extern "C" int sb200_lora_proj(void* handle, void* stream, const void* A, int lda, const void* Bt, int ldb, float* T,
                                int M, int C, int r, int accumulate) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && A && Bt && T && M > 0 && C % 8 == 0 && lda % 8 == 0 && ldb % 8 == 0 &&
                     (r == 4 || r == 8 || r == 16),
                 "lora_proj: arguments (r=%d)", r);
-  int blocks = (M + 7) / 8;
-  if (blocks > ctx->num_sms * 16) blocks = ctx->num_sms * 16;
-  SB200_CUDA_CHECK(launch_pdl(lora_proj_kernel, dim3(blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), static_cast<const bf*>(A), lda,
+  const int blocks = grid_cap(ctx, M, 8, 16);
+  SB200_CUDA_CHECK(launch_pdl(lora_proj_kernel, dim3(blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), true, static_cast<const bf*>(A), lda,
                                                                           static_cast<const bf*>(Bt), ldb, T, M, C, r, accumulate));
   return 0;
 }
 
-static int wgrad_chunks(Ctx* ctx, int rows, int cblocks, int* rows_per_block) {
-  (void)ctx;
+static int wgrad_chunks(int rows, int cblocks, int* rows_per_block) {
   int chunks = (264 + cblocks - 1) / cblocks;  // two per SM of an H100, fixed (not num_sms-derived) so callers can size `ws`: see sb200.h
   if (chunks > 256) chunks = 256;
   int rpb = (rows + chunks - 1) / chunks;
@@ -1057,26 +1028,24 @@ static int wgrad_chunks(Ctx* ctx, int rows, int cblocks, int* rows_per_block) {
 /* ws must hold SB200_WGRAD_WS_FLOATS(C, r) floats */
 extern "C" int sb200_lora_wgrad(void* handle, void* stream, const void* A, int lda, const float* T, float* G,
                                 int gs_c, int gs_r, float scale, int accumulate, int M, int C, int r, float* ws) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && A && T && G && ws && M > 0 && C % 8 == 0 && lda % 8 == 0 && (r == 4 || r == 8 || r == 16),
                 "lora_wgrad: arguments (r=%d)", r);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int cblocks = (C / 8 + kVB - 1) / kVB;
   int rpb;
-  const int chunks = wgrad_chunks(ctx, M, cblocks, &rpb);
+  const int chunks = wgrad_chunks(M, cblocks, &rpb);
   dim3 grid(chunks, cblocks, r == 16 ? 2 : 1), block(kVB, 4);
   if (r == 4)
-    SB200_CUDA_CHECK(launch_pdl(lora_wgrad_kernel<4>, dim3(grid), dim3(block), 0, s, static_cast<const bf*>(A), lda, T, ws, M, C, rpb));
+    SB200_CUDA_CHECK(launch_pdl(lora_wgrad_kernel<4>, dim3(grid), dim3(block), 0, s, true, static_cast<const bf*>(A), lda, T, ws, M, C, rpb));
   else
-    SB200_CUDA_CHECK(launch_pdl(lora_wgrad_kernel<8>, dim3(grid), dim3(block), 0, s, static_cast<const bf*>(A), lda, T, ws, M, C, rpb));
-  SB200_CUDA_CHECK(launch_pdl(lora_wgrad_reduce_kernel, dim3((C * r + 255) / 256), dim3(256), 0, s, ws, G, chunks, C, r, gs_c, gs_r, scale, accumulate));
+    SB200_CUDA_CHECK(launch_pdl(lora_wgrad_kernel<8>, dim3(grid), dim3(block), 0, s, true, static_cast<const bf*>(A), lda, T, ws, M, C, rpb));
+  SB200_CUDA_CHECK(launch_pdl(lora_wgrad_reduce_kernel, dim3((C * r + 255) / 256), dim3(256), 0, s, true, ws, G, chunks, C, r, gs_c, gs_r, scale, accumulate));
   return 0;
 }
 
 extern "C" int sb200_lora_rank_update(void* handle, void* stream, void* dX, int ldx, const float* U, const void* D,
                                       int ldd, float scale, int M, int C, int r) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && dX && U && D && M > 0 && C % 8 == 0 && ldx % 8 == 0 && ldd % 8 == 0 &&
                     (r == 4 || r == 8 || r == 16),
@@ -1084,16 +1053,16 @@ extern "C" int sb200_lora_rank_update(void* handle, void* stream, void* dX, int 
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int cblocks = (C / 8 + kVB - 1) / kVB;
   int rpb;
-  const int chunks = wgrad_chunks(ctx, M, cblocks, &rpb);
+  const int chunks = wgrad_chunks(M, cblocks, &rpb);
   dim3 grid(chunks, cblocks), block(kVB, 4);
   if (r == 4)
-    SB200_CUDA_CHECK(launch_pdl(lora_rank_update_kernel<4>, dim3(grid), dim3(block), 0, s, static_cast<bf*>(dX), ldx, U, static_cast<const bf*>(D), ldd,
+    SB200_CUDA_CHECK(launch_pdl(lora_rank_update_kernel<4>, dim3(grid), dim3(block), 0, s, true, static_cast<bf*>(dX), ldx, U, static_cast<const bf*>(D), ldd,
                                                      scale, M, C, rpb));
   else if (r == 8)
-    SB200_CUDA_CHECK(launch_pdl(lora_rank_update_kernel<8>, dim3(grid), dim3(block), 0, s, static_cast<bf*>(dX), ldx, U, static_cast<const bf*>(D), ldd,
+    SB200_CUDA_CHECK(launch_pdl(lora_rank_update_kernel<8>, dim3(grid), dim3(block), 0, s, true, static_cast<bf*>(dX), ldx, U, static_cast<const bf*>(D), ldd,
                                                      scale, M, C, rpb));
   else
-    SB200_CUDA_CHECK(launch_pdl(lora_rank_update_kernel<16>, dim3(grid), dim3(block), 0, s, static_cast<bf*>(dX), ldx, U, static_cast<const bf*>(D), ldd,
+    SB200_CUDA_CHECK(launch_pdl(lora_rank_update_kernel<16>, dim3(grid), dim3(block), 0, s, true, static_cast<bf*>(dX), ldx, U, static_cast<const bf*>(D), ldd,
                                                      scale, M, C, rpb));
   return 0;
 }
@@ -1109,7 +1078,6 @@ static int fill_geom(ConvGeom* g, const void* x0, int ldx0, int C0, const void* 
 
 extern "C" int sb200_lora_conv_proj(void* handle, void* stream, const void* x0, int ldx0, int C0, const void* x1,
                                     int ldx1, int C1, const void* D, float* T, int B, int H, int W, int stride, int r) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && x0 && D && T && C0 % 8 == 0 && (!x1 || C1 % 8 == 0) && (stride == 1 || stride == 2) &&
                     (r == 4 || r == 8 || r == 16),
@@ -1117,9 +1085,8 @@ extern "C" int sb200_lora_conv_proj(void* handle, void* stream, const void* x0, 
   ConvGeom g;
   fill_geom(&g, x0, ldx0, C0, x1, ldx1, C1, B, H, W, stride);
   const int P = B * g.Ho * g.Wo;
-  int blocks = (P + 7) / 8;
-  if (blocks > ctx->num_sms * 16) blocks = ctx->num_sms * 16;
-  SB200_CUDA_CHECK(launch_pdl(lora_conv_proj_kernel, dim3(blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), g, static_cast<const bf*>(D), T, r));
+  const int blocks = grid_cap(ctx, P, 8, 16);
+  SB200_CUDA_CHECK(launch_pdl(lora_conv_proj_kernel, dim3(blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), true, g, static_cast<const bf*>(D), T, r));
   return 0;
 }
 
@@ -1127,7 +1094,6 @@ extern "C" int sb200_lora_conv_proj(void* handle, void* stream, const void* x0, 
 extern "C" int sb200_lora_conv_wgrad(void* handle, void* stream, const void* x0, int ldx0, int C0, const void* x1,
                                      int ldx1, int C1, const float* U, float* G, float scale, int accumulate, int B,
                                      int H, int W, int stride, int r, float* ws) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && x0 && U && G && ws && C0 % 8 == 0 && (!x1 || C1 % 8 == 0) && (stride == 1 || stride == 2) &&
                     (r == 4 || r == 8 || r == 16),
@@ -1138,35 +1104,34 @@ extern "C" int sb200_lora_conv_wgrad(void* handle, void* stream, const void* x0,
   const int P = B * g.Ho * g.Wo;
   const int cblocks = (g.C / 8 + kVB - 1) / kVB;
   int rpb;
-  const int chunks = wgrad_chunks(ctx, P, cblocks * 9, &rpb);
+  const int chunks = wgrad_chunks(P, cblocks * 9, &rpb);
   dim3 grid(chunks, cblocks, r == 16 ? 18 : 9), block(kVB, 4);
   if (r == 4)
-    SB200_CUDA_CHECK(launch_pdl(lora_conv_wgrad_kernel<4>, dim3(grid), dim3(block), 0, s, g, U, ws, rpb));
+    SB200_CUDA_CHECK(launch_pdl(lora_conv_wgrad_kernel<4>, dim3(grid), dim3(block), 0, s, true, g, U, ws, rpb));
   else
-    SB200_CUDA_CHECK(launch_pdl(lora_conv_wgrad_kernel<8>, dim3(grid), dim3(block), 0, s, g, U, ws, rpb));
+    SB200_CUDA_CHECK(launch_pdl(lora_conv_wgrad_kernel<8>, dim3(grid), dim3(block), 0, s, true, g, U, ws, rpb));
   const int C9 = 9 * g.C;
   // G[j][tap*C + c]: gs_c = 1, gs_r = 9*C
-  SB200_CUDA_CHECK(launch_pdl(lora_wgrad_reduce_kernel, dim3((C9 * r + 255) / 256), dim3(256), 0, s, ws, G, chunks, C9, r, 1, C9, scale, accumulate));
+  SB200_CUDA_CHECK(launch_pdl(lora_wgrad_reduce_kernel, dim3((C9 * r + 255) / 256), dim3(256), 0, s, true, ws, G, chunks, C9, r, 1, C9, scale, accumulate));
   return 0;
 }
 
 extern "C" int sb200_lora_conv_rank_update(void* handle, void* stream, void* dX, const float* U, const void* D,
                                            float scale, int B, int H, int W, int C, int stride, int r) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && dX && U && D && C % 8 == 0 && (stride == 1 || stride == 2) &&
                     (r == 4 || r == 8 || r == 16),
                 "lora_conv_rank_update: arguments");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int blocks = grid_for(static_cast<size_t>(B) * H * W * C / 8, 256, ctx->num_sms);
+  const int blocks = grid_cap(ctx, static_cast<size_t>(B) * H * W * C / 8, 256, 16, true);
   if (r == 4)
-    SB200_CUDA_CHECK(launch_pdl(lora_conv_rank_update_kernel<4>, dim3(blocks), dim3(256), 0, s, static_cast<bf*>(dX), B, H, W, C, H / stride, W / stride,
+    SB200_CUDA_CHECK(launch_pdl(lora_conv_rank_update_kernel<4>, dim3(blocks), dim3(256), 0, s, true, static_cast<bf*>(dX), B, H, W, C, H / stride, W / stride,
                                                           stride, U, static_cast<const bf*>(D), scale));
   else if (r == 8)
-    SB200_CUDA_CHECK(launch_pdl(lora_conv_rank_update_kernel<8>, dim3(blocks), dim3(256), 0, s, static_cast<bf*>(dX), B, H, W, C, H / stride, W / stride,
+    SB200_CUDA_CHECK(launch_pdl(lora_conv_rank_update_kernel<8>, dim3(blocks), dim3(256), 0, s, true, static_cast<bf*>(dX), B, H, W, C, H / stride, W / stride,
                                                           stride, U, static_cast<const bf*>(D), scale));
   else
-    SB200_CUDA_CHECK(launch_pdl(lora_conv_rank_update_kernel<16>, dim3(blocks), dim3(256), 0, s, static_cast<bf*>(dX), B, H, W, C, H / stride, W / stride,
+    SB200_CUDA_CHECK(launch_pdl(lora_conv_rank_update_kernel<16>, dim3(blocks), dim3(256), 0, s, true, static_cast<bf*>(dX), B, H, W, C, H / stride, W / stride,
                                                           stride, U, static_cast<const bf*>(D), scale));
   return 0;
 }
@@ -1174,7 +1139,6 @@ extern "C" int sb200_lora_conv_rank_update(void* handle, void* stream, void* dX,
 /* table: device array of n_tensors {p, g, m, v (device pointers), n (int64)} records (5 x 8 bytes each) */
 extern "C" int sb200_adamw(void* handle, void* stream, const void* table, int n_tensors, long long max_numel,
                            double lr, double beta1, double beta2, double eps, double weight_decay, int step) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && table && n_tensors > 0 && max_numel > 0 && step >= 1, "adamw: arguments");
   SB200_REQUIRE(n_tensors <= 65535, "adamw: %d tensors exceed the grid's 65535 y-blocks", n_tensors);
@@ -1183,7 +1147,7 @@ extern "C" int sb200_adamw(void* handle, void* stream, const void* table, int n_
   const double bc2 = 1.0 - pow(beta2, static_cast<double>(step));
   int bx = static_cast<int>((max_numel + 255) / 256);
   if (bx > 64) bx = 64;
-  SB200_CUDA_CHECK(launch_pdl(adamw_kernel, dim3(dim3(bx, n_tensors)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+  SB200_CUDA_CHECK(launch_pdl(adamw_kernel, dim3(dim3(bx, n_tensors)), dim3(256), 0, static_cast<cudaStream_t>(stream), true, 
       static_cast<const AdamTensor*>(table), static_cast<float>(1.0 - lr * weight_decay),
       static_cast<float>(1.0 - beta1), static_cast<float>(beta2), static_cast<float>(1.0 - beta2),
       static_cast<float>(eps), static_cast<float>(-(lr / bc1)), static_cast<float>(sqrt(bc2))));
@@ -1192,13 +1156,12 @@ extern "C" int sb200_adamw(void* handle, void* stream, const void* table, int n_
 
 extern "C" int sb200_adam_f32(void* handle, void* stream, const void* table, int n_tensors, long long max_numel,
                               double lr, double beta1, double beta2, double eps, double weight_decay, int step) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && table && n_tensors > 0 && max_numel > 0 && step >= 1, "adam_f32: arguments");
   SB200_REQUIRE(n_tensors <= 65535, "adam_f32: %d tensors exceed the grid's 65535 y-blocks", n_tensors);
   const double bc1 = 1.0 - pow(beta1, step), bc2 = 1.0 - pow(beta2, step);
-  const int bx = grid_for(static_cast<size_t>(max_numel), 256, ctx->num_sms);
-  SB200_CUDA_CHECK(launch_pdl(adam_f32_kernel, dim3(bx, n_tensors), dim3(256), 0, static_cast<cudaStream_t>(stream),
+  const int bx = grid_cap(ctx, static_cast<size_t>(max_numel), 256, 16, true);
+  SB200_CUDA_CHECK(launch_pdl(adam_f32_kernel, dim3(bx, n_tensors), dim3(256), 0, static_cast<cudaStream_t>(stream), true,
                               static_cast<const AdamTensorF32*>(table), static_cast<float>(weight_decay),
                               static_cast<float>(1.0 - beta1), static_cast<float>(beta2),
                               static_cast<float>(1.0 - beta2), static_cast<float>(eps), static_cast<float>(-lr / bc1),

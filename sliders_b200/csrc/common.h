@@ -73,8 +73,8 @@ struct Ctx {
 int make_tmap_bf16(Ctx* ctx, CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims,
                    const uint64_t* strides_bytes, const uint32_t* box);
 
-// SB200_PDL=0 disables programmatic dependent launch, 2 applies it to every launch whatever its size (same-box A/B;
-// default 1: only launches that do not fill the machine, see pdl_hint)
+// SB200_PDL=0 disables programmatic dependent launch, 2 applies it to every launch_ex / launch_pdl whatever its size
+// (same-box A/B); default 1: each launch's `pdl` argument decides
 inline int pdl_mode() {
   static const int m = [] {
     const char* e = getenv("SB200_PDL");
@@ -83,20 +83,17 @@ inline int pdl_mode() {
   return m;
 }
 
-// Per-call hint set by the C-ABI entry points: PDL pays off for small launches (launch latency and prologue are a
-// visible share: +3 % at 2 passes per forward) and costs ~1 % on machine-filling ones (8 passes), so the big shapes
-// launch without it.
-inline bool& pdl_hint() {
-  static thread_local bool h = true;
-  return h;
-}
+// PDL pays off for small launches (launch latency and prologue are a visible share: +3 % at 2 passes per forward) and
+// costs ~1 % on machine-filling ones (8 passes), so the GEMM and attention forward use it only on grids of at most two
+// CTAs per SM
+inline bool pdl_small_grid(const Ctx* ctx, long long ctas) { return ctas <= 2LL * ctx->num_sms; }
 
 // <<<grid, block, smem, stream>>> in clusters of `cluster_x` CTAs along x (1: no cluster), with the
-// programmatic-stream-serialization attribute as pdl_mode() / pdl_hint() decide (the kernel must call pdl_wait() before
+// programmatic-stream-serialization attribute as pdl_mode() and `pdl` decide (the kernel must call pdl_wait() before
 // touching global memory)
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                             unsigned cluster_x, Args&&... args) {
+                             unsigned cluster_x, bool pdl, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
@@ -104,7 +101,7 @@ inline cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, si
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = (pdl_mode() == 2 || (pdl_mode() == 1 && pdl_hint())) ? 1 : 0;
+  attr[0].val.programmaticStreamSerializationAllowed = (pdl_mode() == 2 || (pdl_mode() == 1 && pdl)) ? 1 : 0;
   attr[1].id = cudaLaunchAttributeClusterDimension;
   attr[1].val.clusterDim.x = cluster_x;
   attr[1].val.clusterDim.y = 1;
@@ -116,8 +113,18 @@ inline cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, si
 
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                              Args&&... args) {
-  return launch_ex(kernel, grid, block, smem, stream, 1u, static_cast<Args&&>(args)...);
+                              bool pdl, Args&&... args) {
+  return launch_ex(kernel, grid, block, smem, stream, 1u, pdl, static_cast<Args&&>(args)...);
+}
+
+// Grid of a grid-stride kernel: ceil(work / per_block) blocks, at most `waves` per SM, computed in the type of `work`;
+// at_least_one launches one block for empty work.
+template <typename T>
+inline int grid_cap(const Ctx* ctx, T work, int per_block, int waves, bool at_least_one = false) {
+  T blocks = (work + per_block - 1) / per_block;
+  const T cap = static_cast<T>(ctx->num_sms) * waves;
+  if (blocks > cap) blocks = cap;
+  return at_least_one && blocks < 1 ? 1 : static_cast<int>(blocks);
 }
 
 inline Ctx* as_ctx(void* h) { return reinterpret_cast<Ctx*>(h); }
@@ -131,6 +138,28 @@ inline int gn_rows_par(int C) {
 }
 inline bool gn_stats_smem_ok(int C) {
   return C > 0 && sizeof(float) * 2 * static_cast<size_t>(C) * gn_rows_par(C) <= 48 * 1024;
+}
+
+// The partials of at most this many row chunks per sample precede the final (mean, rstd) block in the workspace
+// (the 128 of SB200_GN_STATS_OFFSET).
+constexpr int kGnMaxChunks = 128;
+static_assert(SB200_GN_STATS_OFFSET(1, 1) == 2 * kGnMaxChunks, "GroupNorm workspace layout");
+
+// GroupNorm stats / apply launch shape, forward and backward: a (chunks, B) grid of `threads`-thread blocks, each block
+// walking rows_per_block of the HW rows.  Enough blocks to fill the machine, but each block walks >= 8 rows per thread.
+struct GnShape {
+  int rows_par, threads, chunks, rows_per_block;
+};
+inline GnShape gn_shape(const Ctx* ctx, int B, int HW, int C) {
+  GnShape g;
+  g.rows_par = gn_rows_par(C);
+  g.threads = C / 8 * g.rows_par;
+  int chunks = (ctx->num_sms * 4 + B - 1) / B;
+  if (chunks > kGnMaxChunks) chunks = kGnMaxChunks;
+  g.rows_per_block = (HW + chunks - 1) / chunks;
+  if (g.rows_per_block < g.rows_par * 8) g.rows_per_block = g.rows_par * 8;
+  g.chunks = (HW + g.rows_per_block - 1) / g.rows_per_block;
+  return g;
 }
 
 }  // namespace sb200

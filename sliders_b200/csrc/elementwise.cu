@@ -363,17 +363,16 @@ using namespace sb200;
 extern "C" int sb200_guided_step_loss(void* handle, void* stream, const float* eps_u, const float* eps_c, float g,
                                       const float* x, float cx, float ce, const float* target, int64_t n, int mode,
                                       float* loss, float* ws, const float* dloss, float* d_eps_u) {
-  pdl_hint() = true;
   SB200_REQUIRE(handle && eps_u && eps_c && x && target && n > 0, "guided_step_loss: NULL argument");
   SB200_REQUIRE(mode == 0 ? (loss && ws) : (mode == 1 && dloss && d_eps_u), "guided_step_loss: mode %d outputs", mode);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int parts = SB200_GUIDED_LOSS_BLOCKS(n);
   const int blocks = mode == 0 ? parts : static_cast<int>((n + kLossThreads - 1) / kLossThreads < 1024
                                                                ? (n + kLossThreads - 1) / kLossThreads : 1024);
-  SB200_CUDA_CHECK(launch_pdl(guided_loss_kernel, dim3(blocks), dim3(kLossThreads), 0, s, eps_u, eps_c, g, x, cx, ce,
+  SB200_CUDA_CHECK(launch_pdl(guided_loss_kernel, dim3(blocks), dim3(kLossThreads), 0, s, true, eps_u, eps_c, g, x, cx, ce,
                               target, n, mode, ws, dloss, d_eps_u));
   if (mode == 0)
-    SB200_CUDA_CHECK(launch_pdl(guided_loss_finalize_kernel, dim3(1), dim3(kLossThreads), 0, s,
+    SB200_CUDA_CHECK(launch_pdl(guided_loss_finalize_kernel, dim3(1), dim3(kLossThreads), 0, s, true,
                                 static_cast<const float*>(ws), parts, n, loss));
   SB200_CUDA_CHECK(cudaGetLastError());
   return 0;
@@ -381,7 +380,6 @@ extern "C" int sb200_guided_step_loss(void* handle, void* stream, const float* e
 
 extern "C" int sb200_sinusoid(void* handle, void* stream, const float* values, int n, int dim, void* out,
                               int ldo) {
-  pdl_hint() = true;
   SB200_REQUIRE(handle && values && out, "sinusoid: NULL argument");
   SB200_REQUIRE(n > 0 && dim > 0 && dim % 2 == 0 && ldo >= dim, "sinusoid: dims");
   const int total = n * (dim / 2);
@@ -394,7 +392,6 @@ extern "C" int sb200_sinusoid(void* handle, void* stream, const float* values, i
 extern "C" int sb200_small_linear(void* handle, void* stream, const void* x, int ldx, const void* w, int ldw,
                                   const void* bias, void* out, int ldo, int M, int N, int K, int act_in,
                                   int act_out, const sb200_lora* lora, const void* resid) {
-  pdl_hint() = true;
   SB200_REQUIRE(handle && x && w && out, "small_linear: NULL argument");
   SB200_REQUIRE(M > 0 && M <= kSlMaxM, "small_linear: M=%d must be in [1, %d]", M, kSlMaxM);
   SB200_REQUIRE(N > 0 && K > 0 && K % 8 == 0 && ldx % 8 == 0 && ldw % 8 == 0, "small_linear: dims");
@@ -429,19 +426,16 @@ extern "C" int sb200_small_linear(void* handle, void* stream, const void* x, int
   }
   const int cols_per_block = kSlWarps * kSlColsPerWarp;
   SB200_CUDA_CHECK(launch_pdl(small_linear_kernel, dim3((N + cols_per_block - 1) / cols_per_block),
-                              dim3(kSlWarps * 32), 0, static_cast<cudaStream_t>(stream), a));
+                              dim3(kSlWarps * 32), 0, static_cast<cudaStream_t>(stream), true, a));
   return 0;
 }
 
 extern "C" int sb200_conv_in(void* handle, void* stream, const void* latent_nchw, int latent_is_f32,
                              const void* w, const void* bias, void* out, int B, int H, int W, int Cout) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && latent_nchw && w && out, "conv_in: NULL argument");
   SB200_REQUIRE(Cout % 8 == 0 && Cout * 36 * 2 <= 48 * 1024, "conv_in: Cout=%d unsupported", Cout);
-  const size_t total = static_cast<size_t>(B) * H * W * (Cout / 8);
-  int blocks = static_cast<int>((total + 255) / 256);
-  if (blocks > ctx->num_sms * 8) blocks = ctx->num_sms * 8;
+  const int blocks = grid_cap(ctx, static_cast<size_t>(B) * H * W * (Cout / 8), 256, 8);
   const size_t smem = static_cast<size_t>(Cout) * 36 * 2;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (latent_is_f32)
@@ -459,13 +453,10 @@ extern "C" int sb200_conv_in(void* handle, void* stream, const void* latent_nchw
 
 extern "C" int sb200_conv_out(void* handle, void* stream, const void* x, const void* w, const void* bias,
                               void* out, int out_is_f32, int B, int H, int W, int Cin) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && x && w && out, "conv_out: NULL argument");
   SB200_REQUIRE(Cin % 8 == 0 && Cin * 36 * 2 <= 48 * 1024, "conv_out: Cin=%d unsupported", Cin);
-  const size_t npix = static_cast<size_t>(B) * H * W;
-  int blocks = static_cast<int>((npix + 7) / 8);
-  if (blocks > ctx->num_sms * 8) blocks = ctx->num_sms * 8;
+  const int blocks = grid_cap(ctx, static_cast<size_t>(B) * H * W, 8, 8);
   const size_t smem = static_cast<size_t>(Cin) * 36 * 2;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (out_is_f32)
@@ -483,13 +474,10 @@ extern "C" int sb200_conv_out(void* handle, void* stream, const void* x, const v
 
 extern "C" int sb200_upsample2x(void* handle, void* stream, const void* x, void* out, int B, int H, int W,
                                 int C) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && x && out, "upsample2x: NULL argument");
   SB200_REQUIRE(C % 8 == 0, "upsample2x: C=%d must be a multiple of 8", C);
-  const size_t total = static_cast<size_t>(B) * 4 * H * W * (C / 8);
-  int blocks = static_cast<int>((total + 255) / 256);
-  if (blocks > ctx->num_sms * 16) blocks = ctx->num_sms * 16;
+  const int blocks = grid_cap(ctx, static_cast<size_t>(B) * 4 * H * W * (C / 8), 256, 16);
   upsample2x_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint4*>(x), static_cast<uint4*>(out), B, H, W, C / 8);
   SB200_CUDA_CHECK(cudaGetLastError());
@@ -513,13 +501,11 @@ extern "C" int sb200_cfg_step(void* handle, void* stream, const void* eps2, int 
 
 static int launch_cfg(void* handle, void* stream, const void* eps2, int eps_is_f32, float g, const void* x,
                       float a_t, float a_prev, void* x_prev, void* eps_out, int out_is_f32, int64_t n, int affine) {
-  pdl_hint() = true;
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && eps2 && n > 0, "cfg_ddim: bad arguments");
   SB200_REQUIRE(x || eps_out, "cfg_ddim: nothing to write");
   SB200_REQUIRE(!x || x_prev, "cfg_ddim: x without x_prev");
-  int blocks = static_cast<int>((n + 255) / 256);
-  if (blocks > ctx->num_sms * 8) blocks = ctx->num_sms * 8;
+  const int blocks = grid_cap(ctx, n, 256, 8);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
 #define SB200_LAUNCH_CFG(TE, TO)                                                                     \
   cfg_ddim_kernel<TE, TO><<<blocks, 256, 0, s>>>(static_cast<const TE*>(eps2), g,                    \
@@ -580,8 +566,7 @@ extern "C" int sb200_lora_compose(void* handle, void* stream, const float* raw, 
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const bool vec = rp % 4 == 0 && (reinterpret_cast<uintptr_t>(raw) | reinterpret_cast<uintptr_t>(eff)) % 16 == 0;
   const int64_t work = vec ? n / 4 : n;
-  int blocks = static_cast<int>((work + 255) / 256);
-  if (blocks > ctx->num_sms * 8) blocks = ctx->num_sms * 8;
+  const int blocks = grid_cap(ctx, work, 256, 8);
   if (vec)
     lora_compose_vec_kernel<<<blocks, 256, 0, s>>>(reinterpret_cast<const float4*>(raw), col_mult,
                                                    reinterpret_cast<float4*>(eff), work, rp / 4);

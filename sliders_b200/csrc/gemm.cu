@@ -991,7 +991,8 @@ static int smem_budget(const Ctx* ctx, int slots) {
 // Launches kKernel, kThreads threads per CTA and built for kSlots CTAs per SM, in clusters of `cluster` CTAs.  Its
 // first launch opts it in to the SM's shared memory and checks with the occupancy calculator that kSlots CTAs fit.
 template <void (*kKernel)(GemmParams), int kThreads, int kSlots>
-static int launch_checked(Ctx* ctx, cudaStream_t stream, const GemmParams& p, dim3 grid, int smem, int cluster) {
+static int launch_checked(Ctx* ctx, cudaStream_t stream, const GemmParams& p, dim3 grid, int smem, int cluster,
+                          bool pdl) {
   static bool checked = false;  // one flag per instantiation
   if (!checked) {
     SB200_CUDA_CHECK(cudaFuncSetAttribute(kKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin));
@@ -1005,35 +1006,36 @@ static int launch_checked(Ctx* ctx, cudaStream_t stream, const GemmParams& p, di
                        p.bn, cluster, p.lora_rt, resident, kSlots);
     checked = true;
   }
-  SB200_CUDA_CHECK(launch_ex(kKernel, grid, dim3(kThreads), smem, stream, cluster, p));
+  SB200_CUDA_CHECK(launch_ex(kKernel, grid, dim3(kThreads), smem, stream, cluster, pdl, p));
   return 0;
 }
 
 // gemm_kernel<BN, kCtas, RT> for the call's RT
 template <int BN, int kCtas>
-static int launch_narrow(Ctx* ctx, cudaStream_t s, const GemmParams& p, int rt, int smem) {
+static int launch_narrow(Ctx* ctx, cudaStream_t s, const GemmParams& p, int rt, int smem, bool pdl) {
   const dim3 grid(p.num_m_tiles * p.num_n_tiles * kCtas, p.sk_ws ? p.sk_splits : 1);
   constexpr int T = kGemmThreads;
   switch (rt) {
-    case 0: return launch_checked<gemm_kernel<BN, kCtas, 0>, T, gemm_slots(BN, 0)>(ctx, s, p, grid, smem, kCtas);
-    case 16: return launch_checked<gemm_kernel<BN, kCtas, 16>, T, gemm_slots(BN, 16)>(ctx, s, p, grid, smem, kCtas);
-    case 32: return launch_checked<gemm_kernel<BN, kCtas, 32>, T, gemm_slots(BN, 32)>(ctx, s, p, grid, smem, kCtas);
-    default: return launch_checked<gemm_kernel<BN, kCtas, 64>, T, gemm_slots(BN, 64)>(ctx, s, p, grid, smem, kCtas);
+    case 0: return launch_checked<gemm_kernel<BN, kCtas, 0>, T, gemm_slots(BN, 0)>(ctx, s, p, grid, smem, kCtas, pdl);
+    case 16: return launch_checked<gemm_kernel<BN, kCtas, 16>, T, gemm_slots(BN, 16)>(ctx, s, p, grid, smem, kCtas, pdl);
+    case 32: return launch_checked<gemm_kernel<BN, kCtas, 32>, T, gemm_slots(BN, 32)>(ctx, s, p, grid, smem, kCtas, pdl);
+    default: return launch_checked<gemm_kernel<BN, kCtas, 64>, T, gemm_slots(BN, 64)>(ctx, s, p, grid, smem, kCtas, pdl);
   }
 }
 
 // gemm_wide_kernel<BN, RT, GEGLU> for the call's RT and epilogue
 template <int BN>
-static int launch_wide(Ctx* ctx, cudaStream_t s, const GemmParams& p, int rt, dim3 grid, int smem) {
+static int launch_wide(Ctx* ctx, cudaStream_t s, const GemmParams& p, int rt, dim3 grid, int smem, bool pdl) {
   constexpr int T = kWideThreads;
-  if (rt == 16) return launch_checked<gemm_wide_kernel<BN, 16, false>, T, 1>(ctx, s, p, grid, smem, 1);
-  if (rt != 0) return launch_checked<gemm_wide_kernel<BN, 32, false>, T, 1>(ctx, s, p, grid, smem, 1);
+  if (rt == 16) return launch_checked<gemm_wide_kernel<BN, 16, false>, T, 1>(ctx, s, p, grid, smem, 1, pdl);
+  if (rt != 0) return launch_checked<gemm_wide_kernel<BN, 32, false>, T, 1>(ctx, s, p, grid, smem, 1, pdl);
   if constexpr (BN == 256)
-    if (p.flags & SB200_EPI_GEGLU) return launch_checked<gemm_wide_kernel<BN, 0, true>, T, 1>(ctx, s, p, grid, smem, 1);
-  return launch_checked<gemm_wide_kernel<BN, 0, false>, T, 1>(ctx, s, p, grid, smem, 1);
+    if (p.flags & SB200_EPI_GEGLU) return launch_checked<gemm_wide_kernel<BN, 0, true>, T, 1>(ctx, s, p, grid, smem, 1, pdl);
+  return launch_checked<gemm_wide_kernel<BN, 0, false>, T, 1>(ctx, s, p, grid, smem, 1, pdl);
 }
 
-static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
+// *pdl receives the launch's PDL choice
+static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas, bool* pdl) {
   // Tile order: N fastest reads each A row-tile from DRAM once and re-reads W once per row-tile, which is free while W
   // stays in L2.  When W is the big operand and does not fit (the batched cross-attention K/V projection: 616 x 2048
   // activations against 629 MB of weights) the M-fastest order streams W once instead.
@@ -1058,9 +1060,10 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
     p.stages = stages;
     p.ring_bytes = stages * p.stage_bytes + epi;
     const int smem = kBarRegion + kAlignSlack + p.ring_bytes;
-    pdl_hint() = p.num_m_tiles * p.num_n_tiles <= 2 * ctx->num_sms;
+    *pdl = pdl_small_grid(ctx, p.num_m_tiles * p.num_n_tiles);
     const dim3 grid(std::min(p.num_m_tiles * p.num_n_tiles, ctx->num_sms));
-    st = p.bn == 160 ? launch_wide<160>(ctx, stream, p, rt, grid, smem) : launch_wide<256>(ctx, stream, p, rt, grid, smem);
+    st = p.bn == 160 ? launch_wide<160>(ctx, stream, p, rt, grid, smem, *pdl)
+                     : launch_wide<256>(ctx, stream, p, rt, grid, smem, *pdl);
   } else {
     const int grid_ctas = p.num_m_tiles * p.num_n_tiles * ctas * (p.sk_ws ? p.sk_splits : 1);
     // A grid that gives each SM at most one CTA lets that CTA have the whole SM's shared memory (a deeper ring).
@@ -1072,11 +1075,13 @@ static int launch_gemm(Ctx* ctx, cudaStream_t stream, GemmParams& p, int ctas) {
     p.ring_bytes = std::max(stages * p.stage_bytes, acc_tile_bytes(p.bn, rt) + kEpiBytes + kEpiWarps * p.up_buf_bytes);
     const int smem = kBarRegion + kAlignSlack + p.ring_bytes;
     if (smem > budget) return set_error(SB200_ERR_INVALID, "gemm: tile does not fit shared memory");
-    pdl_hint() = grid_ctas <= 2 * ctx->num_sms;
+    *pdl = pdl_small_grid(ctx, grid_ctas);
     if (p.bn == 128)
-      st = ctas == 2 ? launch_narrow<128, 2>(ctx, stream, p, rt, smem) : launch_narrow<128, 1>(ctx, stream, p, rt, smem);
+      st = ctas == 2 ? launch_narrow<128, 2>(ctx, stream, p, rt, smem, *pdl)
+                     : launch_narrow<128, 1>(ctx, stream, p, rt, smem, *pdl);
     else
-      st = ctas == 2 ? launch_narrow<64, 2>(ctx, stream, p, rt, smem) : launch_narrow<64, 1>(ctx, stream, p, rt, smem);
+      st = ctas == 2 ? launch_narrow<64, 2>(ctx, stream, p, rt, smem, *pdl)
+                     : launch_narrow<64, 1>(ctx, stream, p, rt, smem, *pdl);
   }
   if (st) return st;
   SB200_CUDA_CHECK(cudaGetLastError());
@@ -1114,10 +1119,11 @@ static int tmap_2d(Ctx* ctx, CUtensorMap* out, const void* ptr, int ld, int k, i
 // The part of a GEMM / conv / split-K launch that does not depend on how A is addressed.  The entry point `who` has
 // filled in the problem (M, N, K, flags, kblocks, num_sub, split-K) and the A operand; this validates the epilogue
 // flags and the LoRA, picks the tile (bn_arg as decode_bn reads it), fills in the tile counts and the epilogue
-// pointers, builds the tensor maps of W ([N, K], row stride ldw) and of the LoRA down-projection, and launches.
+// pointers, builds the tensor maps of W ([N, K], row stride ldw) and of the LoRA down-projection, and launches.  *pdl
+// (when given) receives the launch's PDL choice.
 static int plan_and_launch(Ctx* ctx, cudaStream_t stream, GemmParams& p, const char* who, const void* w, int ldw,
                            const void* bias, const void* rowbias, int rows_per_batch, const void* resid, int ldr,
-                           void* out, int ldo, const sb200_lora* lora, int bn_arg) {
+                           void* out, int ldo, const sb200_lora* lora, int bn_arg, bool* pdl = nullptr) {
   const int flags = p.flags;
   const bool geglu = flags & SB200_EPI_GEGLU;
   const bool has_lora = flags & SB200_EPI_LORA;
@@ -1164,7 +1170,8 @@ static int plan_and_launch(Ctx* ctx, cudaStream_t stream, GemmParams& p, const c
   int st;
   if ((st = tmap_2d(ctx, &p.tmB, w, ldw, p.K, p.N, (geglu || tc.ctas == 2) ? tc.bn / 2 : tc.bn))) return st;
   if (has_lora && (st = tmap_2d(ctx, &p.tmL, lora->down, p.K, p.K, lora->rt, lora->rt / tc.ctas))) return st;
-  return launch_gemm(ctx, stream, p, tc.ctas);
+  bool used_pdl;
+  return launch_gemm(ctx, stream, p, tc.ctas, pdl ? pdl : &used_pdl);
 }
 
 // out[m, n] = sum over s (in order) of ws[s][m][n]; four columns per thread
@@ -1221,12 +1228,13 @@ extern "C" int sb200_gemm_splitk_f32(void* handle, void* stream, const void* x, 
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   // single CTAs on tiles 128 wide where N allows, no epilogue
   const int bn_arg = (N % 128 == 0 ? 128 : 64) | 0x2000;
+  bool pdl;  // the reduction launches as the GEMM did
   if ((st = plan_and_launch(ctx, s, p, "gemm_splitk_f32", w, ldw, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr,
-                            bn_arg)))
+                            bn_arg, &pdl)))
     return st;
   const size_t quads = static_cast<size_t>(M) * N / 4;
   SB200_CUDA_CHECK(launch_pdl(splitk_reduce_kernel, dim3(static_cast<unsigned>((quads + 255) / 256)), dim3(256), 0, s,
-                              static_cast<const float*>(ws), p.sk_splits, M, N, out, ldo));
+                              pdl, static_cast<const float*>(ws), p.sk_splits, M, N, out, ldo));
   SB200_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

@@ -22,8 +22,6 @@ struct GnArgs {
   int rows_per_block;
 };
 
-constexpr int kGnMaxChunks = 128;
-
 // Deterministic (atomic-free) reduction: per-thread partials -> shared memory -> one thread per group sums
 // its channels in a fixed order -> partial[b][chunk][g] in global; gn_finalize_kernel sums the chunks in order.
 __global__ void gn_stats_kernel(GnArgs a, float* __restrict__ partial) {
@@ -283,7 +281,7 @@ extern "C" int sb200_groupnorm(void* handle, void* stream, const void* x0, int l
   SB200_REQUIRE(gn_stats_smem_ok(C), "groupnorm: C=%d too large", C);
   SB200_REQUIRE(stats_ws && gamma && beta, "groupnorm: NULL argument");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  pdl_hint() = static_cast<long long>(B) * HW * C <= (16LL << 20);
+  const bool pdl = static_cast<long long>(B) * HW * C <= (16LL << 20);
   GnArgs a;
   a.x0 = static_cast<const __nv_bfloat16*>(x0);
   a.x1 = static_cast<const __nv_bfloat16*>(x1);
@@ -294,24 +292,14 @@ extern "C" int sb200_groupnorm(void* handle, void* stream, const void* x0, int l
   a.HW = HW;
   a.groups = groups;
   a.cpg = C / groups;
-  const int nvec = C / 8;
-  int rows_par = 512 / nvec;
-  if (rows_par < 1) rows_par = 1;
-  const int threads = nvec * rows_par;
-  // enough blocks to fill the machine, but each block should walk >= 8 rows per thread
-  int chunks = (ctx->num_sms * 4 + B - 1) / B;
-  if (chunks > kGnMaxChunks) chunks = kGnMaxChunks;
-  int rows_per_block = (HW + chunks - 1) / chunks;
-  const int min_rows = rows_par * 8;
-  if (rows_per_block < min_rows) rows_per_block = min_rows;
-  chunks = (HW + rows_per_block - 1) / rows_per_block;
-  a.rows_per_block = rows_per_block;
+  const GnShape g = gn_shape(ctx, B, HW, C);
+  a.rows_per_block = g.rows_per_block;
   // workspace: partial[B][chunks][G][2] followed by final[B][G][2]
-  float* final_stats = stats_ws + static_cast<size_t>(B) * kGnMaxChunks * groups * 2;
-  SB200_CUDA_CHECK(launch_pdl(gn_stats_kernel, dim3(chunks, B), dim3(threads), sizeof(float) * 2 * C * rows_par, s, a,
-                              stats_ws));
-  SB200_CUDA_CHECK(launch_pdl(gn_finalize_kernel, dim3(B), dim3(1024), 0, s, stats_ws, final_stats, chunks, groups,
-                              1.f / (static_cast<float>(HW) * a.cpg), eps));
+  float* final_stats = stats_ws + SB200_GN_STATS_OFFSET(B, groups);
+  SB200_CUDA_CHECK(launch_pdl(gn_stats_kernel, dim3(g.chunks, B), dim3(g.threads), sizeof(float) * 2 * C * g.rows_par,
+                              s, pdl, a, stats_ws));
+  SB200_CUDA_CHECK(launch_pdl(gn_finalize_kernel, dim3(B), dim3(1024), 0, s, pdl, stats_ws, final_stats, g.chunks,
+                              groups, 1.f / (static_cast<float>(HW) * a.cpg), eps));
   GnApplyArgs ap;
   ap.in = a;
   ap.gamma = static_cast<const __nv_bfloat16*>(gamma);
@@ -321,7 +309,7 @@ extern "C" int sb200_groupnorm(void* handle, void* stream, const void* x0, int l
   ap.B = B;
   ap.eps = eps;
   ap.silu = silu;
-  SB200_CUDA_CHECK(launch_pdl(gn_apply_kernel, dim3(chunks, B), dim3(threads), 0, s, ap, final_stats));
+  SB200_CUDA_CHECK(launch_pdl(gn_apply_kernel, dim3(g.chunks, B), dim3(g.threads), 0, s, pdl, ap, final_stats));
   return 0;
 }
 
@@ -332,13 +320,11 @@ extern "C" int sb200_layernorm(void* handle, void* stream, const void* x, int ld
   SB200_REQUIRE(M > 0 && C > 0 && C % 8 == 0 && C <= kLnMaxVec * 256, "layernorm: C=%d unsupported", C);
   SB200_REQUIRE(ldx % 8 == 0 && ldo % 8 == 0, "layernorm: leading dims");
   const int warps = 8;
-  int blocks = (M + warps - 1) / warps;
-  const int max_blocks = ctx->num_sms * 16;
-  if (blocks > max_blocks) blocks = max_blocks;
+  const int blocks = grid_cap(ctx, M, warps, 16);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  pdl_hint() = static_cast<long long>(M) * C <= (8LL << 20);
+  const bool pdl = static_cast<long long>(M) * C <= (8LL << 20);
 #define SB200_LN(NV)                                                                                      \
-  SB200_CUDA_CHECK(launch_pdl(layernorm_kernel<NV>, dim3(blocks), dim3(warps * 32), static_cast<size_t>(C) * 4, st,                 \
+  SB200_CUDA_CHECK(launch_pdl(layernorm_kernel<NV>, dim3(blocks), dim3(warps * 32), static_cast<size_t>(C) * 4, st, pdl, \
                               static_cast<const __nv_bfloat16*>(x), ldx, static_cast<const __nv_bfloat16*>(gamma), \
                               static_cast<const __nv_bfloat16*>(beta), static_cast<__nv_bfloat16*>(out), ldo, M, C, \
                               eps))

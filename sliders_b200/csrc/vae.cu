@@ -245,12 +245,6 @@ __global__ void __launch_bounds__(kSmThreads) softmax_rows_kernel(const float* _
   }
 }
 
-static int grid_for(const Ctx* ctx, size_t items, int per_block, int waves) {
-  size_t blocks = (items + per_block - 1) / per_block;
-  const size_t cap = static_cast<size_t>(ctx->num_sms) * waves;
-  return static_cast<int>(blocks < cap ? blocks : cap);
-}
-
 }  // namespace sb200
 
 using namespace sb200;
@@ -262,7 +256,7 @@ extern "C" int sb200_vae_conv_in_u8(void* handle, void* stream, const uint8_t* i
   SB200_REQUIRE(B > 0 && H > 0 && W > 0, "vae_conv_in_u8: dims %dx%dx%d", B, H, W);
   SB200_REQUIRE(Cout % 8 == 0 && Cout > 0 && Cout * 27 * 2 <= 48 * 1024, "vae_conv_in_u8: Cout=%d unsupported", Cout);
   const size_t smem = static_cast<size_t>(Cout) * 27 * 2;
-  vae_conv_in_u8_kernel<<<grid_for(ctx, static_cast<size_t>(B) * H * W * (Cout / 8), 256, 8), 256, smem,
+  vae_conv_in_u8_kernel<<<grid_cap(ctx, static_cast<size_t>(B) * H * W * (Cout / 8), 256, 8), 256, smem,
                           static_cast<cudaStream_t>(stream)>>>(img, static_cast<const __nv_bfloat16*>(w),
                                                                static_cast<const __nv_bfloat16*>(bias),
                                                                static_cast<__nv_bfloat16*>(out), B, H, W, Cout);
@@ -277,7 +271,7 @@ extern "C" int sb200_vae_conv_out_u8(void* handle, void* stream, const void* x, 
   SB200_REQUIRE(B > 0 && H > 0 && W > 0, "vae_conv_out_u8: dims %dx%dx%d", B, H, W);
   SB200_REQUIRE(Cin % 8 == 0 && Cin > 0 && Cin * 27 * 2 <= 48 * 1024, "vae_conv_out_u8: Cin=%d unsupported", Cin);
   const size_t smem = static_cast<size_t>(Cin) * 27 * 2;
-  vae_conv_out_u8_kernel<<<grid_for(ctx, static_cast<size_t>(B) * H * W, 256 / kOutLanes, 8), 256, smem,
+  vae_conv_out_u8_kernel<<<grid_cap(ctx, static_cast<size_t>(B) * H * W, 256 / kOutLanes, 8), 256, smem,
                            static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(w),
       static_cast<const __nv_bfloat16*>(bias), img, y_f32, B, H, W, Cin);
@@ -297,7 +291,7 @@ extern "C" int sb200_vae_moments(void* handle, void* stream, const void* x, cons
   if (smem > 48 * 1024)
     SB200_CUDA_CHECK(cudaFuncSetAttribute(vae_moments_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           static_cast<int>(smem)));
-  vae_moments_kernel<<<grid_for(ctx, static_cast<size_t>(B) * H * W, 8, 2), 256, smem,
+  vae_moments_kernel<<<grid_cap(ctx, static_cast<size_t>(B) * H * W, 8, 2), 256, smem,
                        static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(w),
       static_cast<const __nv_bfloat16*>(bias), quant_w, quant_b, eps, scaling, z, B, H, W, Cin);
@@ -310,7 +304,7 @@ extern "C" int sb200_vae_post_quant(void* handle, void* stream, const float* z, 
   Ctx* ctx = as_ctx(handle);
   SB200_REQUIRE(ctx && z && post_w && post_b && out, "vae_post_quant: NULL argument");
   SB200_REQUIRE(B > 0 && HW > 0 && scaling != 0.f, "vae_post_quant: B=%d HW=%d scaling=%g", B, HW, scaling);
-  vae_post_quant_kernel<<<grid_for(ctx, static_cast<size_t>(B) * HW, 256, 8), 256, 0,
+  vae_post_quant_kernel<<<grid_cap(ctx, static_cast<size_t>(B) * HW, 256, 8), 256, 0,
                           static_cast<cudaStream_t>(stream)>>>(z, post_w, post_b, scaling, out, B, HW);
   SB200_CUDA_CHECK(cudaGetLastError());
   return 0;

@@ -17,7 +17,6 @@ BF16 = torch.bfloat16
 
 # launches issued through this module since import (bench.py reports it as gpu_launches)
 launch_count = 0
-_KERNELS_PER_CALL = {"groupnorm": 3, "groupnorm_bwd": 3, "lora_wgrad": 2}  # stats + finalize + apply; partial + reduce
 
 
 def _p(t: Optional[torch.Tensor]) -> C.c_void_p:
@@ -37,7 +36,6 @@ def _ctx(t: torch.Tensor):
 # Optional per-call device timing (bench.py's roofline leg): when `profile_log` is a list every wrapper brackets
 # its launch with CUDA events on the launching stream and appends (name, flops, start_event, end_event).
 profile_log = None
-_pending_start = None
 
 
 # Optional call recording (bench.py's per-kernel-class timing): while `record_calls` is a list and the current stream is
@@ -47,20 +45,6 @@ _pending_start = None
 record_calls = None
 
 
-class _Recorder:
-    def __init__(self, lib):
-        self._lib = lib
-
-    def __getattr__(self, name):
-        fn = getattr(self._lib, name)
-
-        def call(*args):
-            record_calls.append([fn, args, None, 0.0])
-            return fn(*args)
-
-        return call
-
-
 def replay_calls(calls) -> None:
     stream = _stream()
     for fn, args, _, _ in calls:
@@ -68,27 +52,34 @@ def replay_calls(calls) -> None:
         _cabi.check(fn(args[0], stream, *args[2:]))
 
 
-def _begin():
-    global _pending_start
+def _call(fn: str, anchor: torch.Tensor, *args, kernels: int = 1, name: str = "other", flops: float = 0.0) -> None:
+    """C-ABI function `fn`(handle of anchor's device, current stream, *args), which enqueues `kernels` launches, with
+    the module's launch count, profiling and call recording."""
+    global launch_count
     if profile_log is not None:
-        _pending_start = torch.cuda.Event(enable_timing=True)
-        _pending_start.record()
-    lib = _cabi.load()
+        start = torch.cuda.Event(enable_timing=True)
+        start.record()
+    f = getattr(_cabi.load(), fn)
+    args = (_ctx(anchor), _stream()) + args
+    entry = None
     if record_calls is not None and torch.cuda.is_current_stream_capturing():
-        return _Recorder(lib)
-    return lib
-
-
-def _count(name: str = "", flops: float = 0.0) -> None:
-    global launch_count, _pending_start
-    launch_count += _KERNELS_PER_CALL.get(name, 1)
-    if record_calls and record_calls[-1][2] is None:
-        record_calls[-1][2], record_calls[-1][3] = name or "other", flops
-    if profile_log is not None and _pending_start is not None:
+        entry = [f, args, None, 0.0]
+        record_calls.append(entry)
+    _cabi.check(f(*args))
+    launch_count += kernels
+    if entry is not None:
+        entry[2], entry[3] = name, flops
+    if profile_log is not None:
         end = torch.cuda.Event(enable_timing=True)
         end.record()
-        profile_log.append((name or "other", flops, _pending_start, end))
-        _pending_start = None
+        profile_log.append((name, flops, start, end))
+
+
+def _epilogue(bias, rowbias, resid, lora, geglu: bool = False) -> int:
+    """The SB200_EPI_* flag word of a `gemm` / `conv3x3` call."""
+    return ((EPI_BIAS if bias is not None else 0) | (EPI_ROWBIAS if rowbias is not None else 0)
+            | (EPI_RESID if resid is not None else 0) | (EPI_GEGLU if geglu else 0)
+            | (EPI_LORA if lora is not None else 0))
 
 
 LORA_MAX_RANK = 16
@@ -143,26 +134,14 @@ def gemm(x: torch.Tensor, w: torch.Tensor, *, bias=None, rowbias=None, rows_per_
     """out[M,N] = epilogue([x | x1] @ w.T): one wgmma `gemm_kernel` launch."""
     M, K0 = x.shape
     N, K = w.shape
-    flags = 0
-    if bias is not None:
-        flags |= EPI_BIAS
-    if rowbias is not None:
-        flags |= EPI_ROWBIAS
-    if resid is not None:
-        flags |= EPI_RESID
-    if geglu:
-        flags |= EPI_GEGLU
-    if lora is not None:
-        flags |= EPI_LORA
+    flags = _epilogue(bias, rowbias, resid, lora, geglu)
     nout = N // 2 if geglu else N
     if out is None:
         out = torch.empty((M, nout), device=x.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_gemm(
-        _ctx(x), _stream(), _p(x), x.stride(0), _p(x1), x1.stride(0) if x1 is not None else 0, K0,
-        _p(w), w.stride(0), _p(out), out.stride(0), M, N, K, flags, _p(bias), _p(rowbias), rows_per_batch,
-        _p(resid), resid.stride(0) if resid is not None else 0, lora.ref(M) if lora is not None else None, bn))
-    _count("gemm", 2.0 * M * N * K)
+    _call("sb200_gemm", x, _p(x), x.stride(0), _p(x1), x1.stride(0) if x1 is not None else 0, K0,
+          _p(w), w.stride(0), _p(out), out.stride(0), M, N, K, flags, _p(bias), _p(rowbias), rows_per_batch,
+          _p(resid), resid.stride(0) if resid is not None else 0, lora.ref(M) if lora is not None else None, bn,
+          name="gemm", flops=2.0 * M * N * K)
     return out
 
 
@@ -176,17 +155,7 @@ def conv3x3(x0: torch.Tensor, w_packed: torch.Tensor, *, x1: Optional[torch.Tens
     B, H, W, C0 = x0.shape
     C1 = x1.shape[-1] if x1 is not None else 0
     Cout = w_packed.shape[0]
-    flags = 0
-    if bias is not None:
-        flags |= EPI_BIAS
-    if rowbias is not None:
-        flags |= EPI_ROWBIAS
-    if resid is not None:
-        flags |= EPI_RESID
-    if lora is not None:
-        flags |= EPI_LORA
-    if pad_bottom_right:
-        flags |= CONV_PAD_BR
+    flags = _epilogue(bias, rowbias, resid, lora) | (CONV_PAD_BR if pad_bottom_right else 0)
     Ho, Wo = H // stride, W // stride
     if out is None:
         out = torch.empty((B, Ho, Wo, Cout), device=x0.device, dtype=BF16)
@@ -194,12 +163,10 @@ def conv3x3(x0: torch.Tensor, w_packed: torch.Tensor, *, x1: Optional[torch.Tens
           or out.stride(0) != Ho * out.stride(1)):
         raise ValueError(f"conv3x3: out {tuple(out.shape)} / strides {out.stride()} is not a [B*Ho*Wo, ldo] matrix "
                          f"of [{B}, {Ho}, {Wo}, {Cout}]")
-    lib = _begin()
-    _cabi.check(lib.sb200_conv3x3(
-        _ctx(x0), _stream(), _p(x0), x0.stride(2), _p(x1), x1.stride(2) if x1 is not None else 0, C0, C1,
-        _p(w_packed), _p(out), out.stride(2), B, H, W, Cout, stride, flags, _p(bias), _p(rowbias), _p(resid),
-        resid.stride(2) if resid is not None else 0, lora.ref(B * Ho * Wo) if lora is not None else None, bn))
-    _count("conv3x3", 2.0 * B * (H // stride) * (W // stride) * Cout * 9 * (C0 + C1))
+    _call("sb200_conv3x3", x0, _p(x0), x0.stride(2), _p(x1), x1.stride(2) if x1 is not None else 0, C0, C1,
+          _p(w_packed), _p(out), out.stride(2), B, H, W, Cout, stride, flags, _p(bias), _p(rowbias), _p(resid),
+          resid.stride(2) if resid is not None else 0, lora.ref(B * Ho * Wo) if lora is not None else None, bn,
+          name="conv3x3", flops=2.0 * B * Ho * Wo * Cout * 9 * (C0 + C1))
     return out
 
 
@@ -217,11 +184,9 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, B: int, heads: 
                             or not lse.is_contiguous()):
         raise ValueError(f"attention: lse {tuple(lse.shape)} {lse.dtype} is not a contiguous fp32 [{B}, {heads}, {Sq}]")
     out = torch.empty((B * Sq, heads * head_dim), device=q.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_attention(_ctx(q), _stream(), _p(q), q.stride(0), _p(k), k.stride(0), _p(v),
-                                    v.stride(0), _p(out), out.stride(0), B, heads, Sq, Skv, int(head_dim),
-                                    float(scale), _p(lse)))
-    _count("attention", 4.0 * B * heads * Sq * Skv * head_dim)
+    _call("sb200_attention", q, _p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(out), out.stride(0),
+          B, heads, Sq, Skv, int(head_dim), float(scale), _p(lse),
+          name="attention", flops=4.0 * B * heads * Sq * Skv * head_dim)
     return out
 
 
@@ -239,12 +204,10 @@ def groupnorm(x0: torch.Tensor, gamma, beta, groups: int, eps: float, silu: bool
         _row_matrix(x1, x1.shape, "groupnorm", "x1")
     out = torch.empty(shp[:-1] + (C0 + C1,), device=x0.device, dtype=BF16)
     if stats_ws is None:
-        stats_ws = torch.empty(B * groups * 2 * 129, device=x0.device, dtype=torch.float32)  # SB200_GN_WS_FLOATS
-    lib = _begin()
-    _cabi.check(lib.sb200_groupnorm(_ctx(x0), _stream(), _p(x0), x0.stride(-2), C0, _p(x1),
-                                    x1.stride(-2) if x1 is not None else 0, C1, _p(gamma), _p(beta), _p(out),
-                                    C0 + C1, B, HW, groups, float(eps), int(silu), _p(stats_ws)))
-    _count("groupnorm")
+        stats_ws = gn_ws(B, groups, x0.device)
+    _call("sb200_groupnorm", x0, _p(x0), x0.stride(-2), C0, _p(x1), x1.stride(-2) if x1 is not None else 0, C1,
+          _p(gamma), _p(beta), _p(out), C0 + C1, B, HW, groups, float(eps), int(silu), _p(stats_ws),
+          kernels=3, name="groupnorm")
     return out
 
 
@@ -252,10 +215,8 @@ def layernorm(x: torch.Tensor, gamma, beta, eps: float = 1e-5) -> torch.Tensor:
     M, Cc = x.shape
     _row_matrix(x, (M, Cc), "layernorm", "x")
     out = torch.empty((M, Cc), device=x.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_layernorm(_ctx(x), _stream(), _p(x), x.stride(0), _p(gamma), _p(beta), _p(out), Cc, M,
-                                    Cc, float(eps)))
-    _count("layernorm")
+    _call("sb200_layernorm", x, _p(x), x.stride(0), _p(gamma), _p(beta), _p(out), Cc, M, Cc, float(eps),
+          name="layernorm")
     return out
 
 
@@ -271,11 +232,8 @@ def small_linear(x: torch.Tensor, w: torch.Tensor, bias=None, *, act_in: bool = 
         raise ValueError(f"small_linear: resid {tuple(resid.shape)} {resid.dtype} / strides {resid.stride()} is not a "
                          f"contiguous [{M}, {N}] bf16 matrix")
     out = torch.empty((M, N), device=x.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_small_linear(_ctx(x), _stream(), _p(x), x.stride(0), _p(w), w.stride(0), _p(bias),
-                                       _p(out), N, M, N, K, int(act_in), int(act_out),
-                                       lora.ref(M) if lora is not None else None, _p(resid)))
-    _count("small_linear")
+    _call("sb200_small_linear", x, _p(x), x.stride(0), _p(w), w.stride(0), _p(bias), _p(out), N, M, N, K,
+          int(act_in), int(act_out), lora.ref(M) if lora is not None else None, _p(resid), name="small_linear")
     return out
 
 
@@ -283,9 +241,7 @@ def sinusoid(values: torch.Tensor, dim: int) -> torch.Tensor:
     """values: fp32 [n] on device -> [n, dim] bf16 ([cos | sin])."""
     n = values.numel()
     out = torch.empty((n, dim), device=values.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_sinusoid(_ctx(values), _stream(), _p(values), n, dim, _p(out), dim))
-    _count("sinusoid")
+    _call("sb200_sinusoid", values, _p(values), n, dim, _p(out), dim, name="sinusoid")
     return out
 
 
@@ -295,10 +251,8 @@ def conv_in(latent: torch.Tensor, w_packed: torch.Tensor, bias) -> torch.Tensor:
     assert Cc == 4 and latent.is_contiguous()
     Cout = w_packed.shape[0]
     out = torch.empty((B, H, W, Cout), device=latent.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_conv_in(_ctx(latent), _stream(), _p(latent), int(latent.dtype == torch.float32),
-                                  _p(w_packed), _p(bias), _p(out), B, H, W, Cout))
-    _count("conv_in")
+    _call("sb200_conv_in", latent, _p(latent), int(latent.dtype == torch.float32), _p(w_packed), _p(bias), _p(out),
+          B, H, W, Cout, name="conv_in")
     return out
 
 
@@ -308,10 +262,8 @@ def conv_out(x: torch.Tensor, w_packed: torch.Tensor, bias, out_dtype=BF16) -> t
     if x.dtype != BF16 or not x.is_contiguous():
         raise ValueError(f"conv_out: x {tuple(x.shape)} {x.dtype} / strides {x.stride()} is not contiguous NHWC bf16")
     out = torch.empty((B, 4, H, W), device=x.device, dtype=out_dtype)
-    lib = _begin()
-    _cabi.check(lib.sb200_conv_out(_ctx(x), _stream(), _p(x), _p(w_packed), _p(bias), _p(out),
-                                   int(out_dtype == torch.float32), B, H, W, Cin))
-    _count("conv_out")
+    _call("sb200_conv_out", x, _p(x), _p(w_packed), _p(bias), _p(out), int(out_dtype == torch.float32), B, H, W, Cin,
+          name="conv_out")
     return out
 
 
@@ -321,9 +273,7 @@ def upsample2x(x: torch.Tensor) -> torch.Tensor:
     if x.dtype != BF16 or not x.is_contiguous():
         raise ValueError(f"upsample2x: x {tuple(x.shape)} {x.dtype} / strides {x.stride()} is not contiguous NHWC bf16")
     out = torch.empty((B, 2 * H, 2 * W, Cc), device=x.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_upsample2x(_ctx(x), _stream(), _p(x), _p(out), B, H, W, Cc))
-    _count("upsample2x")
+    _call("sb200_upsample2x", x, _p(x), _p(out), B, H, W, Cc, name="upsample2x")
     return out
 
 
@@ -340,10 +290,8 @@ def vae_conv_in_u8(img: torch.Tensor, w_packed: torch.Tensor, bias) -> torch.Ten
     B, H, W, _ = _image_shape(img, "vae_conv_in_u8", "img", torch.uint8, 3)
     Cout = w_packed.shape[0]
     out = torch.empty((B, H, W, Cout), device=img.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_vae_conv_in_u8(_ctx(img), _stream(), _p(img), _p(w_packed), _p(bias), _p(out), B, H, W,
-                                         Cout))
-    _count("vae_conv_in_u8", 2.0 * B * H * W * Cout * 27)
+    _call("sb200_vae_conv_in_u8", img, _p(img), _p(w_packed), _p(bias), _p(out), B, H, W, Cout,
+          name="vae_conv_in_u8", flops=2.0 * B * H * W * Cout * 27)
     return out
 
 
@@ -354,10 +302,8 @@ def vae_conv_out_u8(x: torch.Tensor, w_packed: torch.Tensor, bias, return_float:
     B, H, W, Cin = _image_shape(x, "vae_conv_out_u8", "x", BF16)
     img = torch.empty((B, H, W, 3), device=x.device, dtype=torch.uint8)
     y = torch.empty((B, 3, H, W), device=x.device, dtype=torch.float32) if return_float else None
-    lib = _begin()
-    _cabi.check(lib.sb200_vae_conv_out_u8(_ctx(x), _stream(), _p(x), _p(w_packed), _p(bias), _p(img), _p(y), B, H, W,
-                                          Cin))
-    _count("vae_conv_out_u8", 2.0 * B * H * W * 3 * 9 * Cin)
+    _call("sb200_vae_conv_out_u8", x, _p(x), _p(w_packed), _p(bias), _p(img), _p(y), B, H, W, Cin,
+          name="vae_conv_out_u8", flops=2.0 * B * H * W * 3 * 9 * Cin)
     return (img, y) if return_float else img
 
 
@@ -372,10 +318,8 @@ def vae_moments(x: torch.Tensor, w_packed: torch.Tensor, bias, quant_w: torch.Te
     if eps is not None and (tuple(eps.shape) != (B, 4, H, W) or eps.dtype != torch.float32 or not eps.is_contiguous()):
         raise ValueError(f"vae_moments: eps {tuple(eps.shape)} {eps.dtype} is not a contiguous fp32 [{B}, 4, {H}, {W}]")
     z = torch.empty((B, 4, H, W), device=x.device, dtype=torch.float32)
-    lib = _begin()
-    _cabi.check(lib.sb200_vae_moments(_ctx(x), _stream(), _p(x), _p(w_packed), _p(bias), _p(quant_w.contiguous()),
-                                      _p(quant_b.contiguous()), _p(eps), float(scaling), _p(z), B, H, W, Cin))
-    _count("vae_moments", 2.0 * B * H * W * 8 * 9 * Cin)
+    _call("sb200_vae_moments", x, _p(x), _p(w_packed), _p(bias), _p(quant_w.contiguous()), _p(quant_b.contiguous()),
+          _p(eps), float(scaling), _p(z), B, H, W, Cin, name="vae_moments", flops=2.0 * B * H * W * 8 * 9 * Cin)
     return z
 
 
@@ -386,10 +330,8 @@ def vae_post_quant(z: torch.Tensor, post_w: torch.Tensor, post_b: torch.Tensor, 
     if tuple(post_w.shape) != (4, 4) or post_w.dtype != torch.float32 or post_b.dtype != torch.float32:
         raise ValueError("vae_post_quant: post_w / post_b must be fp32 [4, 4] / [4]")
     out = torch.empty_like(z)
-    lib = _begin()
-    _cabi.check(lib.sb200_vae_post_quant(_ctx(z), _stream(), _p(z), _p(post_w.contiguous()), _p(post_b.contiguous()),
-                                         float(scaling), _p(out), z.shape[0], z.shape[2] * z.shape[3]))
-    _count("vae_post_quant")
+    _call("sb200_vae_post_quant", z, _p(z), _p(post_w.contiguous()), _p(post_b.contiguous()), float(scaling), _p(out),
+          z.shape[0], z.shape[2] * z.shape[3], name="vae_post_quant")
     return out
 
 
@@ -398,13 +340,9 @@ def softmax_rows(s: torch.Tensor, scale: float, out: Optional[torch.Tensor] = No
     `softmax_rows_kernel`."""
     rows, cols = s.shape
     _row_matrix(s, (rows, cols), "softmax_rows", "s", dtype=torch.float32)
-    p = _row_matrix_out(out, (rows, cols), "softmax_rows")
-    if p is None:
-        p = torch.empty((rows, cols), device=s.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_softmax_rows(_ctx(s), _stream(), _p(s), s.stride(0), _p(p), p.stride(0), rows, cols,
-                                       float(scale)))
-    _count("softmax_rows")
+    p = _out(out, (rows, cols), "softmax_rows", s.device)
+    _call("sb200_softmax_rows", s, _p(s), s.stride(0), _p(p), p.stride(0), rows, cols, float(scale),
+          name="softmax_rows")
     return p
 
 
@@ -432,12 +370,9 @@ def cfg_ddim(eps2: torch.Tensor, guidance: float, x: Optional[torch.Tensor] = No
     x_prev = torch.empty(shape, device=eps2.device, dtype=out_dtype) if x is not None else None
     if x is not None and x.dtype != out_dtype:
         x = x.to(out_dtype)
-    lib = _begin()
-    fn = lib.sb200_cfg_step if affine else lib.sb200_cfg_ddim
-    _cabi.check(fn(_ctx(eps2), _stream(), _p(eps2), int(eps2.dtype == torch.float32),
-                                   float(guidance), _p(x), float(a_t), float(a_prev), _p(x_prev), _p(eps_out),
-                                   int(out_dtype == torch.float32), n))
-    _count("cfg_ddim")
+    _call("sb200_cfg_step" if affine else "sb200_cfg_ddim", eps2, _p(eps2), int(eps2.dtype == torch.float32),
+          float(guidance), _p(x), float(a_t), float(a_prev), _p(x_prev), _p(eps_out), int(out_dtype == torch.float32), n,
+          name="cfg_ddim")
     return eps_out, x_prev
 
 
@@ -461,15 +396,11 @@ def attention_bwd(q, k, v, o, dout, lse, B: int, heads: int, Sq: int, Skv: int, 
     """dq (and dk, dv) are 2-D (possibly column-sliced) outputs.  `attn_bwd_prep_kernel` + `attention_bwd_kernel`
     (x2 when dk/dv are requested)."""
     dsum = torch.empty(B * heads * Sq, device=q.device, dtype=torch.float32)
-    lib = _begin()
-    _cabi.check(lib.sb200_attention_bwd(
-        _ctx(q), _stream(), _p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(o), o.stride(0),
-        _p(dout), dout.stride(0), _p(lse), _p(dsum), _p(dq), dq.stride(0), _p(dk),
-        dk.stride(0) if dk is not None else 0, _p(dv), dv.stride(0) if dv is not None else 0, B, heads, Sq, Skv,
-        int(head_dim), float(scale)))
-    global launch_count
-    launch_count += 1 if dk is None else 2
-    _count("attention_bwd", (6.0 if dk is None else 14.0) * B * heads * Sq * Skv * head_dim)
+    _call("sb200_attention_bwd", q, _p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(o), o.stride(0),
+          _p(dout), dout.stride(0), _p(lse), _p(dsum), _p(dq), dq.stride(0), _p(dk),
+          dk.stride(0) if dk is not None else 0, _p(dv), dv.stride(0) if dv is not None else 0, B, heads, Sq, Skv,
+          int(head_dim), float(scale), kernels=2 if dk is None else 3, name="attention_bwd",
+          flops=(6.0 if dk is None else 14.0) * B * heads * Sq * Skv * head_dim)
 
 
 def attn_bwd_splits(B: int, heads: int, Sq: int, Skv: int) -> int:
@@ -488,14 +419,10 @@ def attention_bwd_split(q, k, v, o, dout, lse, B: int, heads: int, Sq: int, Skv:
     nsplit = attn_bwd_splits(B, heads, Sq, Skv)
     ws_n = 2 * nsplit * B * Skv * heads * head_dim if nsplit > 1 else 0
     ws = torch.empty(max(ws_n, 1), device=q.device, dtype=torch.float32)
-    lib = _begin()
-    _cabi.check(lib.sb200_attention_bwd_ws(
-        _ctx(q), _stream(), _p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(o), o.stride(0),
-        _p(dout), dout.stride(0), _p(lse), _p(dsum), _p(dq), dq.stride(0), _p(dk), dk.stride(0), _p(dv), dv.stride(0),
-        B, heads, Sq, Skv, int(head_dim), float(scale), _p(ws), ws_n))
-    global launch_count
-    launch_count += 2 if nsplit == 1 else 3
-    _count("attention_bwd", 14.0 * B * heads * Sq * Skv * head_dim)
+    _call("sb200_attention_bwd_ws", q, _p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(o), o.stride(0),
+          _p(dout), dout.stride(0), _p(lse), _p(dsum), _p(dq), dq.stride(0), _p(dk), dk.stride(0), _p(dv), dv.stride(0),
+          B, heads, Sq, Skv, int(head_dim), float(scale), _p(ws), ws_n, kernels=3 if nsplit == 1 else 4,
+          name="attention_bwd", flops=14.0 * B * heads * Sq * Skv * head_dim)
 
 
 def splitk_ws_floats(M: int, N: int, K: int) -> int:
@@ -513,19 +440,13 @@ def gemm_splitk_f32(x: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor
     M, K = x.shape
     N = w.shape[0]
     assert w.shape[1] == K
-    if out is None:
-        out = torch.empty((M, N), device=x.device, dtype=torch.float32)
-    _row_matrix(out, (M, N), "gemm_splitk_f32", dtype=torch.float32)
+    out = _out(out, (M, N), "gemm_splitk_f32", x.device, torch.float32)
     if out.device != x.device:
         raise ValueError(f"gemm_splitk_f32: out is on {out.device}, x on {x.device}")
     n_ws = splitk_ws_floats(M, N, K)
     ws = torch.empty(n_ws, device=x.device, dtype=torch.float32)
-    lib = _begin()
-    _cabi.check(lib.sb200_gemm_splitk_f32(_ctx(x), _stream(), _p(x), x.stride(0), _p(w), w.stride(0), _p(out),
-                                          out.stride(0), M, N, K, _p(ws), n_ws))
-    global launch_count
-    launch_count += 1
-    _count("gemm", 2.0 * M * N * K)
+    _call("sb200_gemm_splitk_f32", x, _p(x), x.stride(0), _p(w), w.stride(0), _p(out), out.stride(0), M, N, K, _p(ws),
+          n_ws, kernels=2, name="gemm", flops=2.0 * M * N * K)
     return out
 
 
@@ -535,22 +456,16 @@ def guided_step_loss_fwd(eps_u, eps_c, g: float, x, cx: float, ce: float, target
     parts = min(256, n // 2048 + 1)  # SB200_GUIDED_LOSS_BLOCKS
     ws = torch.empty(parts, device=eps_u.device, dtype=torch.float32)
     loss = torch.empty((), device=eps_u.device, dtype=torch.float32)
-    lib = _begin()
-    _cabi.check(lib.sb200_guided_step_loss(_ctx(eps_u), _stream(), _p(eps_u), _p(eps_c), float(g), _p(x), float(cx),
-                                           float(ce), _p(target), n, 0, _p(loss), _p(ws), None, None))
-    global launch_count
-    launch_count += 1
-    _count()
+    _call("sb200_guided_step_loss", eps_u, _p(eps_u), _p(eps_c), float(g), _p(x), float(cx), float(ce), _p(target), n,
+          0, _p(loss), _p(ws), None, None, kernels=2)
     return loss
 
 
 def guided_step_loss_bwd(eps_u, eps_c, g: float, x, cx: float, ce: float, target, dloss) -> torch.Tensor:
     """d loss / d eps_u scaled by the device scalar dloss: one `guided_loss_kernel` launch."""
     d = torch.empty_like(eps_u)
-    lib = _begin()
-    _cabi.check(lib.sb200_guided_step_loss(_ctx(eps_u), _stream(), _p(eps_u), _p(eps_c), float(g), _p(x), float(cx),
-                                           float(ce), _p(target), eps_u.numel(), 1, None, None, _p(dloss), _p(d)))
-    _count()
+    _call("sb200_guided_step_loss", eps_u, _p(eps_u), _p(eps_c), float(g), _p(x), float(cx), float(ce), _p(target),
+          eps_u.numel(), 1, None, None, _p(dloss), _p(d))
     return d
 
 
@@ -594,9 +509,11 @@ def _row_matrix(t: torch.Tensor, shape, what: str, name: str = "out", dtype=BF16
     return t
 
 
-def _row_matrix_out(out: Optional[torch.Tensor], shape, what: str, dtype=BF16) -> Optional[torch.Tensor]:
-    """`_row_matrix` for an optional output: None stays None (the caller allocates)."""
-    return None if out is None else _row_matrix(out, shape, what, "out", dtype)
+def _out(out: Optional[torch.Tensor], shape, what: str, device, dtype=BF16) -> torch.Tensor:
+    """An optional output: `out` checked by `_row_matrix`, or a new tensor of the shape when None."""
+    if out is None:
+        return torch.empty(shape, device=device, dtype=dtype)
+    return _row_matrix(out, shape, what, "out", dtype)
 
 
 def groupnorm_bwd(x0, gamma, beta, groups: int, silu: bool, dy, stats_ws, *, x1=None, add=None,
@@ -609,57 +526,39 @@ def groupnorm_bwd(x0, gamma, beta, groups: int, silu: bool, dy, stats_ws, *, x1=
     HW = x0.numel() // (B * C0)
     C1 = x1.shape[-1] if x1 is not None else 0
     Cc = C0 + C1
-    dx = _row_matrix_out(out, shp[:-1] + (Cc,), "groupnorm_bwd")
-    if dx is None:
-        dx = torch.empty(shp[:-1] + (Cc,), device=x0.device, dtype=BF16)
+    dx = _out(out, shp[:-1] + (Cc,), "groupnorm_bwd", x0.device)
     ws = gn_ws(B, groups, x0.device)
     fwd = stats_ws if stats_ws.dim() == 3 else stats_ws[B * groups * 2 * GN_STATS_OFFSET:]
     assert fwd.is_contiguous()
-    lib = _begin()
-    _cabi.check(lib.sb200_groupnorm_bwd(
-        _ctx(x0), _stream(), _p(x0), x0.stride(-2), C0, _p(x1), x1.stride(-2) if x1 is not None else 0, C1,
-        _p(gamma), _p(beta), _p(dy), dy.stride(-2), _p(add), add.stride(-2) if add is not None else 0, _p(dx),
-        dx.stride(-2), B, HW, groups, int(silu), _p(fwd), _p(ws)))
-    _count("groupnorm_bwd")
+    _call("sb200_groupnorm_bwd", x0, _p(x0), x0.stride(-2), C0, _p(x1), x1.stride(-2) if x1 is not None else 0, C1,
+          _p(gamma), _p(beta), _p(dy), dy.stride(-2), _p(add), add.stride(-2) if add is not None else 0, _p(dx),
+          dx.stride(-2), B, HW, groups, int(silu), _p(fwd), _p(ws), kernels=3, name="groupnorm_bwd")
     return dx
 
 
 def layernorm_bwd(x, gamma, dy, eps: float = 1e-5, add=None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """`out`: an [M, C] row-strided matrix (e.g. a column slice of a wider buffer) to write dx into."""
     M, Cc = x.shape
-    dx = _row_matrix_out(out, (M, Cc), "layernorm_bwd")
-    if dx is None:
-        dx = torch.empty((M, Cc), device=x.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_layernorm_bwd(_ctx(x), _stream(), _p(x), x.stride(0), _p(gamma), _p(dy), dy.stride(0),
-                                        _p(add), add.stride(0) if add is not None else 0, _p(dx), dx.stride(0), M,
-                                        Cc, float(eps)))
-    _count()
+    dx = _out(out, (M, Cc), "layernorm_bwd", x.device)
+    _call("sb200_layernorm_bwd", x, _p(x), x.stride(0), _p(gamma), _p(dy), dy.stride(0), _p(add),
+          add.stride(0) if add is not None else 0, _p(dx), dx.stride(0), M, Cc, float(eps))
     return dx
 
 
 def geglu(pre: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """`out`: an [M, F] row-strided matrix to write a * gelu(g) into."""
     M, F2 = pre.shape
-    o = _row_matrix_out(out, (M, F2 // 2), "geglu")
-    if o is None:
-        o = torch.empty((M, F2 // 2), device=pre.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_geglu(_ctx(pre), _stream(), _p(pre), pre.stride(0), _p(o), o.stride(0), M, F2 // 2))
-    _count()
+    o = _out(out, (M, F2 // 2), "geglu", pre.device)
+    _call("sb200_geglu", pre, _p(pre), pre.stride(0), _p(o), o.stride(0), M, F2 // 2)
     return o
 
 
 def geglu_bwd(pre: torch.Tensor, dout: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """`out`: an [M, 2F] row-strided matrix to write [da | dg] into."""
     M, F2 = pre.shape
-    dpre = _row_matrix_out(out, (M, F2), "geglu_bwd")
-    if dpre is None:
-        dpre = torch.empty((M, F2), device=pre.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_geglu_bwd(_ctx(pre), _stream(), _p(pre), pre.stride(0), _p(dout), dout.stride(0),
-                                    _p(dpre), dpre.stride(0), M, F2 // 2))
-    _count()
+    dpre = _out(out, (M, F2), "geglu_bwd", pre.device)
+    _call("sb200_geglu_bwd", pre, _p(pre), pre.stride(0), _p(dout), dout.stride(0), _p(dpre), dpre.stride(0), M,
+          F2 // 2)
     return dpre
 
 
@@ -668,10 +567,8 @@ def add(a: torch.Tensor, b: torch.Tensor, c: Optional[torch.Tensor] = None, out:
     M, Cc = a.shape
     if out is None:
         out = torch.empty((M, Cc), device=a.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_add(_ctx(a), _stream(), _p(a), a.stride(0), _p(b), b.stride(0), _p(c),
-                              c.stride(0) if c is not None else 0, _p(out), out.stride(0), M, Cc))
-    _count()
+    _call("sb200_add", a, _p(a), a.stride(0), _p(b), b.stride(0), _p(c), c.stride(0) if c is not None else 0, _p(out),
+          out.stride(0), M, Cc)
     return out
 
 
@@ -687,27 +584,21 @@ def lora_compose(raw: torch.Tensor, col_mult: torch.Tensor, out: Optional[torch.
         out = torch.empty_like(raw)
     elif out.shape != raw.shape or out.dtype != torch.float32 or not out.is_contiguous():
         raise ValueError("lora_compose: out must be a contiguous fp32 matrix shaped like raw")
-    lib = _begin()
-    _cabi.check(lib.sb200_lora_compose(_ctx(raw), _stream(), _p(raw), _p(col_mult), _p(out), rows, rp))
-    _count("lora_compose")
+    _call("sb200_lora_compose", raw, _p(raw), _p(col_mult), _p(out), rows, rp, name="lora_compose")
     return out
 
 
 def upsample2x_bwd(dy: torch.Tensor) -> torch.Tensor:
     B, H2, W2, Cc = dy.shape
     dx = torch.empty((B, H2 // 2, W2 // 2, Cc), device=dy.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_upsample2x_bwd(_ctx(dy), _stream(), _p(dy), _p(dx), B, H2 // 2, W2 // 2, Cc))
-    _count()
+    _call("sb200_upsample2x_bwd", dy, _p(dy), _p(dx), B, H2 // 2, W2 // 2, Cc)
     return dx
 
 
 def zero_stuff(dy: torch.Tensor) -> torch.Tensor:
     B, Ho, Wo, Cc = dy.shape
     z = torch.empty((B, 2 * Ho, 2 * Wo, Cc), device=dy.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_zero_stuff(_ctx(dy), _stream(), _p(dy), _p(z), B, Ho, Wo, Cc))
-    _count()
+    _call("sb200_zero_stuff", dy, _p(dy), _p(z), B, Ho, Wo, Cc)
     return z
 
 
@@ -717,10 +608,7 @@ def conv_out_bwd(deps: torch.Tensor, w_packed: torch.Tensor) -> torch.Tensor:
     Cc = w_packed.shape[-1]
     deps = deps.contiguous()
     dx = torch.empty((B, H, W, Cc), device=deps.device, dtype=BF16)
-    lib = _begin()
-    _cabi.check(lib.sb200_conv_out_bwd(_ctx(deps), _stream(), _p(deps), int(deps.dtype == torch.float32),
-                                       _p(w_packed), _p(dx), B, H, W, Cc))
-    _count()
+    _call("sb200_conv_out_bwd", deps, _p(deps), int(deps.dtype == torch.float32), _p(w_packed), _p(dx), B, H, W, Cc)
     return dx
 
 
@@ -729,9 +617,7 @@ def colsum(dy: torch.Tensor) -> torch.Tensor:
     B, Cc = dy.shape[0], dy.shape[-1]
     HW = dy.numel() // (B * Cc)
     out = torch.empty((B, Cc), device=dy.device, dtype=torch.float32)
-    lib = _begin()
-    _cabi.check(lib.sb200_colsum(_ctx(dy), _stream(), _p(dy), dy.stride(-2), _p(out), B, HW, Cc))
-    _count()
+    _call("sb200_colsum", dy, _p(dy), dy.stride(-2), _p(out), B, HW, Cc)
     return out
 
 
@@ -747,10 +633,7 @@ def lora_proj(A: torch.Tensor, Bt: torch.Tensor, out: Optional[torch.Tensor] = N
     M, Cc = A.shape
     r = Bt.shape[0]
     T = out if out is not None else torch.empty((M, r), device=A.device, dtype=torch.float32)
-    lib = _begin()
-    _cabi.check(lib.sb200_lora_proj(_ctx(A), _stream(), _p(A), A.stride(0), _p(Bt), Bt.stride(0), _p(T), M, Cc, r,
-                                    int(out is not None)))
-    _count()
+    _call("sb200_lora_proj", A, _p(A), A.stride(0), _p(Bt), Bt.stride(0), _p(T), M, Cc, r, int(out is not None))
     return T
 
 
@@ -762,19 +645,15 @@ def lora_wgrad(A: torch.Tensor, T: torch.Tensor, G: torch.Tensor, transposed: bo
     r = T.shape[1]
     gs_c, gs_r = (G.stride(1), G.stride(0)) if transposed else (G.stride(0), G.stride(1))
     ws = _wgrad_ws(Cc, r, A.device)
-    lib = _begin()
-    _cabi.check(lib.sb200_lora_wgrad(_ctx(A), _stream(), _p(A), A.stride(0), _p(T), _p(G), gs_c, gs_r, float(scale),
-                                     int(accumulate), M, Cc, r, _p(ws)))
-    _count("lora_wgrad")
+    _call("sb200_lora_wgrad", A, _p(A), A.stride(0), _p(T), _p(G), gs_c, gs_r, float(scale), int(accumulate), M, Cc, r,
+          _p(ws), kernels=2, name="lora_wgrad")
 
 
 def lora_rank_update(dX: torch.Tensor, U: torch.Tensor, D: torch.Tensor, scale: float) -> None:
     """dX += scale * U @ D   (dX [M, C] bf16 in place, U [M, r] fp32, D [r, C] bf16)."""
     M, Cc = dX.shape
-    lib = _begin()
-    _cabi.check(lib.sb200_lora_rank_update(_ctx(dX), _stream(), _p(dX), dX.stride(0), _p(U), _p(D), D.stride(0),
-                                           float(scale), M, Cc, U.shape[1]))
-    _count()
+    _call("sb200_lora_rank_update", dX, _p(dX), dX.stride(0), _p(U), _p(D), D.stride(0), float(scale), M, Cc,
+          U.shape[1])
 
 
 def lora_conv_proj(x0: torch.Tensor, D: torch.Tensor, stride: int = 1, x1: Optional[torch.Tensor] = None):
@@ -783,10 +662,8 @@ def lora_conv_proj(x0: torch.Tensor, D: torch.Tensor, stride: int = 1, x1: Optio
     C1 = x1.shape[-1] if x1 is not None else 0
     r = D.shape[0]
     T = torch.empty((B * (H // stride) * (W // stride), r), device=x0.device, dtype=torch.float32)
-    lib = _begin()
-    _cabi.check(lib.sb200_lora_conv_proj(_ctx(x0), _stream(), _p(x0), x0.stride(2), C0, _p(x1),
-                                         x1.stride(2) if x1 is not None else 0, C1, _p(D), _p(T), B, H, W, stride, r))
-    _count()
+    _call("sb200_lora_conv_proj", x0, _p(x0), x0.stride(2), C0, _p(x1), x1.stride(2) if x1 is not None else 0, C1,
+          _p(D), _p(T), B, H, W, stride, r)
     return T
 
 
@@ -797,36 +674,26 @@ def lora_conv_wgrad(x0: torch.Tensor, U: torch.Tensor, G: torch.Tensor, scale: f
     C1 = x1.shape[-1] if x1 is not None else 0
     r = U.shape[1]
     ws = _wgrad_ws(9 * (C0 + C1), r, x0.device)
-    lib = _begin()
-    _cabi.check(lib.sb200_lora_conv_wgrad(_ctx(x0), _stream(), _p(x0), x0.stride(2), C0, _p(x1),
-                                          x1.stride(2) if x1 is not None else 0, C1, _p(U), _p(G), float(scale),
-                                          int(accumulate), B, H, W, stride, r, _p(ws)))
-    _count("lora_wgrad")
+    _call("sb200_lora_conv_wgrad", x0, _p(x0), x0.stride(2), C0, _p(x1), x1.stride(2) if x1 is not None else 0, C1,
+          _p(U), _p(G), float(scale), int(accumulate), B, H, W, stride, r, _p(ws), kernels=2, name="lora_wgrad")
 
 
 def lora_conv_rank_update(dX: torch.Tensor, U: torch.Tensor, D: torch.Tensor, scale: float, stride: int = 1) -> None:
     """dX [B,H,W,C] (contiguous, in place) += scale * conv_transpose(U [B,Ho,Wo,r], D [r,3,3,C])."""
     B, H, W, Cc = dX.shape
     assert dX.is_contiguous()
-    lib = _begin()
-    _cabi.check(lib.sb200_lora_conv_rank_update(_ctx(dX), _stream(), _p(dX), _p(U), _p(D), float(scale), B, H, W, Cc,
-                                                stride, U.shape[1]))
-    _count()
+    _call("sb200_lora_conv_rank_update", dX, _p(dX), _p(U), _p(D), float(scale), B, H, W, Cc, stride, U.shape[1])
 
 
 def adamw(table: torch.Tensor, n_tensors: int, max_numel: int, lr: float, beta1: float, beta2: float, eps: float,
           weight_decay: float, step: int) -> None:
     """One fused `adamw_kernel` launch over a device table of (p, g, m, v, n) records (int64 [n_tensors, 5])."""
-    lib = _begin()
-    _cabi.check(lib.sb200_adamw(_ctx(table), _stream(), _p(table), n_tensors, int(max_numel), float(lr), float(beta1),
-                                float(beta2), float(eps), float(weight_decay), int(step)))
-    _count()
+    _call("sb200_adamw", table, _p(table), n_tensors, int(max_numel), float(lr), float(beta1), float(beta2), float(eps),
+          float(weight_decay), int(step))
 
 
 def adam_f32(table: torch.Tensor, n_tensors: int, max_numel: int, lr: float, beta1: float, beta2: float, eps: float,
              weight_decay: float, step: int) -> None:
     """One `adam_f32_kernel` launch over a device table of fp32 (p, g, m, v, n) records (int64 [n_tensors, 5])."""
-    lib = _begin()
-    _cabi.check(lib.sb200_adam_f32(_ctx(table), _stream(), _p(table), n_tensors, int(max_numel), float(lr),
-                                   float(beta1), float(beta2), float(eps), float(weight_decay), int(step)))
-    _count()
+    _call("sb200_adam_f32", table, _p(table), n_tensors, int(max_numel), float(lr), float(beta1), float(beta2),
+          float(eps), float(weight_decay), int(step))
